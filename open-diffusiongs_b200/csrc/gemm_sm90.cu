@@ -6,7 +6,9 @@
 // accumulators in registers), warp 8 = TMA producer (its warpgroup gives its registers to the consumers).  Operands are staged by TMA into a 128-byte-swizzled
 // shared-memory ring (BK = 64 bf16 = one swizzle row) that runs continuously across the CTA's tiles, so the producer
 // loads the next tile while the consumers run the epilogue of the current one.  Tile = 128 x BN (BN = 256 or 128),
-// wgmma m64nBNk16, one k-block group kept in flight while the next is issued.
+// wgmma m64nBNk16, one k-block group kept in flight while the next is issued.  The inference epilogues stage the
+// finished tile in shared memory and hand it to the TMA unit (a store, or for the in-place residual update a reduce-add
+// in L2), so the consumers go on to the next tile's mainloop while the tile is written out.
 //
 // Fused epilogues = the elementwise tails of the reference DiT block
 // (diffusionGS/models/transformers/utils_transformer.py:270-290, timm Attention/Mlp):
@@ -47,15 +49,15 @@ static EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                   const uint32_t* box) {
+int make_tmap(CUtensorMap* out, CUtensorMapDataType dtype, const void* base, int rank, const uint64_t* dims,
+              const uint64_t* strides_bytes, const uint32_t* box) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) { set_error("cuTensorMapEncodeTiled not available (no CUDA driver?)"); return DGS_ERR_CUDA; }
   cuuint64_t gdim[5], gstr[5];
   cuuint32_t bx[5], es[5];
   for (int i = 0; i < rank; i++) { gdim[i] = dims[i]; bx[i] = box[i]; es[i] = 1; }
   for (int i = 0; i + 1 < rank; i++) gstr[i] = strides_bytes[i];
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx, es,
+  CUresult r = fn(out, dtype, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx, es,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed with CUresult %d", (int)r); return DGS_ERR_CUDA; }
@@ -68,13 +70,20 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
 constexpr int BM = 128, BK = 64;
 constexpr int GEMM_THREADS = WS_THREADS;
 
-template <int BN>
+// OUT_BYTES: element size of the output tile staged in shared memory for the TMA-store epilogue (0: the epilogue
+// writes from registers).  The staging buffer takes what would otherwise be operand stages.
+template <int BN, int OUT_BYTES>
 struct GemmCfg {
-  static constexpr int STAGES = (BN == 256) ? 4 : 6;
+  static constexpr int SMEM_LIMIT = 227 * 1024;
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int OUT_TILE_BYTES = BM * BN * OUT_BYTES;
+  static constexpr int EXTRA = 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int FIT = (SMEM_LIMIT - EXTRA - OUT_TILE_BYTES) / STAGE_BYTES;
+  static constexpr int STAGES = FIT < (BN == 256 ? 4 : 6) ? FIT : (BN == 256 ? 4 : 6);
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + OUT_TILE_BYTES + EXTRA;
+  static_assert(STAGES >= 3 && SMEM_BYTES <= SMEM_LIMIT, "GEMM configuration does not fit in shared memory");
 };
 
 __device__ __forceinline__ float epi_gelu_tanh(float x) {  // nn.GELU(approximate="tanh"), tanh on the MUFU pipe
@@ -135,13 +144,75 @@ __device__ __forceinline__ void epilogue_fragment(const GemmEpilogue& ep, const 
         float* x = reinterpret_cast<float*>(ep.out) + ro + n;
         const float2 r = *reinterpret_cast<const float2*>(ep.resid ? ep.resid + ro + n : x);
         const float2 g = __ldg(reinterpret_cast<const float2*>(gate_row + n));
-        *reinterpret_cast<float2*>(x) = make_float2(fmaf(g.x, v.x, r.x), fmaf(g.y, v.y, r.y));
+        // r + round(g v), not fmaf: the same value as the in-place TMA reduce-add of epilogue_tma
+        *reinterpret_cast<float2*>(x) = make_float2(__fadd_rn(r.x, __fmul_rn(g.x, v.x)), __fadd_rn(r.y, __fmul_rn(g.y, v.y)));
       } else {  // EPI_F32
         float2* o = reinterpret_cast<float2*>(reinterpret_cast<float*>(ep.out) + ro + n);
         if (reduce) atomicAdd(o, v);
         else *o = v;
       }
     }
+  }
+}
+
+// The output element type of the epilogues that stage their tile for a TMA store (see epilogue_tma).
+template <int EPI>
+constexpr int epi_out_bytes() { return (EPI == EPI_GATE_RESID_F32 || EPI == EPI_F32) ? 4 : 2; }
+
+// Epilogue of one warpgroup's 64 x BN fragment through shared memory: the values are computed in registers as in
+// epilogue_fragment, written to this warpgroup's staging buffer, and one thread hands the buffer to the TMA unit, which
+// writes it out while the warpgroup goes on with its next tile's mainloop.  Rows >= M and columns >= N are clipped by
+// the TMA unit.  The staging buffer holds column blocks of 128 bytes (64 bf16 / 32 fp32 columns) x 64 rows, 8 KB each,
+// 128-byte swizzled like the TMA box that stores it: the 16-byte chunk c of row r sits at chunk c ^ (r % 8), which also
+// makes the fragment writes free of bank conflicts.
+// EPI_GATE_RESID_F32 (in place, no ep.resid) stages gate * (acc + b) and adds it into x with a TMA reduce-add, so x is
+// never read by the SM.  The result is x + round(g * v) rather than fmaf(g, v, x): one more fp32 rounding per update.
+template <int EPI, int BN>
+__device__ __forceinline__ void epilogue_tma(const GemmEpilogue& ep, const float (&acc)[BN / 2], uint8_t* stage,
+                                             const CUtensorMap* tmC, int m0, int n0, int M, int N, int wg, int wq, int lane) {
+  constexpr int OB = epi_out_bytes<EPI>();
+  constexpr int COLS = 128 / OB;  // columns per staging row
+  const bool leader = wq == 0 && lane == 0;
+  if (leader) bulk_wait_read<0>();  // the stores of this warpgroup's previous tile have read the buffer
+  named_bar_sync(1 + wg, 128);
+#pragma unroll
+  for (int i = 0; i < 2; i++) {
+    const int r = 16 * wq + (lane >> 2) + 8 * i;  // row in the warpgroup's 64-row slice; r % 8 == lane / 4
+    const float* gate_row = nullptr;
+    if (EPI == EPI_GATE_RESID_F32) {
+      const int row = min(m0 + r, M - 1);  // rows >= M are clipped by the store, but must not index past the gates
+      gate_row = ep.gate + (size_t)(row / ep.rows_per_sample) * ep.gate_stride;
+    }
+#pragma unroll
+    for (int j = 0; j < BN / 8; j++) {
+      const int n = n0 + 8 * j + 2 * (lane & 3);
+      if (n0 + 8 * j >= N) break;  // N % 32 == 0: whole 8-column groups are in or out
+      float2 v = make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+      if (ep.bias) {
+        const float2 b = __ldg(reinterpret_cast<const float2*>(ep.bias + n));
+        v.x += b.x; v.y += b.y;
+      }
+      if (EPI == EPI_BIAS_GELU_BF16) { v.x = epi_gelu_tanh(v.x); v.y = epi_gelu_tanh(v.y); }
+      if (EPI == EPI_GATE_RESID_F32) {
+        const float2 g = __ldg(reinterpret_cast<const float2*>(gate_row + n));
+        v.x *= g.x; v.y *= g.y;
+      }
+      const int byte = ((8 * j) % COLS + 2 * (lane & 3)) * OB;  // within the 128-byte staging row
+      uint8_t* p = stage + (8 * j / COLS) * 8192 + r * 128 + ((((byte >> 4) ^ (lane >> 2)) << 4) | (byte & 15));
+      if (OB == 2) *reinterpret_cast<uint32_t*>(p) = pack2_bf16(v.x, v.y);
+      else *reinterpret_cast<float2*>(p) = v;
+    }
+  }
+  fence_proxy_async();  // make the generic-proxy writes visible to the TMA unit
+  named_bar_sync(1 + wg, 128);
+  if (leader) {
+#pragma unroll
+    for (int b = 0; b < BN / COLS; b++) {
+      if (n0 + b * COLS >= N) break;
+      if (EPI == EPI_GATE_RESID_F32) tma_reduce_add_2d(tmC, stage + b * 8192, n0 + b * COLS, m0);
+      else tma_store_2d(tmC, stage + b * 8192, n0 + b * COLS, m0);
+    }
+    bulk_commit();
   }
 }
 
@@ -152,17 +223,20 @@ __device__ __forceinline__ void epilogue_fragment(const GemmEpilogue& ep, const 
 //              (atom to atom along M/N), SBO = 1024 B (8 K rows), and step 16 K rows = 2048 B per wgmma.
 // splits > 1 (split-K, EPI_F32 only): work unit u = (tile u % num_tiles, K range u / num_tiles); every unit adds its
 // partial product into the (pre-zeroed) output.
-template <int BN, int EPI, bool MN>
+// TMA_EPI: the epilogue goes through shared memory and a TMA store into tmC (epilogue_tma); otherwise it writes from
+// registers (epilogue_fragment) and tmC is unused.
+template <int BN, int EPI, bool MN, bool TMA_EPI>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmEpilogue ep,
-                 int M, int N, int K, int splits) {
-  using Cfg = GemmCfg<BN>;
+gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                 const __grid_constant__ CUtensorMap tmC, GemmEpilogue ep, int M, int N, int K, int splits) {
+  using Cfg = GemmCfg<BN, TMA_EPI ? epi_out_bytes<EPI>() : 0>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
   uint8_t* sA = smem;
   uint8_t* sB = smem + Cfg::STAGES * Cfg::A_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
+  uint8_t* sC = smem + Cfg::STAGES * Cfg::STAGE_BYTES;  // TMA_EPI: one 64 x BN staging buffer per consumer warpgroup
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sC + Cfg::OUT_TILE_BYTES);
   uint64_t* empty_bar = full_bar + Cfg::STAGES;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -241,9 +315,15 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       wg_wait<0>();
       wg_fence_regs(acc);
       if (prev >= 0 && lane == 0) mbar_arrive(empty_bar + prev);
-      const int row0 = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
-      epilogue_fragment<EPI, BN>(ep, acc, row0, n0 + 2 * (lane & 3), M, N, splits > 1);
+      if constexpr (TMA_EPI) {
+        epilogue_tma<EPI, BN>(ep, acc, sC + wg * (Cfg::OUT_TILE_BYTES / 2), &tmC, m0 + wg * 64, n0, M, N, wg, warp & 3,
+                              lane);
+      } else {
+        const int row0 = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+        epilogue_fragment<EPI, BN>(ep, acc, row0, n0 + 2 * (lane & 3), M, N, splits > 1);
+      }
     }
+    if (TMA_EPI && (warp & 3) == 0 && lane == 0) bulk_wait<0>();  // the output is written before the grid completes
   }
 }
 
@@ -260,11 +340,11 @@ static int num_sms() {
   return n;
 }
 
-template <int BN, int EPI, bool MN = false>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmEpilogue& ep, int M, int N, int K,
-                       cudaStream_t st, int splits = 1) {
-  using Cfg = GemmCfg<BN>;
-  auto kern = gemm_bf16_kernel<BN, EPI, MN>;
+template <int BN, int EPI, bool MN, bool TMA_EPI>
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const GemmEpilogue& ep,
+                       int M, int N, int K, cudaStream_t st, int splits = 1) {
+  using Cfg = GemmCfg<BN, TMA_EPI ? epi_out_bytes<EPI>() : 0>;
+  auto kern = gemm_bf16_kernel<BN, EPI, MN, TMA_EPI>;
   static bool configured = false;
   if (!configured) {
     DGS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -274,9 +354,23 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const Gem
   DGS_REQUIRE(sms > 0, "gemm: cannot query the device's SM count");
   const int units = ceil_div(M, BM) * ceil_div(N, BN) * splits;
   const int grid = units < sms ? units : sms;
-  DGS_CUDA_OK(launch_pdl(kern, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, st, tmA, tmB, ep, M, N, K, splits));
+  DGS_CUDA_OK(launch_pdl(kern, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, st, tmA, tmB, tmC, ep, M, N, K, splits));
   DGS_POST_LAUNCH();
   return DGS_OK;
+}
+
+template <int EPI>
+static int launch_epi(bool wide, bool tma_epi, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC,
+                      const GemmEpilogue& ep, int M, int N, int K, cudaStream_t st) {
+  if constexpr (EPI != EPI_DGELU_BF16) {  // dGELU reads the saved pre-activation per element: register epilogue only
+    if (tma_epi) {
+      if constexpr (epi_out_bytes<EPI>() == 2)
+        if (wide) return launch_gemm<256, EPI, false, true>(tmA, tmB, tmC, ep, M, N, K, st);
+      return launch_gemm<128, EPI, false, true>(tmA, tmB, tmC, ep, M, N, K, st);
+    }
+  }
+  return wide ? launch_gemm<256, EPI, false, false>(tmA, tmB, tmC, ep, M, N, K, st)
+              : launch_gemm<128, EPI, false, false>(tmA, tmB, tmC, ep, M, N, K, st);
 }
 
 int gemm_bf16(const void* A, const void* W, int M, int N, int K, int epi, const GemmEpilogue& ep, cudaStream_t st) {
@@ -286,10 +380,22 @@ int gemm_bf16(const void* A, const void* W, int M, int N, int K, int epi, const 
               "gemm: operand row strides must be multiples of 8 elements (K=%d lda=%d ldb=%d)", K, ep.lda, ep.ldb);
   DGS_REQUIRE(epi != EPI_DGELU_BF16 || ep.aux, "gemm: EPI_DGELU_BF16 needs aux = saved pre-activation");
   DGS_REQUIRE(((uintptr_t)A % 16) == 0 && ((uintptr_t)W % 16) == 0, "gemm: operands must be 16-byte aligned");
-  // 128 x 256 tiles when they fill at least one wave of the persistent grid, else 128 x 128 tiles for more CTAs
-  const bool wide = (N % 256 == 0) && (ceil_div(M, BM) * (N / 256) >= num_sms());
+  const int sms = num_sms();
+  DGS_REQUIRE(sms > 0, "gemm: cannot query the device's SM count");
+  // The epilogue stages the tile in shared memory for a TMA store (or, in place, a TMA reduce-add) when the output rows
+  // meet the TMA's 16-byte alignment.  The training variants (aux stores, a separate residual source), dGELU and
+  // unaligned outputs write from registers.
+  const bool out_f32 = epi == EPI_GATE_RESID_F32 || epi == EPI_F32;
+  const int ob = out_f32 ? 4 : 2;
+  const bool tma_epi = epi != EPI_DGELU_BF16 && !ep.aux && !ep.resid && ep.ldc >= N && ((size_t)ep.ldc * ob) % 16 == 0 &&
+                       ((uintptr_t)ep.out % 16) == 0;
+  // 128 x 256 tiles only when every CTA of the persistent grid gets at least two of them, so that each tile's epilogue
+  // drains under the next tile's mainloop; else 128 x 128 tiles.  A staged fp32 tile of 128 x 256 (128 KB) would leave
+  // room for two operand stages only, so staged fp32 outputs always use 128 x 128 tiles.
+  const bool wide = (N % 256 == 0) && (ceil_div(M, BM) * (N / 256) >= 2 * sms) && !(tma_epi && out_f32);
   const int BN = wide ? 256 : 128;
-  CUtensorMap tmA, tmB;
+  CUtensorMap tmA, tmB, tmC;
+  memset(&tmC, 0, sizeof(tmC));
   {
     uint64_t dims[2] = {(uint64_t)K, (uint64_t)M}, str[1] = {(uint64_t)(ep.lda ? ep.lda : K) * 2};
     uint32_t box[2] = {BK, BM};
@@ -302,9 +408,15 @@ int gemm_bf16(const void* A, const void* W, int M, int N, int K, int epi, const 
     int rc = make_tmap_bf16(&tmB, W, 2, dims, str, box);
     if (rc) return rc;
   }
-#define DGS_GEMM_CASE(E)                                                                  \
-  case E:                                                                                 \
-    return wide ? launch_gemm<256, E>(tmA, tmB, ep, M, N, K, st) : launch_gemm<128, E>(tmA, tmB, ep, M, N, K, st);
+  if (tma_epi) {  // one box = one 128-byte column block x the 64 rows of a consumer warpgroup
+    uint64_t dims[2] = {(uint64_t)N, (uint64_t)M}, str[1] = {(uint64_t)ep.ldc * ob};
+    uint32_t box[2] = {(uint32_t)(128 / ob), 64};
+    int rc = make_tmap(&tmC, out_f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, ep.out, 2,
+                       dims, str, box);
+    if (rc) return rc;
+  }
+#define DGS_GEMM_CASE(E) \
+  case E: return launch_epi<E>(wide, tma_epi, tmA, tmB, tmC, ep, M, N, K, st);
   switch (epi) {
     DGS_GEMM_CASE(EPI_BIAS_BF16)
     DGS_GEMM_CASE(EPI_BIAS_GELU_BF16)
@@ -328,7 +440,8 @@ int gemm_bf16_tn(const void* A, const void* W, int M, int N, int K, const GemmEp
   const int sms = num_sms();
   const bool wide = (N % 256 == 0) && (ceil_div(M, BM) * (N / 256) >= sms);
   const int BN = wide ? 256 : 128;
-  CUtensorMap tmA, tmB;
+  CUtensorMap tmA, tmB, tmC;
+  memset(&tmC, 0, sizeof(tmC));  // unused: split-K partial sums are added from registers
   uint32_t box[2] = {64, BK};  // [64 contiguous M/N elements (128 B) x 64 K rows]
   {
     uint64_t dims[2] = {(uint64_t)M, (uint64_t)K}, str[1] = {(uint64_t)lda * 2};
@@ -352,8 +465,8 @@ int gemm_bf16_tn(const void* A, const void* W, int M, int N, int K, const GemmEp
   GemmEpilogue e2 = ep;
   e2.ldc = ldc;
   if (splits > 1) DGS_CUDA_OK(cudaMemset2DAsync(ep.out, (size_t)ldc * 4, 0, (size_t)N * 4, (size_t)M, st));
-  return wide ? launch_gemm<256, EPI_F32, true>(tmA, tmB, e2, M, N, K, st, splits)
-              : launch_gemm<128, EPI_F32, true>(tmA, tmB, e2, M, N, K, st, splits);
+  return wide ? launch_gemm<256, EPI_F32, true, false>(tmA, tmB, tmC, e2, M, N, K, st, splits)
+              : launch_gemm<128, EPI_F32, true, false>(tmA, tmB, tmC, e2, M, N, K, st, splits);
 }
 
 }  // namespace dgs
