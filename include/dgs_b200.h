@@ -303,6 +303,20 @@ typedef struct {
 int dgs_dit_backward_ex(const dgs_dit_weights* w, const dgs_dit_weights_t* wT, const dgs_dit_io* io,
                         const dgs_dit_out_grads* dout, const dgs_dit_grads* grads, const dgs_dit_bwd_opts* opts,
                         void* workspace, size_t workspace_bytes, void* stream);
+/* Introspection used by the per-block parity tests: copies of what a training forward (dgs_dit_forward with
+ * io->train_state) left in the train state for block `layer` into caller DEVICE buffers (any may be NULL).
+ * M = B*N rows, Np = round_up(N, 128):
+ *   x [M, width] fp32: the residual stream entering block `layer` (0 <= layer <= layers; layer == layers is the final
+ *   stream), in both modes.  Recompute mode takes it around the inference block (in-place residual), store mode around
+ *   the training block (separate residual buffers).
+ *   Store mode only, 0 <= layer < layers: x_mid [M, width] fp32 (after the attention branch), h1 / h2 [M, width] bf16
+ *   (LayerNorm + modulate outputs), qkv [M, 3*width] bf16, attn [M, width] bf16, lse [B, heads, Np] fp32 (log2-domain
+ *   log-sum-exp of the scaled scores; pad entries undefined), proj_out / fc2_out [M, width] bf16 (branch outputs + bias,
+ *   before the gate), u_pre / u [M, mlp_hidden] bf16 (fc1 + bias, and its GELU).
+ * An out-of-range layer, or a per-layer tensor requested in recompute mode, is DGS_ERR_INVALID_ARGUMENT. */
+int dgs_dit_export_state(const dgs_dit_weights* w, int B, int V, int H, int W, int train_mode, const void* train_state,
+                         int layer, float* x, float* x_mid, void* h1, void* qkv, void* attn, float* lse, void* proj_out,
+                         void* h2, void* u_pre, void* u, void* fc2_out, void* stream);
 int dgs_event_create(void** event);                 /* cudaEventCreateWithFlags(DisableTiming) */
 int dgs_event_destroy(void* event);
 int dgs_stream_wait_event(void* stream, void* event);

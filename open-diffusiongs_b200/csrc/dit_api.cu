@@ -314,6 +314,44 @@ size_t dgs_dit_train_state_bytes_ex(const dgs_dit_weights* w, int B, int V, int 
   return TrainState(nullptr, w, B, V, H, W, train_mode).bytes;
 }
 
+int dgs_dit_export_state(const dgs_dit_weights* w, int B, int V, int H, int W, int train_mode, const void* train_state,
+                         int layer, float* x, float* x_mid, void* h1, void* qkv, void* attn, float* lse, void* proj_out,
+                         void* h2, void* u_pre, void* u, void* fc2_out, void* stream) {
+  DGS_TRY(check_dit(w, B, V, H, W));
+  DGS_REQUIRE(train_mode == DGS_TRAIN_STORE || train_mode == DGS_TRAIN_RECOMPUTE, "bad train_mode %d", train_mode);
+  DGS_REQUIRE(train_state != nullptr, "train_state is NULL");
+  const int L = w->layers;
+  DGS_REQUIRE(layer >= 0 && layer <= L, "layer %d out of range [0, %d]", layer, L);
+  const bool per_layer = x_mid || h1 || qkv || attn || lse || proj_out || h2 || u_pre || u || fc2_out;
+  DGS_REQUIRE(!per_layer || train_mode == DGS_TRAIN_STORE,
+              "per-layer tensors are kept only in DGS_TRAIN_STORE mode (recompute mode keeps the residual stream alone)");
+  DGS_REQUIRE(!per_layer || layer < L, "per-layer tensors exist for layers [0, %d), not %d", L, layer);
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t T = (size_t)V * (H / w->patch) * (W / w->patch), N = T + w->n_gaussians, D = w->width;
+  const size_t MD = (size_t)B * N * D, MU = (size_t)B * N * w->mlp_hidden;
+  const size_t LS = (size_t)B * w->heads * attention_lse_stride((int)N);
+  TrainState ts(const_cast<void*>(train_state), w, B, V, H, W, train_mode);
+  const size_t l = (size_t)layer;
+  auto copy = [&](void* dst, const void* src, size_t bytes) -> int {
+    if (dst) DGS_CUDA_OK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st));
+    return DGS_OK;
+  };
+  const size_t f4 = sizeof(float), b2 = sizeof(__nv_bfloat16);
+  DGS_TRY(copy(x, ts.x_all + l * MD, MD * f4));
+  if (!per_layer) return DGS_OK;
+  DGS_TRY(copy(x_mid, ts.x_mid + l * MD, MD * f4));
+  DGS_TRY(copy(h1, ts.h1 + l * MD, MD * b2));
+  DGS_TRY(copy(qkv, ts.qkv + l * 3 * MD, 3 * MD * b2));
+  DGS_TRY(copy(attn, ts.attn + l * MD, MD * b2));
+  DGS_TRY(copy(lse, ts.lse + l * LS, LS * f4));
+  DGS_TRY(copy(proj_out, ts.proj_out + l * MD, MD * b2));
+  DGS_TRY(copy(h2, ts.h2 + l * MD, MD * b2));
+  DGS_TRY(copy(u_pre, ts.u_pre + l * MU, MU * b2));
+  DGS_TRY(copy(u, ts.u + l * MU, MU * b2));
+  DGS_TRY(copy(fc2_out, ts.fc2_out + l * MD, MD * b2));
+  return DGS_OK;
+}
+
 int dgs_dit_backward(const dgs_dit_weights* w, const dgs_dit_weights_t* wT, const dgs_dit_io* io,
                      const dgs_dit_out_grads* dout, const dgs_dit_grads* g, void* workspace, size_t workspace_bytes,
                      void* stream) {

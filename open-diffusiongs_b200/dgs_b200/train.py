@@ -163,6 +163,33 @@ class DitTrainer:
             self._state = torch.empty(n, dtype=torch.uint8, device=self.master.device)
         return self._state
 
+    STATE_FIELDS = ("x", "x_mid", "h1", "qkv", "attn", "lse", "proj_out", "h2", "u_pre", "u", "fc2_out")
+
+    def export_state(self, B, V, H, W, layer, names=("x",)):
+        """Copies of block `layer`'s tensors from the last training forward at shape (B, V, H, W) (dgs_dit_export_state):
+        {name: tensor} for `names` out of STATE_FIELDS.  "x" is the residual stream entering the block ([B, N, width]
+        fp32; layer == num_layers: the final stream) in both modes; the others exist in store mode only (not recompute)."""
+        unknown = set(names) - set(self.STATE_FIELDS)
+        if unknown:
+            raise ValueError(f"unknown train-state tensors {sorted(unknown)}; expected a subset of {self.STATE_FIELDS}")
+        if self._state is None:
+            raise RuntimeError("DitTrainer.export_state: no training forward has run")
+        c = self.model.cfg
+        w, _ = self.model.packed_weights()
+        N = c.n_gaussians + V * (H // c.patch_size) * (W // c.patch_size)
+        D, U, heads = c.width, 4 * c.width, c.width // c.dim_heads
+        dev = self.master.device
+        shapes = dict(x=(B, N, D), x_mid=(B, N, D), h1=(B, N, D), qkv=(B, N, 3 * D), attn=(B, N, D),
+                      lse=(B, heads, (N + 127) // 128 * 128), proj_out=(B, N, D), h2=(B, N, D), u_pre=(B, N, U),
+                      u=(B, N, U), fc2_out=(B, N, D))
+        f32 = ("x", "x_mid", "lse")
+        out = {k: torch.empty(shapes[k], dtype=torch.float32 if k in f32 else torch.bfloat16, device=dev) for k in names}
+        args = [out[k].data_ptr() if k in out else None for k in self.STATE_FIELDS]
+        with torch.cuda.device(dev):
+            check(_lib.lib().dgs_dit_export_state(C.byref(w), B, V, H, W, self.train_mode, self._state.data_ptr(), int(layer),
+                                                  *args, _stream(dev)))
+        return out
+
     def zero_grad(self):
         self.arena.zero_()
         if self._accum is not None:

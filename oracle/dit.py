@@ -93,6 +93,97 @@ class _Head(nn.Module):
         return self.linear(modulate(self.layernorm(x), shift, scale))
 
 
+def _bf16(t):
+    return t.to(torch.bfloat16).to(t.dtype)
+
+
+@torch.no_grad()
+def conditioning64(model, t):
+    """c = t_embedder(t) in fp64 (the adaLN input before its SiLU) for any module with the reference's tree."""
+    te = model.t_embedder.mlp
+    half = te[0].weight.shape[1] // 2
+    freqs = torch.exp(-math.log(10000) * torch.arange(half, dtype=torch.float64, device=t.device) / half)
+    args = t[:, None].double() * freqs[None]
+    emb = torch.cat([torch.cos(args), torch.sin(args)], dim=-1)
+    h = F.silu(F.linear(emb, te[0].weight.double(), te[0].bias.double()))
+    return F.linear(h, te[2].weight.double(), te[2].bias.double())
+
+
+@torch.no_grad()
+def block_modulation64(blk, c):
+    """[B, 6*width] fp64: shift_msa | scale_msa | gate_msa | shift_mlp | scale_mlp | gate_mlp of one DiTBlock."""
+    lin = blk.adaLN_modulation[1]
+    return F.linear(F.silu(c.double()), lin.weight.double(), lin.bias.double())
+
+
+@torch.no_grad()
+def dit_block_matched(blk, x, mod, feed=None, rounding=True, softmax_scale=None, head_chunk=None):
+    """One DiTBlock (same arithmetic as DiTBlock.forward) in fp64 from given inputs, rounding to bf16 where the CUDA
+    kernels round: the LayerNorm+modulate outputs h1 / h2, the GEMM weights, the qkv GEMM output, the unnormalised
+    softmax probabilities P (scaled by the row max, normalised after P.V by the fp64 sum of the unrounded ones), the
+    attention output and the GELU output u.  The gated residual updates use the unrounded branch outputs, as the
+    fused GEMM epilogues do.  rounding=False: the plain fp64 block.
+
+    blk: a DiTBlock-shaped module (attn.qkv, attn.proj, mlp.fc1, mlp.fc2; the adaLN linear is not read), x [B, N, w],
+    mod [B, 6w] (block_modulation64).  feed: {name: tensor} replaces this function's own value of that intermediate by
+    the given one before it is used downstream (teacher forcing: each stage is fed the product's previous tensor);
+    keys out of x_mid, h1, qkv, attn, h2, u.  head_chunk: heads per attention pass (bounds the fp64 score memory).
+    Returns every intermediate (fp64): h1, qkv, attn, lse (log2-domain log-sum-exp of the scaled scores, [B, heads, N]),
+    proj_out, x_mid, h2, u_pre, u, fc2_out, x_out."""
+    feed = feed or {}
+    rnd = _bf16 if rounding else (lambda t: t)
+    B, N, D = x.shape
+    heads = blk.attn.num_heads if hasattr(blk.attn, "num_heads") else D // 64
+    hd = D // heads
+    scale = hd ** -0.5 if softmax_scale is None else softmax_scale
+    x = x.double()
+    mod = mod.double()
+    s1, c1, g1, s2, c2, g2 = (m[:, None, :] for m in mod.chunk(6, dim=1))
+    W = lambda lin: rnd(lin.weight.detach().double())  # noqa: E731
+    b = lambda lin: lin.bias.detach().double()  # noqa: E731
+    get = lambda k, v: feed[k].double() if k in feed else v  # noqa: E731
+    out = {}
+
+    def ln(t):
+        mu = t.mean(-1, keepdim=True)
+        var = (t - mu).pow(2).mean(-1, keepdim=True)
+        return (t - mu) / torch.sqrt(var + 1e-6)
+
+    out["h1"] = rnd(ln(x) * (1 + c1) + s1)
+    h1 = get("h1", out["h1"])
+    out["qkv"] = rnd(F.linear(h1, W(blk.attn.qkv), b(blk.attn.qkv)))
+    qkv = get("qkv", out["qkv"]).reshape(B, N, 3, heads, hd).permute(2, 0, 3, 1, 4)  # [3, B, H, N, hd]
+    attn = torch.empty(B, heads, N, hd, dtype=torch.float64, device=x.device)
+    lse = torch.empty(B, heads, N, dtype=torch.float64, device=x.device)
+    step = head_chunk or heads
+    for h0 in range(0, heads, step):
+        q, k, v = (qkv[i, :, h0:h0 + step] for i in range(3))
+        s = (q @ k.transpose(-1, -2)) * scale
+        mx = s.amax(-1, keepdim=True)
+        p = torch.exp(s - mx)
+        den = p.sum(-1, keepdim=True)
+        attn[:, h0:h0 + step] = (rnd(p) @ v) / den
+        lse[:, h0:h0 + step] = (mx + torch.log(den)).squeeze(-1) / math.log(2.0)
+        del s, p
+    out["attn"] = rnd(attn.permute(0, 2, 1, 3).reshape(B, N, D))
+    out["lse"] = lse
+    a = get("attn", out["attn"])
+    proj = F.linear(a, W(blk.attn.proj), b(blk.attn.proj))
+    out["proj_out"] = rnd(proj)
+    out["x_mid"] = x + g1 * proj
+    x_mid = get("x_mid", out["x_mid"])
+    out["h2"] = rnd(ln(x_mid) * (1 + c2) + s2)
+    h2 = get("h2", out["h2"])
+    pre = F.linear(h2, W(blk.mlp.fc1), b(blk.mlp.fc1))
+    out["u_pre"] = rnd(pre)
+    out["u"] = rnd(F.gelu(pre, approximate="tanh"))
+    u = get("u", out["u"])
+    fc2 = F.linear(u, W(blk.mlp.fc2), b(blk.mlp.fc2))
+    out["fc2_out"] = rnd(fc2)
+    out["x_out"] = x_mid + g2 * fc2
+    return out
+
+
 def _init_linear(m):
     if isinstance(m, nn.Linear):
         nn.init.normal_(m.weight, mean=0.0, std=0.02)

@@ -50,3 +50,21 @@ def test_argument_validation_without_gpu():
     assert rc == 1 and b"degree" in L.dgs_last_error()
     assert L.dgs_raster_geom_bytes(1, 1000) > 1000 * 56
     assert L.dgs_raster_image_bytes(1, 256, 256) >= 256 * 256 * 8
+    # DiT train-state read-out: every case fails its argument checks before any copy, so the pointers are never read
+    w = _lib.DitWeights(width=1024, heads=16, layers=2, patch=8, n_gaussians=2, mlp_hidden=4096)
+    fake = ctypes.c_void_p(256)
+
+    def export(mode, layer, state=fake, **bufs):
+        return L.dgs_dit_export_state(ctypes.byref(w), 1, 4, 32, 32, mode, state, layer,
+                                      *[bufs.get(k) for k in ("x", "x_mid", "h1", "qkv", "attn", "lse", "proj_out", "h2",
+                                                              "u_pre", "u", "fc2_out")], None)
+    STORE, RECOMPUTE = _lib.TRAIN_STORE, _lib.TRAIN_RECOMPUTE
+    assert export(STORE, 3, x=fake) == 1 and b"out of range" in L.dgs_last_error()
+    assert export(RECOMPUTE, -1, x=fake) == 1 and b"out of range" in L.dgs_last_error()
+    assert export(RECOMPUTE, 0, h1=fake) == 1 and b"STORE" in L.dgs_last_error()
+    assert export(RECOMPUTE, 1, lse=fake) == 1 and b"STORE" in L.dgs_last_error()
+    assert export(STORE, 2, u=fake) == 1 and b"layers [0, 2)" in L.dgs_last_error()
+    assert export(STORE, 0, state=None, x=fake) == 1 and b"train_state is NULL" in L.dgs_last_error()
+    assert export(7, 0, x=fake) == 1 and b"train_mode" in L.dgs_last_error()
+    w.width = 512
+    assert export(STORE, 0, x=fake) == 1 and b"width" in L.dgs_last_error()

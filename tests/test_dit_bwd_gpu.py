@@ -199,14 +199,19 @@ def test_adamw_matches_torch():
     assert rel(p, ref_p.data) < 1e-6
 
 
-def _grad_compare(layers, B, V, H, W, scene, tag):
+def _grad_compare(layers, B, V, H, W, scene, tag, seed=0, regime=None, sq_errs=None):
+    """-> (whole-gradient rel error, {parameter: rel error}); `regime(model, seed)` rescales the weights first;
+    sq_errs (a dict) receives {parameter: (squared error norm, squared reference norm)}."""
     from dgs_b200.denoiser import DGSDenoiser, DGSDenoiserScene
     from dgs_b200.train import DitTrainer
     from oracle.dit import DenoiserOracle
     from test_dit_gpu import _inputs
-    torch.manual_seed(0)
+    torch.manual_seed(seed)
     cfg = dict(patch_size=8, num_layers=layers, ray_pe_type="plk" if scene else "relative_plk")
-    model = (DGSDenoiserScene if scene else DGSDenoiser)(cfg).to(DEV)
+    model = (DGSDenoiserScene if scene else DGSDenoiser)(cfg)
+    if regime is not None:
+        regime(model, seed)
+    model = model.to(DEV)
     oracle = DenoiserOracle(layers=layers, scene=scene).to(DEV)
     oracle.load_state_dict(model.state_dict(), strict=True)
     trainer = DitTrainer(model)
@@ -229,8 +234,11 @@ def _grad_compare(layers, B, V, H, W, scene, tag):
         gg = ours[name].grad
         assert gg is not None and p.grad is not None, name
         errs[name] = rel(gg, p.grad)
-        num += float((gg.double() - p.grad.double()).pow(2).sum())
-        den += float(p.grad.double().pow(2).sum())
+        n2, d2 = float((gg.double() - p.grad.double()).pow(2).sum()), float(p.grad.double().pow(2).sum())
+        num += n2
+        den += d2
+        if sq_errs is not None:
+            sq_errs[name] = (n2, d2)
     total = (num / den) ** 0.5
     worst = sorted(errs.items(), key=lambda kv: -kv[1])[:6]
     print(f"[{tag}] loss ours={float(loss):.6e} ref={float(ref_loss):.6e}  whole-gradient rel={total:.2e}  worst: " +
