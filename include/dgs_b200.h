@@ -317,6 +317,24 @@ int dgs_dit_backward_ex(const dgs_dit_weights* w, const dgs_dit_weights_t* wT, c
 int dgs_dit_export_state(const dgs_dit_weights* w, int B, int V, int H, int W, int train_mode, const void* train_state,
                          int layer, float* x, float* x_mid, void* h1, void* qkv, void* attn, float* lse, void* proj_out,
                          void* h2, void* u_pre, void* u, void* fc2_out, void* stream);
+/* Introspection used by the end-stage parity tests: copies of the tensors on either side of the blocks into caller
+ * DEVICE buffers (any may be NULL), all fp32.  M = B*N rows, T image tokens per sample, G = n_gaussians.
+ * Left by the last training forward (dgs_dit_forward with io->train_state; c, mod, gs_tok and img_gs by the last
+ * forward that used `workspace`, training or not):
+ *   x_pre [M, width]: the assembled tokens [pos embedding | tokenizer output] before the input LayerNorm;
+ *   c [B, width]: the conditioning t_embedder(t), before the adaLN SiLU;
+ *   mod [B, layers*6*width + 4*width]: the adaLN table (block l at l*6*width; upsampler then decoder shift | scale);
+ *   gs_tok [B*G, 14] and img_gs [B*T, patch*patch*14]: the raw head outputs, before the Gaussian epilogue.
+ * Left by dgs_dit_backward(_ex) on the same train state and workspace (undefined before a backward):
+ *   dx0 [M, width]: the gradient of the residual stream entering block 0 (the input LayerNorm's output);
+ *   dx_pre [M, width]: the gradient of x_pre;
+ *   dmod [B, layers*6*width + 4*width]: the gradient of the adaLN table;
+ *   dc [B, width]: the gradient of c (after the SiLU backward);
+ *   d_gs_tok [B*G, 14]: the gradient of gs_tok.
+ * A NULL train state, a bad mode or a workspace smaller than dgs_dit_workspace_bytes is DGS_ERR_INVALID_ARGUMENT. */
+int dgs_dit_export_ends(const dgs_dit_weights* w, int B, int V, int H, int W, int train_mode, const void* train_state,
+                        const void* workspace, size_t workspace_bytes, float* x_pre, float* c, float* mod, float* gs_tok,
+                        float* img_gs, float* dx0, float* dx_pre, float* dmod, float* dc, float* d_gs_tok, void* stream);
 int dgs_event_create(void** event);                 /* cudaEventCreateWithFlags(DisableTiming) */
 int dgs_event_destroy(void* event);
 int dgs_stream_wait_event(void* stream, void* event);

@@ -352,6 +352,37 @@ int dgs_dit_export_state(const dgs_dit_weights* w, int B, int V, int H, int W, i
   return DGS_OK;
 }
 
+int dgs_dit_export_ends(const dgs_dit_weights* w, int B, int V, int H, int W, int train_mode, const void* train_state,
+                        const void* workspace, size_t workspace_bytes, float* x_pre, float* c, float* mod, float* gs_tok,
+                        float* img_gs, float* dx0, float* dx_pre, float* dmod, float* dc, float* d_gs_tok, void* stream) {
+  DGS_TRY(check_dit(w, B, V, H, W));
+  DGS_REQUIRE(train_mode == DGS_TRAIN_STORE || train_mode == DGS_TRAIN_RECOMPUTE, "bad train_mode %d", train_mode);
+  DGS_REQUIRE(train_state != nullptr, "train_state is NULL");
+  DitWorkspace ws(const_cast<void*>(workspace), w, B, V, H, W);
+  DGS_REQUIRE(workspace && workspace_bytes >= ws.bytes, "workspace too small: %zu < %zu", workspace_bytes, ws.bytes);
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t T = (size_t)V * (H / w->patch) * (W / w->patch), N = T + w->n_gaussians, D = w->width;
+  const size_t MD = (size_t)B * N * D, mod_n = (size_t)B * ((size_t)w->layers * 6 * D + 4 * D);
+  TrainState ts(const_cast<void*>(train_state), w, B, V, H, W, train_mode);
+  auto copy = [&](void* dst, const void* src, size_t n) -> int {
+    if (dst) DGS_CUDA_OK(cudaMemcpyAsync(dst, src, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    return DGS_OK;
+  };
+  // none of these is written again after the pass that produces it: the forward's by the later forward stages, the
+  // backward's by the later backward stages (dx is final once block 0 is differentiated, dcond slice 0 once silu_bwd ran)
+  DGS_TRY(copy(x_pre, ts.x_pre, MD));
+  DGS_TRY(copy(c, ws.c, (size_t)B * D));
+  DGS_TRY(copy(mod, ws.mod, mod_n));
+  DGS_TRY(copy(gs_tok, ws.gs_tok, (size_t)B * w->n_gaussians * 14));
+  DGS_TRY(copy(img_gs, ws.img_gs, (size_t)B * T * w->patch * w->patch * 14));
+  DGS_TRY(copy(dx0, ts.dx, MD));
+  DGS_TRY(copy(dx_pre, ts.dx_pre, MD));
+  DGS_TRY(copy(dmod, ts.dmod, mod_n));
+  DGS_TRY(copy(dc, ts.dcond, (size_t)B * D));
+  DGS_TRY(copy(d_gs_tok, ts.d_gs_tok, (size_t)B * w->n_gaussians * 14));
+  return DGS_OK;
+}
+
 int dgs_dit_backward(const dgs_dit_weights* w, const dgs_dit_weights_t* wT, const dgs_dit_io* io,
                      const dgs_dit_out_grads* dout, const dgs_dit_grads* g, void* workspace, size_t workspace_bytes,
                      void* stream) {

@@ -123,6 +123,7 @@ def lib():
                                           C.POINTER(DitOutGrads), C.POINTER(DitGrads), C.POINTER(DitBwdOpts), vp,
                                           C.c_size_t, vp]
         L.dgs_dit_export_state.argtypes = [C.POINTER(DitWeights)] + [C.c_int] * 5 + [vp, C.c_int] + [vp] * 12
+        L.dgs_dit_export_ends.argtypes = [C.POINTER(DitWeights)] + [C.c_int] * 5 + [vp, vp, C.c_size_t] + [vp] * 11
         L.dgs_event_create.argtypes = [C.POINTER(C.c_void_p)]
         L.dgs_event_destroy.argtypes = [vp]
         L.dgs_stream_wait_event.argtypes = [vp, vp]
@@ -181,4 +182,5 @@ EXPORTED = [  # every symbol include/dgs_b200.h declares (checked by tests/test_
     "dgs_attention_bwd", "dgs_gemm_bf16_ex", "dgs_ln_modulate_bwd", "dgs_gate_bwd", "dgs_cast_transpose_f32", "dgs_gemm_bf16_tn",
     "dgs_dit_train_state_bytes_ex", "dgs_dit_backward_ex", "dgs_event_create", "dgs_event_destroy", "dgs_stream_wait_event",
     "dgs_adamw_ema_step", "dgs_render_batch_forward_mse", "dgs_render_batch_backward_mse", "dgs_dit_export_state",
+    "dgs_dit_export_ends",
 ]

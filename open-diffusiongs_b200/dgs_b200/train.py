@@ -190,6 +190,36 @@ class DitTrainer:
                                                   *args, _stream(dev)))
         return out
 
+    ENDS_FIELDS = ("x_pre", "c", "mod", "gs_tok", "img_gs", "dx0", "dx_pre", "dmod", "dc", "d_gs_tok")
+
+    def export_ends(self, B, V, H, W, names=("x_pre",)):
+        """Copies of the tensors on either side of the blocks (dgs_dit_export_ends), all fp32: {name: tensor} for
+        `names` out of ENDS_FIELDS.  From the last training forward at shape (B, V, H, W): x_pre [B, N, width] (tokens
+        before the input LayerNorm), c [B, width] (conditioning before the adaLN SiLU), mod [B, L*6*width + 4*width]
+        (adaLN table), gs_tok [B, G, 14] and img_gs [B, T, p*p*14] (raw head outputs).  From the backward that
+        followed it (undefined before one): dx0 [B, N, width] (gradient entering block 0), dx_pre, dmod, dc and
+        d_gs_tok, the gradients of x_pre, mod, c and gs_tok."""
+        unknown = set(names) - set(self.ENDS_FIELDS)
+        if unknown:
+            raise ValueError(f"unknown end-stage tensors {sorted(unknown)}; expected a subset of {self.ENDS_FIELDS}")
+        if self._state is None:
+            raise RuntimeError("DitTrainer.export_ends: no training forward has run")
+        c = self.model.cfg
+        w, _ = self.model.packed_weights()
+        p, G, D = c.patch_size, c.n_gaussians, c.width
+        T = V * (H // p) * (W // p)
+        N, R = G + T, c.num_layers * 6 * D + 4 * D
+        shapes = dict(x_pre=(B, N, D), c=(B, D), mod=(B, R), gs_tok=(B, G, 14), img_gs=(B, T, p * p * 14),
+                      dx0=(B, N, D), dx_pre=(B, N, D), dmod=(B, R), dc=(B, D), d_gs_tok=(B, G, 14))
+        dev = self.master.device
+        out = {k: torch.empty(shapes[k], dtype=torch.float32, device=dev) for k in names}
+        args = [out[k].data_ptr() if k in out else None for k in self.ENDS_FIELDS]
+        ws = self.model._workspace
+        with torch.cuda.device(dev):
+            check(_lib.lib().dgs_dit_export_ends(C.byref(w), B, V, H, W, self.train_mode, self._state.data_ptr(),
+                                                 ws.data_ptr(), ws.numel(), *args, _stream(dev)))
+        return out
+
     def zero_grad(self):
         self.arena.zero_()
         if self._accum is not None:

@@ -97,16 +97,29 @@ def _bf16(t):
     return t.to(torch.bfloat16).to(t.dtype)
 
 
+def cond64(model, t, fp32_args=False, defects=()):
+    """c = t_embedder(t) in fp64 (the adaLN input before its SiLU), differentiable in the module's parameters.
+    fp32_args: the timestep argument t * freq is formed in fp32, as the reference (TimestepEmbedder.forward) and the
+    kernel do; at t ~ 1e3 that moves c by ~1e-5 against the fp64 argument.  defects: see END_DEFECTS."""
+    te = model.t_embedder.mlp
+    half = te[0].weight.shape[1] // 2
+    if fp32_args:
+        freqs = torch.exp(-math.log(10000) * torch.arange(half, dtype=torch.float32, device=t.device) / half)
+        args = (t[:, None].float() * freqs[None]).double()
+    else:
+        freqs = torch.exp(-math.log(10000) * torch.arange(half, dtype=torch.float64, device=t.device) / half)
+        args = t[:, None].double() * freqs[None]
+    emb = torch.cat([torch.cos(args), torch.sin(args)], dim=-1)
+    if "cos_sin_swapped" in defects:
+        emb = torch.cat([torch.sin(args), torch.cos(args)], dim=-1)
+    h = F.silu(F.linear(emb, te[0].weight.double(), te[0].bias.double()))
+    return F.linear(h, te[2].weight.double(), te[2].bias.double())
+
+
 @torch.no_grad()
 def conditioning64(model, t):
     """c = t_embedder(t) in fp64 (the adaLN input before its SiLU) for any module with the reference's tree."""
-    te = model.t_embedder.mlp
-    half = te[0].weight.shape[1] // 2
-    freqs = torch.exp(-math.log(10000) * torch.arange(half, dtype=torch.float64, device=t.device) / half)
-    args = t[:, None].double() * freqs[None]
-    emb = torch.cat([torch.cos(args), torch.sin(args)], dim=-1)
-    h = F.silu(F.linear(emb, te[0].weight.double(), te[0].bias.double()))
-    return F.linear(h, te[2].weight.double(), te[2].bias.double())
+    return cond64(model, t)
 
 
 @torch.no_grad()
@@ -181,6 +194,168 @@ def dit_block_matched(blk, x, mod, feed=None, rounding=True, softmax_scale=None,
     fc2 = F.linear(u, W(blk.mlp.fc2), b(blk.mlp.fc2))
     out["fc2_out"] = rnd(fc2)
     out["x_out"] = x_mid + g2 * fc2
+    return out
+
+
+# ---- the stages on either side of the blocks, in fp64 and differentiable (fp64 autograd gives their backward) ----
+# matched=True rounds where the kernels round; plain fp64 otherwise.  `defects` plants a named defect (END_DEFECTS) so
+# that tests/test_dit_ends_power_cpu.py can show the GPU checks would see it; the product path never sets one.
+END_DEFECTS = ("lo_dropped_tokenizer", "lo_dropped_upsampler", "lo_dropped_decoder", "cross_swapped",
+               "clamp_grad_everywhere", "depth_third_dropped", "pos_grad_sample0", "cos_sin_swapped")
+
+
+def _hi_lo(t):
+    hi = _bf16(t)
+    return hi, _bf16(t - hi)
+
+
+class _SplitLinear(torch.autograd.Function):
+    """y = a W^T as the split-bf16 GEMMs compute it: hi(a) hi(W) + lo(a) hi(W) + hi(a) lo(W) (lo(a) lo(W) is the
+    ~2^-18 term they leave out), and its backward as the kernels compute it: the output gradient g rounded to bf16
+    first when g_bf16, da = bf16(g W_d) with W_d = hi(W) if dgrad_hi else W, dW = g^T hi(a) if wgrad_hi else
+    g^T (hi(a) + lo(a)).  drop_lo: the two lo terms left out (a planted defect)."""
+
+    @staticmethod
+    def forward(ctx, a, w, g_bf16, dgrad_hi, wgrad_hi, drop_lo):
+        ah, al = _hi_lo(a)
+        wh, wl = _hi_lo(w)
+        y = ah @ wh.t()
+        if not drop_lo:
+            y = y + al @ wh.t() + ah @ wl.t()
+        ctx.save_for_backward(a, w)
+        ctx.flags = (g_bf16, dgrad_hi, wgrad_hi)
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        a, w = ctx.saved_tensors
+        g_bf16, dgrad_hi, wgrad_hi = ctx.flags
+        g = _bf16(gy) if g_bf16 else gy
+        da = dw = None
+        if ctx.needs_input_grad[0]:
+            da = _bf16(g @ (_bf16(w) if dgrad_hi else w))
+        if ctx.needs_input_grad[1]:
+            ah, al = _hi_lo(a)
+            aw = ah if wgrad_hi else ah + al
+            dw = g.reshape(-1, g.shape[-1]).t() @ aw.reshape(-1, a.shape[-1])
+        return da, dw, None, None, None, None
+
+
+def _linear64(a, w, matched, g_bf16, dgrad_hi, wgrad_hi, drop_lo=False):
+    if matched:
+        return _SplitLinear.apply(a, w.double(), g_bf16, dgrad_hi, wgrad_hi, drop_lo)
+    return F.linear(a, w.double())
+
+
+def _layernorm64(x, w, eps):
+    mu = x.mean(-1, keepdim=True)
+    var = (x - mu).pow(2).mean(-1, keepdim=True)
+    y = (x - mu) / torch.sqrt(var + eps)
+    return y if w is None else y * w.double()
+
+
+def posed_patches64(images, ray_o, ray_d, ray_pe_type, patch, defects=()):
+    """[B, V*(H/p)*(W/p), p*p*9] fp64: the posed image (rgb*2-1 | Pluecker rays) patchified as the tokenizer reads it
+    ("b v c (hh ph) (ww pw) -> b (v hh ww) (ph pw c)")."""
+    images, ray_o, ray_d = images[:, :, :3].double(), ray_o.double(), ray_d.double()
+    if ray_pe_type == "relative_plk":
+        o_dot_d = torch.sum(-ray_o * ray_d, dim=2, keepdim=True)
+        posed = torch.cat([images * 2.0 - 1.0, ray_d, ray_o + o_dot_d * ray_d], dim=2)
+    else:
+        cross = torch.cross(ray_d, ray_o, dim=2) if "cross_swapped" in defects else torch.cross(ray_o, ray_d, dim=2)
+        posed = torch.cat([images * 2.0 - 1.0, cross, ray_d], dim=2)
+    b, v, c, h, w = posed.shape
+    p = patch
+    return posed.reshape(b, v, c, h // p, p, w // p, p).permute(0, 1, 3, 5, 4, 6, 2).reshape(b, -1, p * p * c)
+
+
+def input_stage64(model, images, ray_o, ray_d, ray_pe_type, matched=False, eps=1e-5, patches=None, defects=()):
+    """The input stage: {patches, tok, x_pre = [pos embedding | tok], x0 = LayerNorm(x_pre) * weight} in fp64.
+    matched: the tokenizer product split-bf16 as the kernel computes it, and in the backward the weight gradient
+    bf16(d tok)^T hi(patches).  `patches` replaces posed_patches64's (e.g. the product's)."""
+    if patches is None:
+        p = math.isqrt(model.image_tokenizer[1].weight.shape[1] // 9)
+        patches = posed_patches64(images, ray_o, ray_d, ray_pe_type, p, defects)
+    tok = _linear64(patches, model.image_tokenizer[1].weight, matched, g_bf16=True, dgrad_hi=True, wgrad_hi=True,
+                    drop_lo="lo_dropped_tokenizer" in defects)
+    B, D = tok.shape[0], tok.shape[-1]
+    pos = model.gaussians_pos_embedding.double().reshape(-1, D)
+    pos = pos[None].expand(B, -1, -1)
+    if "pos_grad_sample0" in defects:
+        pos = torch.cat([pos[:1], pos[1:].detach()], dim=0)
+    x_pre = torch.cat([pos, tok], dim=1)
+    x0 = _layernorm64(x_pre, model.transformer_input_layernorm.weight, eps)
+    return dict(patches=patches, tok=tok, x_pre=x_pre, x0=x0)
+
+
+def mod_table64(model, c):
+    """[B, L*6w + 4w] fp64: the adaLN modulation of every block (shift_msa | scale_msa | gate_msa | shift_mlp |
+    scale_mlp | gate_mlp) then of the upsampler and the decoder head (shift | scale each), from c (cond64)."""
+    lins = [blk.adaLN_modulation[1] for blk in model.transformer] + \
+        [model.upsampler.adaLN_modulation[1], model.image_token_decoder.adaLN_modulation[1]]
+    s = F.silu(c.double())
+    return torch.cat([F.linear(s, lin.weight.double(), lin.bias.double()) for lin in lins], dim=1)
+
+
+def gaussians_epilogue64(gs_tok, img_gs, ray_o, ray_d, depth_mode, near=0.0, far=500.0, defects=()):
+    """The raw head outputs -> the renderer-ready Gaussians (denoiser.py:103-120, 362-413; denoiser_scene.py:263,
+    406-410) in fp64.  gs_tok [B, G, 14], img_gs [B, T, p*p*14]; depth_mode 0: (2 sigmoid(m) - 1) * 1.8 + o.(-d)
+    (object model, 'relative_plk'), 1: sigmoid(m) * (far - near) + near (scene model), 2: sigmoid(m) (object model,
+    'plk').  -> {xyz, features, scaling, rotation, opacity, img_aligned_xyz, depth_m (the sigmoid argument m)}."""
+    ray_o, ray_d = ray_o.double(), ray_d.double()
+    b, v, _, h, w = ray_o.shape
+    p = math.isqrt(img_gs.shape[-1] // 14)
+    img_g = img_gs.double().reshape(b, -1, 14)
+    allg = torch.cat((gs_tok.double(), img_g), dim=1)
+    xyz, features, scaling, rotation, opacity = allg.split([3, 3, 3, 4, 1], dim=2)
+    features = features.reshape(b, -1, 1, 3)
+    if "clamp_grad_everywhere" in defects:
+        scaling = scaling - 2.3 + ((scaling - 2.3).clamp(max=-1.20) - (scaling - 2.3)).detach()
+    else:
+        scaling = (scaling - 2.3).clamp(max=-1.20)
+    opacity = opacity - 2.0
+    n_img = img_g.shape[1]
+    ia = xyz[:, -n_img:, :].reshape(b, v, h // p, w // p, p, p, 3).permute(0, 1, 6, 2, 4, 3, 5).reshape(b, v, 3, h, w)
+    m = ia.mean(dim=2, keepdim=True)
+    if "depth_third_dropped" in defects:
+        s = ia.sum(dim=2, keepdim=True)
+        m = s - (s - m).detach()
+    if depth_mode == 1:
+        depth = torch.sigmoid(m) * (far - near) + near
+    elif depth_mode == 0:
+        depth = (2.0 * torch.sigmoid(m) - 1.0) * 1.8 + torch.sum(-ray_o * ray_d, dim=2, keepdim=True)
+    else:
+        depth = torch.sigmoid(m)
+    ia = ray_o + depth * ray_d
+    ia_flat = ia.reshape(b, v, 3, h // p, p, w // p, p).permute(0, 1, 3, 5, 4, 6, 2).reshape(b, -1, 3)
+    xyz = torch.cat((xyz[:, :-n_img, :], ia_flat), dim=1)
+    return dict(xyz=xyz, features=features, scaling=scaling, rotation=rotation, opacity=opacity, img_aligned_xyz=ia,
+                depth_m=m)
+
+
+def heads64(model, x, mod_heads, ray_o, ray_d, depth_mode, near=0.0, far=500.0, matched=False, defects=(), feed=None):
+    """The two heads on the final residual stream x [B, G + T, w] with their modulation mod_heads [B, 4w] (the last
+    4w columns of mod_table64): {gs_tok [B, G, 14], img_gs [B, T, p*p*14], h_ups, h_dec} and every output of
+    gaussians_epilogue64.  matched: the upsampler and decoder products split-bf16 as the kernels compute them; in the
+    backward the decoder's output gradient d_img and both heads' dh rounded to bf16, dh of the decoder through hi(W),
+    and its weight gradient through hi(h).  feed: {"gs_tok" / "img_gs": tensor} -- the epilogue runs on the given raw
+    outputs (e.g. the product's) while the gradient still flows into this function's own heads, so that a raw value
+    within rounding noise of the `scaling` clamp takes the same branch as in the product's backward."""
+    x = x.double()
+    G = model.gaussians_pos_embedding.numel() // x.shape[-1]
+    D = x.shape[-1]
+    mu, md = mod_heads[:, :2 * D].double(), mod_heads[:, 2 * D:].double()
+    ups, dec = model.upsampler, model.image_token_decoder
+    h_ups = modulate(_layernorm64(x[:, :G], ups.layernorm.weight, 1e-5), mu[:, :D], mu[:, D:])
+    h_dec = modulate(_layernorm64(x[:, G:], dec.layernorm.weight, 1e-5), md[:, :D], md[:, D:])
+    gs_tok = _linear64(h_ups, ups.linear.weight, matched, g_bf16=False, dgrad_hi=False, wgrad_hi=False,
+                       drop_lo="lo_dropped_upsampler" in defects)
+    img_gs = _linear64(h_dec, dec.linear.weight, matched, g_bf16=True, dgrad_hi=True, wgrad_hi=True,
+                       drop_lo="lo_dropped_decoder" in defects)
+    feed = feed or {}
+    fed = lambda k, v: v + (feed[k].double() - v).detach() if k in feed else v  # noqa: E731
+    out = gaussians_epilogue64(fed("gs_tok", gs_tok), fed("img_gs", img_gs), ray_o, ray_d, depth_mode, near, far, defects)
+    out.update(gs_tok=gs_tok, img_gs=img_gs, h_ups=h_ups, h_dec=h_dec)
     return out
 
 

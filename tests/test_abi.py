@@ -66,5 +66,18 @@ def test_argument_validation_without_gpu():
     assert export(STORE, 2, u=fake) == 1 and b"layers [0, 2)" in L.dgs_last_error()
     assert export(STORE, 0, state=None, x=fake) == 1 and b"train_state is NULL" in L.dgs_last_error()
     assert export(7, 0, x=fake) == 1 and b"train_mode" in L.dgs_last_error()
+    # end-stage read-out: likewise rejected before any copy
+    ws_bytes = L.dgs_dit_workspace_bytes(ctypes.byref(w), 1, 4, 32, 32)
+    assert ws_bytes > 0
+
+    def ends(mode=STORE, state=fake, ws=fake, nbytes=ws_bytes, **bufs):
+        return L.dgs_dit_export_ends(ctypes.byref(w), 1, 4, 32, 32, mode, state, ws, nbytes,
+                                     *[bufs.get(k) for k in ("x_pre", "c", "mod", "gs_tok", "img_gs", "dx0", "dx_pre",
+                                                             "dmod", "dc", "d_gs_tok")], None)
+    assert ends(state=None, c=fake) == 1 and b"train_state is NULL" in L.dgs_last_error()
+    assert ends(nbytes=ws_bytes - 1, mod=fake) == 1 and b"workspace too small" in L.dgs_last_error()
+    assert ends(ws=None, dx0=fake) == 1 and b"workspace too small" in L.dgs_last_error()
+    assert ends(mode=7, dmod=fake) == 1 and b"train_mode" in L.dgs_last_error()
     w.width = 512
     assert export(STORE, 0, x=fake) == 1 and b"width" in L.dgs_last_error()
+    assert ends(x_pre=fake) == 1 and b"width" in L.dgs_last_error()
