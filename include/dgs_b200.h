@@ -390,6 +390,44 @@ int dgs_ln_modulate(const float* x, const float* ln_w, const float* shift, const
                     void* h, int B, int rows, int width, float eps, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * B2b. LPIPS-VGG perceptual distance, the lpips term of LossComputer (diffusionGS/utils/losses.py:243-309, which calls
+ * lpips.LPIPS(net="vgg") in eval mode): ScalingLayer (x - shift) / scale, torchvision VGG16 features[0:30] (13 conv3x3
+ * + ReLU, 4 max-pools), channel-normalised taps relu1_2 .. relu5_3, 1x1 `lin` weights, spatial mean, sum over taps.
+ * Inputs NCHW fp32 [n, 3, H, W] in [-1, 1]; out [n] fp32.  Activations are bf16, GEMMs accumulate in fp32.
+ * H and W must be multiples of 16 and at least 16, n > 0; anything else is DGS_ERR_INVALID_ARGUMENT.
+ * The images are processed in chunks of as many as the workspace holds (dgs_lpips_workspace_bytes(c, H, W) bytes run
+ * c images at a time; at least c = 1); the results do not depend on the chunking.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+  /* conv l = 0..12 (torchvision features indices 0,2,5,7,10,12,14,17,19,21,24,26,28):
+     conv_w[l]  bf16 [C_out, 9*C_in] with K ordered (ky, kx, c_in); conv1_1's C_in is zero-padded from 3 to 8;
+     conv_wt[l] bf16 [C_in, 9*C_out] = W flipped in both spatial axes and transposed: Wt[ci, (ky, kx, co)] =
+                W[co, ci, 2-ky, 2-kx]; conv1_1's copy has 32 rows, rows 3..31 zero (the input gradient's GEMM);
+     conv_b[l]  fp32 [C_out] */
+  const void* conv_w[13];
+  const void* conv_wt[13];
+  const float* conv_b[13];
+  const float* lin[5];   /* lin{k}.model.1.weight, fp32 [C_k] = 64, 128, 256, 512, 512 */
+  const float* shift;    /* scaling_layer.shift, fp32 [3] */
+  const float* scale;    /* scaling_layer.scale, fp32 [3] */
+} dgs_lpips_weights;
+
+/* Workspace for c images at a time (about 109 MB per image at 256 x 256, most of it the im2col operand). */
+size_t dgs_lpips_workspace_bytes(int n, int H, int W);
+/* Training state for n images: in0's post-ReLU activations of all 13 convolutions in bf16 (35 MB per image at 256 x 256)
+ * and the gradient of the distance w.r.t. in0's activations at the 5 taps in fp32 (32 MB per image).  The second
+ * input's activations are never kept. */
+size_t dgs_lpips_state_bytes(int n, int H, int W);
+/* out[i] = LPIPS(in0[i], in1[i]).  state: NULL for inference, else a buffer of dgs_lpips_state_bytes(n, H, W) that must
+ * stay untouched until dgs_lpips_backward has run.  Inference and training forwards give the same out, bit for bit. */
+int dgs_lpips_forward(const dgs_lpips_weights* w, int n, int H, int W, const float* in0, const float* in1, float* out,
+                      void* state /* NULL = inference */, void* workspace, size_t workspace_bytes, void* stream);
+/* d_in0 [n, 3, H, W] fp32 (overwritten) = dout[i] * d out[i] / d in0[i], dout = device fp32 [n].  The gradient w.r.t. in1
+ * is not computed.  The workspace need not be the forward's. */
+int dgs_lpips_backward(const dgs_lpips_weights* w, int n, int H, int W, const void* state, const float* dout,
+                       float* d_in0, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * B3. The elementwise callers either side of the path.
  * ---------------------------------------------------------------------------------------------- */
 /* TransformInput (diffusionGS/systems/utils.py:621-757, patch_size=None): per-pixel world-space rays.

@@ -7,7 +7,8 @@
 
 namespace dgs {
 
-enum GemmEpi { EPI_BIAS_BF16 = 0, EPI_BIAS_GELU_BF16 = 1, EPI_GATE_RESID_F32 = 2, EPI_F32 = 3, EPI_DGELU_BF16 = 4 };
+enum GemmEpi { EPI_BIAS_BF16 = 0, EPI_BIAS_GELU_BF16 = 1, EPI_GATE_RESID_F32 = 2, EPI_F32 = 3, EPI_DGELU_BF16 = 4,
+               EPI_BIAS_RELU_BF16 = 5 };
 
 struct GemmEpilogue {
   void* out = nullptr;          // bf16 or fp32 [M, ldc]

@@ -17,6 +17,7 @@
 //   EPI_GATE_RESID_F32  x += gate[sample] * (acc + b)       (attn.proj / mlp.fc2 + gate + residual, fp32 stream)
 //   EPI_F32             y = acc (+ b), fp32                 (tokenizer, decoder head, weight gradients)
 //   EPI_DGELU_BF16      y = acc * gelu'(u)                  (backward of mlp.fc2 -> act: u = saved pre-activation)
+//   EPI_BIAS_RELU_BF16  y = max(acc + b, 0)                 (the LPIPS VGG convolutions, lpips.cu)
 // Training mode (GemmEpilogue::aux / resid): fc1 also stores its pre-activation, the gate epilogues also store the
 // pre-gate branch output and may read the residual from a different buffer than they write.
 #include <cstdlib>
@@ -132,8 +133,9 @@ __device__ __forceinline__ void epilogue_fragment(const GemmEpilogue& ep, const 
       }
       if ((EPI == EPI_BIAS_GELU_BF16 || EPI == EPI_GATE_RESID_F32) && ep.aux)  // training: keep acc + b (bf16)
         *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(ep.aux) + ro + n) = pack2_bf16(v.x, v.y);
-      if (EPI == EPI_BIAS_BF16 || EPI == EPI_BIAS_GELU_BF16 || EPI == EPI_DGELU_BF16) {
+      if (EPI == EPI_BIAS_BF16 || EPI == EPI_BIAS_GELU_BF16 || EPI == EPI_DGELU_BF16 || EPI == EPI_BIAS_RELU_BF16) {
         if (EPI == EPI_BIAS_GELU_BF16) { v.x = epi_gelu_tanh(v.x); v.y = epi_gelu_tanh(v.y); }
+        if (EPI == EPI_BIAS_RELU_BF16) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); }
         if (EPI == EPI_DGELU_BF16) {
           const __nv_bfloat162 u = *reinterpret_cast<const __nv_bfloat162*>(reinterpret_cast<const __nv_bfloat16*>(ep.aux) + ro + n);
           const float2 uf = __bfloat1622float2(u);
@@ -193,6 +195,7 @@ __device__ __forceinline__ void epilogue_tma(const GemmEpilogue& ep, const float
         v.x += b.x; v.y += b.y;
       }
       if (EPI == EPI_BIAS_GELU_BF16) { v.x = epi_gelu_tanh(v.x); v.y = epi_gelu_tanh(v.y); }
+      if (EPI == EPI_BIAS_RELU_BF16) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); }
       if (EPI == EPI_GATE_RESID_F32) {
         const float2 g = __ldg(reinterpret_cast<const float2*>(gate_row + n));
         v.x *= g.x; v.y *= g.y;
@@ -423,6 +426,7 @@ int gemm_bf16(const void* A, const void* W, int M, int N, int K, int epi, const 
     DGS_GEMM_CASE(EPI_GATE_RESID_F32)
     DGS_GEMM_CASE(EPI_F32)
     DGS_GEMM_CASE(EPI_DGELU_BF16)
+    DGS_GEMM_CASE(EPI_BIAS_RELU_BF16)
     default:
       set_error("gemm: unknown epilogue %d", epi);
       return DGS_ERR_INVALID_ARGUMENT;

@@ -54,6 +54,11 @@ class RenderMse(C.Structure):  # dgs_render_mse
                 ("images", C.c_void_p)]
 
 
+class LpipsWeights(C.Structure):  # dgs_lpips_weights
+    _fields_ = [("conv_w", C.c_void_p * 13), ("conv_wt", C.c_void_p * 13), ("conv_b", C.c_void_p * 13),
+                ("lin", C.c_void_p * 5), ("shift", C.c_void_p), ("scale", C.c_void_p)]
+
+
 GRAD_FIELDS_A = ("tokenizer_w", "pos_embed", "in_ln_w", "t0_w", "t0_b", "t2_w", "t2_b")
 GRAD_FIELDS_B = ("qkv_w", "qkv_b", "proj_w", "proj_b", "fc1_w", "fc1_b", "fc2_w", "fc2_b", "adaln_w", "adaln_b", "ups_ln_w",
                  "ups_w", "ups_adaln_w", "ups_adaln_b", "dec_ln_w", "dec_w", "dec_adaln_w", "dec_adaln_b")
@@ -147,6 +152,13 @@ def lib():
         L.dgs_rays_from_cameras.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp]
         L.dgs_q_sample.argtypes = [vp, vp, vp, vp, vp, C.c_int, C.c_longlong, vp, vp]
         L.dgs_p_sample_step.argtypes = [vp, vp, vp, vp, vp, vp, vp, C.c_int, C.c_longlong, vp, vp]
+        L.dgs_lpips_workspace_bytes.restype = C.c_size_t
+        L.dgs_lpips_workspace_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
+        L.dgs_lpips_state_bytes.restype = C.c_size_t
+        L.dgs_lpips_state_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
+        L.dgs_lpips_forward.argtypes = [C.POINTER(LpipsWeights), C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp, C.c_size_t,
+                                        vp]
+        L.dgs_lpips_backward.argtypes = [C.POINTER(LpipsWeights), C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, C.c_size_t, vp]
         _lib = L
     return _lib
 
@@ -182,5 +194,5 @@ EXPORTED = [  # every symbol include/dgs_b200.h declares (checked by tests/test_
     "dgs_attention_bwd", "dgs_gemm_bf16_ex", "dgs_ln_modulate_bwd", "dgs_gate_bwd", "dgs_cast_transpose_f32", "dgs_gemm_bf16_tn",
     "dgs_dit_train_state_bytes_ex", "dgs_dit_backward_ex", "dgs_event_create", "dgs_event_destroy", "dgs_stream_wait_event",
     "dgs_adamw_ema_step", "dgs_render_batch_forward_mse", "dgs_render_batch_backward_mse", "dgs_dit_export_state",
-    "dgs_dit_export_ends",
+    "dgs_dit_export_ends", "dgs_lpips_workspace_bytes", "dgs_lpips_state_bytes", "dgs_lpips_forward", "dgs_lpips_backward",
 ]

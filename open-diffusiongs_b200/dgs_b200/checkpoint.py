@@ -18,6 +18,7 @@ import torch
 SYSTEM_PREFIX = "shape_model."           # attribute name of the denoiser inside the reference's systems
 RELEASE_PREFIX = "denoiser."             # original (Adobe) release format
 _LOSS_PREFIXES = ("loss_computer.", "denoiser.loss_computer.")
+LPIPS_PREFIXES = ("loss_computer.lpips_loss_module.", "denoiser.loss_computer.lpips_loss_module.")
 
 
 def extract_denoiser_state_dict(obj):
@@ -49,6 +50,28 @@ def extract_denoiser_state_dict(obj):
     return out, meta, ignored
 
 
+def lpips_state_dict(obj):
+    """-> the frozen LPIPS-VGG weights a checkpoint holds under "loss_computer.lpips_loss_module.*" (Lightning layout, or a
+    bare dict) or "denoiser.loss_computer.lpips_loss_module.*" (release layout), with that prefix removed: the keys of
+    `lpips.LPIPS(net="vgg").state_dict()`.  These are among the keys `extract_denoiser_state_dict` drops; {} when the
+    checkpoint has none."""
+    if isinstance(obj, dict) and "state_dict" in obj and isinstance(obj["state_dict"], dict):
+        sd = obj["state_dict"]
+    elif isinstance(obj, dict) and "model" in obj and isinstance(obj["model"], dict):
+        sd = obj["model"]
+    else:
+        sd = obj
+    if not isinstance(sd, dict):
+        raise ValueError("not a checkpoint: expected a (nested) dict of tensors")
+    out = {}
+    for k, v in sd.items():
+        for p in LPIPS_PREFIXES:
+            if k.startswith(p):
+                out[k[len(p):]] = v
+                break
+    return out
+
+
 def load_checkpoint(model, path_or_obj, strict=True, map_location="cpu"):
     """Load any of the three layouts into a `DGSDenoiser[Scene]`; returns the meta dict (epoch / global_step).
     Tensors are cast to the parameters' dtype (released checkpoints are fp16/bf16, the master weights here are fp32)."""
@@ -71,8 +94,8 @@ def load_checkpoint(model, path_or_obj, strict=True, map_location="cpu"):
 
 def system_checkpoint(model, epoch=0, global_step=0, extra_state_dict=None):
     """The Lightning layout the reference reads: {"state_dict": {"shape_model.<key>": tensor}, "epoch", "global_step"}.
-    `extra_state_dict` (e.g. the frozen LPIPS weights "loss_computer.lpips_loss_module.*", which this repository does not
-    hold) is merged in unchanged when the caller has it."""
+    `extra_state_dict` (e.g. the frozen LPIPS weights, `dgs_b200.lpips.LPIPS.lpips_state_dict(
+    "loss_computer.lpips_loss_module.")`) is merged in unchanged."""
     sd = {SYSTEM_PREFIX + k: v.detach().cpu().clone() for k, v in model.state_dict().items()}
     if extra_state_dict:
         clash = [k for k in extra_state_dict if k in sd]

@@ -7,9 +7,11 @@ What runs where:
   blend-forward kernel and the blend-backward kernel forms dL/dpix = lambda * 2 (c - gt) / n itself
   (dgs_render_batch_forward_mse / _backward_mse).  `LossComputer.forward(..., l2_loss=...)` takes that value; without it
   the l2 term is computed from the images with torch device ops (same numbers, the unfused form).
-* lpips (lambda_lpips = 0.1 in the shipped yamls): LPIPS-VGG16 needs the `lpips` package and its trained weights, neither of
-  which exists offline; it is a bring-your-own nn.Module (`lpips_module(x, y) -> [n,1,1,1]`, inputs in [-1,1] at 256 x 256 as
-  in losses.py:300-303).  Without one the term is zero and `combine` refuses a non-zero lambda_lpips.
+* lpips (lambda_lpips 0.5 from step 151 in diffusionGS_rel.yaml, 0.1 in diffusionGS_scene.yaml): `dgs_b200.lpips.LPIPS`, the
+  LPIPS-VGG16 distance on the library's kernels, with its weights read from the reference's checkpoints
+  (`LPIPS.from_checkpoint(path)`); any module with the `lpips.LPIPS(net="vgg")` call convention (`lpips_module(x, y) ->
+  [n,1,1,1]`, inputs in [-1,1] at 256 x 256 as in losses.py:300-303) may be passed instead.  Without one the term is zero
+  and `combine` refuses a non-zero lambda_lpips.
 * ssim, pointsdist (lambda 0 in every shipped yaml): the reference evaluates them anyway and multiplies by 0; here a
   zero-weight term is skipped unless its module is supplied (ssim) / `compute_pointsdist=True`.
 * l2_xyz: plain device ops (a masked MSE over img_aligned_xyz, losses.py:286-291).
@@ -93,7 +95,8 @@ class LossComputer(nn.Module):
             lam = C(lambdas.get(name.replace("loss_", "lambda_"), 0.0), epoch, global_step)
             if lam != 0.0:
                 if name == "loss_lpips" and self.lpips_loss_module is None:
-                    raise RuntimeError("lambda_lpips != 0 but no LPIPS module was supplied (bring your own: lpips.LPIPS(net='vgg'))")
+                    raise RuntimeError("lambda_lpips != 0 but no LPIPS module was supplied "
+                                       "(e.g. dgs_b200.lpips.LPIPS.from_checkpoint(path))")
                 if name == "loss_ssim" and self.ssim_loss_module is None:
                     raise RuntimeError("lambda_ssim != 0 but no SSIM module was supplied")
                 if name == "loss_pointsdist" and not self.compute_pointsdist:
