@@ -428,6 +428,32 @@ int dgs_lpips_backward(const dgs_lpips_weights* w, int n, int H, int W, const vo
                        float* d_in0, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * B2c. SSIM with an 11-tap Gaussian window (sigma 1.5), C1 = (0.01 R)^2, C2 = (0.03 R)^2, R = data_range, per image
+ * the mean over the 3 channels and the (H-10) x (W-10) valid pixels; optionally PSNR of the images clamped to [0, 1].
+ *   sample_covariance = 0: pytorch_msssim.SSIM(win_size=11, win_sigma=1.5, channel=3), the ssim term of LossComputer
+ *                          (diffusionGS/utils/losses.py:216-234, 314-318);
+ *   sample_covariance = 1: skimage structural_similarity(gaussian_weights=True, win_size=11, channel_axis=0) of
+ *                          MetricComputer.compute_ssim (losses.py:373-473): variances scaled by 121/120.  Its
+ *                          reflect-padded filter is only read inside the valid window, so the value is the same mean.
+ * Images NCHW fp32 [n, 3, H, W]; 0 < n <= 65535, H and W >= 11, data_range > 0, else DGS_ERR_INVALID_ARGUMENT.
+ * No atomics: results do not depend on n or on whether a training state is written, bit for bit.
+ * ---------------------------------------------------------------------------------------------- */
+/* Workspace of one forward: one partial sum pair per (image, 32 x 32 output tile). */
+size_t dgs_ssim_workspace_bytes(int n, int H, int W);
+/* Training state: 3 coefficient maps x 3 channels x (H-10)(W-10) fp32 per image. */
+size_t dgs_ssim_state_bytes(int n, int H, int W);
+/* ssim[i] = SSIM(x[i], y[i]) (device fp32 [n]); psnr[i] = -10 log10(mean (clamp(x) - clamp(y))^2) when psnr != NULL
+ * (+inf for identical images).  state: NULL for inference, else a buffer of dgs_ssim_state_bytes(n, H, W) that must stay
+ * untouched until dgs_ssim_backward has run. */
+int dgs_ssim_forward(int n, int H, int W, const float* x, const float* y, float data_range, int sample_covariance,
+                     float* ssim /* [n] */, float* psnr /* [n] or NULL */, void* state /* NULL = inference */,
+                     void* workspace, size_t workspace_bytes, void* stream);
+/* d_x [n, 3, H, W] fp32 (overwritten) = dout[i] * d ssim[i] / d x[i], dout = device fp32 [n] (the gradient of ssim, not of
+ * 1 - ssim).  x and y are the forward's images.  The gradient w.r.t. y is not computed. */
+int dgs_ssim_backward(int n, int H, int W, const float* x, const float* y, const void* state, const float* dout,
+                      float* d_x, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * B3. The elementwise callers either side of the path.
  * ---------------------------------------------------------------------------------------------- */
 /* TransformInput (diffusionGS/systems/utils.py:621-757, patch_size=None): per-pixel world-space rays.

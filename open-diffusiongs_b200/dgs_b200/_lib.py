@@ -159,6 +159,13 @@ def lib():
         L.dgs_lpips_forward.argtypes = [C.POINTER(LpipsWeights), C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp, C.c_size_t,
                                         vp]
         L.dgs_lpips_backward.argtypes = [C.POINTER(LpipsWeights), C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, C.c_size_t, vp]
+        L.dgs_ssim_workspace_bytes.restype = C.c_size_t
+        L.dgs_ssim_workspace_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
+        L.dgs_ssim_state_bytes.restype = C.c_size_t
+        L.dgs_ssim_state_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
+        L.dgs_ssim_forward.argtypes = [C.c_int, C.c_int, C.c_int, vp, vp, C.c_float, C.c_int, vp, vp, vp, vp, C.c_size_t,
+                                       vp]
+        L.dgs_ssim_backward.argtypes = [C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]
         _lib = L
     return _lib
 
@@ -195,4 +202,5 @@ EXPORTED = [  # every symbol include/dgs_b200.h declares (checked by tests/test_
     "dgs_dit_train_state_bytes_ex", "dgs_dit_backward_ex", "dgs_event_create", "dgs_event_destroy", "dgs_stream_wait_event",
     "dgs_adamw_ema_step", "dgs_render_batch_forward_mse", "dgs_render_batch_backward_mse", "dgs_dit_export_state",
     "dgs_dit_export_ends", "dgs_lpips_workspace_bytes", "dgs_lpips_state_bytes", "dgs_lpips_forward", "dgs_lpips_backward",
+    "dgs_ssim_workspace_bytes", "dgs_ssim_state_bytes", "dgs_ssim_forward", "dgs_ssim_backward",
 ]

@@ -12,8 +12,11 @@ What runs where:
   (`LPIPS.from_checkpoint(path)`); any module with the `lpips.LPIPS(net="vgg")` call convention (`lpips_module(x, y) ->
   [n,1,1,1]`, inputs in [-1,1] at 256 x 256 as in losses.py:300-303) may be passed instead.  Without one the term is zero
   and `combine` refuses a non-zero lambda_lpips.
-* ssim, pointsdist (lambda 0 in every shipped yaml): the reference evaluates them anyway and multiplies by 0; here a
-  zero-weight term is skipped unless its module is supplied (ssim) / `compute_pointsdist=True`.
+* ssim: `dgs_b200.ssim.SsimLoss`, the reference's 1 - pytorch_msssim.SSIM(win_size=11, win_sigma=1.5) on the library's
+  kernels (`LossComputer(ssim_module=SsimLoss())`).  Every shipped yaml weights it 0: the reference evaluates it anyway
+  and multiplies by 0; here the term is skipped unless a module is supplied, and `combine` refuses a non-zero lambda_ssim
+  without one.
+* pointsdist (lambda 0 in every shipped yaml): skipped unless `compute_pointsdist=True`.
 * l2_xyz: plain device ops (a masked MSE over img_aligned_xyz, losses.py:286-291).
 """
 import torch
