@@ -118,6 +118,10 @@ __device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_g
 __device__ __forceinline__ void named_bar_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
+// signal the barrier without waiting for it (the other `threads` - 32 * warps participants bar.sync on the same id)
+__device__ __forceinline__ void named_bar_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
 
 // 2^x on the MUFU pipe (ex2.approx.ftz: 2 ulp, flushes denormals; -inf -> 0)
 __device__ __forceinline__ float ex2_approx(float x) {
