@@ -251,6 +251,38 @@ size_t dgs_dit_workspace_bytes(const dgs_dit_weights* w, int B, int V, int H, in
 int dgs_dit_forward(const dgs_dit_weights* w, const dgs_dit_io* io, void* workspace, size_t workspace_bytes,
                     void* stream);
 
+/* ---- opt-in FP8 (e4m3) inference: the qkv, mlp.fc1 and mlp.fc2 GEMMs of every block on e4m3 operands ----
+ * Weights: e4m3 [L, N, K] row-major with one fp32 scale per output channel, [L, N].  Activations: e4m3 [M, K] with
+ * one fp32 scale per row and 128-column group, stored transposed as [K/128][round_up(M, 4)].  Every scale is a power
+ * of two, 2^ceil(log2(amax / 448)) (1 for an all-zero group), so quantizing is an exact scaling and one
+ * round-to-nearest-even: q = e4m3(x / s).  A GEMM computes sw[n] * sum over k-blocks of sa[kb][m] * (qa qw^T)_kb, then
+ * the bf16 path's epilogue.  Everything else (input stage, conditioning, attention, attn.proj, heads) is the bf16 path;
+ * there is no FP8 training. */
+typedef struct {
+  const void* qkv_w; const float* qkv_s;  /* e4m3 [L, 3w, w], fp32 [L, 3w] */
+  const void* fc1_w; const float* fc1_s;  /* e4m3 [L, 4w, w], fp32 [L, 4w] */
+  const void* fc2_w; const float* fc2_s;  /* e4m3 [L, w, 4w], fp32 [L, w]  */
+} dgs_dit_weights_fp8;
+/* dgs_dit_workspace_bytes plus the activation scale arrays */
+size_t dgs_dit_workspace_bytes_fp8(const dgs_dit_weights* w, int B, int V, int H, int W);
+/* dgs_dit_forward with the three GEMMs above on FP8 (w8); w supplies every other weight.  Inference only: a non-NULL
+ * io->train_state is DGS_ERR_INVALID_ARGUMENT. */
+int dgs_dit_forward_fp8(const dgs_dit_weights* w, const dgs_dit_weights_fp8* w8, const dgs_dit_io* io, void* workspace,
+                        size_t workspace_bytes, void* stream);
+/* Building blocks of the FP8 forward (the same kernels it launches), for the unit tests and weight packing:
+ * q [rows, cols] e4m3, scale [rows] = x [rows, cols] fp32 with one power-of-two scale per row (the weight format). */
+int dgs_quantize_rows_e4m3(const float* x, int rows, int cols, void* q, float* scale, void* stream);
+/* dgs_ln_modulate (no LayerNorm weight) -> q e4m3 [B*rows, width] and q_scale [width/128][round_up(B*rows, 4)] */
+int dgs_ln_modulate_fp8(const float* x, const float* shift, const float* scale, int mod_stride, void* q, float* q_scale,
+                        int B, int rows, int width, float eps, void* stream);
+/* FP8 GEMM, A e4m3 [M, K] with group scales sa, W e4m3 [N, K] with channel scales sw; K % 128 == 0, N % 128 == 0,
+ * 16-byte aligned pointers.  epi: 0 = (acc + bias) -> bf16; 2 = out(fp32) += gate[row / rows_per_sample] * (acc + bias),
+ * in place; 3 = (acc + bias) -> fp32; 6 = GELU(tanh)(acc + bias) -> e4m3 out [M, ldc] with its group scales out_scale
+ * [N/128][round_up(M, 4)].  ldc: output row stride in elements. */
+int dgs_gemm_fp8(const void* A, const float* sa, const void* W, const float* sw, const float* bias, const float* gate,
+                 void* out, float* out_scale, int M, int N, int K, int epi, int ldc, int gate_stride,
+                 int rows_per_sample, void* stream);
+
 /* ---- training: backward of dgs_dit_forward (what torch autograd derives for denoiser.py:306-416 in the reference) ----
  * dgrad GEMMs read TRANSPOSED bf16 copies of the block weights (W^T, [in, out] row-major) so that every GEMM of the
  * backward runs on the same K-major wgmma kernel as the forward; the caller refreshes them after each optimizer step

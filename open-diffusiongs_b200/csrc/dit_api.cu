@@ -193,6 +193,72 @@ int block_forward(const dgs_dit_weights* w, int l, const float* m, int mod_strid
   return DGS_OK;
 }
 
+// FP8 inference: the activation scales of the e4m3 copies of h (LN outputs, [w/128][Ms]) and u (GELU output,
+// [4w/128][Ms]), carved after the bf16 workspace; the e4m3 activations themselves live in h / u.
+struct Fp8Workspace {
+  float* sa_h;
+  float* sa_u;
+  size_t bytes;
+  Fp8Workspace(void* base, const dgs_dit_weights* w, int B, int V, int H, int W) {
+    const size_t T = (size_t)V * (H / w->patch) * (W / w->patch), N = T + w->n_gaussians;
+    const size_t Ms = (size_t)fp8_scale_stride((int)(B * N));
+    Carver c(base);
+    sa_h = c.take<float>((size_t)(w->width / 128) * Ms);
+    sa_u = c.take<float>((size_t)(w->mlp_hidden / 128) * Ms);
+    bytes = c.bytes();
+  }
+};
+
+// One DiTBlock on the FP8 path (inference, residual stream x updated in place): LN -> e4m3, qkv (FP8) -> bf16,
+// attention and attn.proj as in block_forward, LN -> e4m3, fc1 (FP8) + GELU -> e4m3, fc2 (FP8) gated into x.
+int block_forward_fp8(const dgs_dit_weights* w, const dgs_dit_weights_fp8* w8, int l, const float* m, int mod_stride,
+                      int B, int N, float* x, uint8_t* h8, float* sa_h, __nv_bfloat16* qkv, __nv_bfloat16* attn,
+                      uint8_t* u8, float* sa_u, cudaStream_t st) {
+  const int D = w->width, U = w->mlp_hidden, M = B * N;
+  {
+    ProfScope ps(st, PROF_DIT_LN);
+    DGS_TRY(ln_modulate_fp8(x, m, m + D, mod_stride, h8, sa_h, B, N, D, 1e-6f, st));
+  }
+  {
+    ProfScope ps(st, PROF_DIT_GEMM_QKV);
+    GemmEpilogue ep;
+    ep.out = qkv; ep.ldc = 3 * D; ep.bias = w->qkv_b + (size_t)l * 3 * D;
+    DGS_TRY(gemm_fp8(h8, sa_h, (const uint8_t*)w8->qkv_w + (size_t)l * 3 * D * D, w8->qkv_s + (size_t)l * 3 * D, M, 3 * D,
+                     D, EPI_BIAS_BF16, ep, nullptr, st));
+  }
+  {
+    ProfScope ps(st, PROF_DIT_ATTN);
+    DGS_TRY(attention_fwd(qkv, attn, nullptr, B, N, w->heads, st));
+  }
+  {
+    ProfScope ps(st, PROF_DIT_GEMM_PROJ);
+    GemmEpilogue ep;
+    ep.out = x; ep.ldc = D; ep.bias = w->proj_b + (size_t)l * D;
+    ep.gate = m + 2 * D; ep.gate_stride = mod_stride; ep.rows_per_sample = N;
+    DGS_TRY(gemm_bf16(attn, (const __nv_bfloat16*)w->proj_w + (size_t)l * D * D, M, D, D, EPI_GATE_RESID_F32, ep, st));
+  }
+  {
+    ProfScope ps(st, PROF_DIT_LN);
+    DGS_TRY(ln_modulate_fp8(x, m + 3 * D, m + 4 * D, mod_stride, h8, sa_h, B, N, D, 1e-6f, st));
+  }
+  {
+    ProfScope ps(st, PROF_DIT_GEMM_FC1);
+    GemmEpilogue ep;
+    ep.out = u8; ep.ldc = U; ep.bias = w->fc1_b + (size_t)l * U;
+    DGS_TRY(gemm_fp8(h8, sa_h, (const uint8_t*)w8->fc1_w + (size_t)l * U * D, w8->fc1_s + (size_t)l * U, M, U, D,
+                     EPI_BIAS_GELU_E4M3, ep, sa_u, st));
+  }
+  {
+    ProfScope ps(st, PROF_DIT_GEMM_FC2);
+    GemmEpilogue ep;
+    ep.out = x; ep.ldc = D; ep.bias = w->fc2_b + (size_t)l * D;
+    ep.gate = m + 5 * D; ep.gate_stride = mod_stride; ep.rows_per_sample = N;
+    DGS_TRY(gemm_fp8(u8, sa_u, (const uint8_t*)w8->fc2_w + (size_t)l * D * U, w8->fc2_s + (size_t)l * D, M, D, U,
+                     EPI_GATE_RESID_F32, ep, nullptr, st));
+  }
+  return DGS_OK;
+}
+
 // the training-mode buffers of block l: slice l of the stacked tensors (store mode) or the single slot (recompute mode);
 // `keep_aux` = false drops the stores only the backward reads (recompute-mode forward pass)
 BlockBufs train_bufs(const TrainState& ts, const dgs_dit_weights* w, int l, size_t MD, size_t MU, int B, int N, bool keep_aux) {
@@ -208,26 +274,19 @@ BlockBufs train_bufs(const TrainState& ts, const dgs_dit_weights* w, int l, size
   return b;
 }
 
-}  // namespace
-
-extern "C" {
-
-size_t dgs_dit_workspace_bytes(const dgs_dit_weights* w, int B, int V, int H, int W) {
-  if (check_dit(w, B, V, H, W)) return 0;
-  return DitWorkspace(nullptr, w, B, V, H, W).bytes;
-}
-
-int dgs_dit_forward(const dgs_dit_weights* w, const dgs_dit_io* io, void* workspace, size_t workspace_bytes,
-                    void* stream) {
+// dgs_dit_forward (w8 == NULL) and dgs_dit_forward_fp8 (w8 != NULL: inference with the FP8 block GEMMs)
+int dit_forward(const dgs_dit_weights* w, const dgs_dit_weights_fp8* w8, const dgs_dit_io* io, void* workspace,
+                size_t workspace_bytes, cudaStream_t st) {
   DGS_REQUIRE(io != nullptr, "io is NULL");
   DGS_TRY(check_dit(w, io->B, io->V, io->H, io->W));
   DGS_REQUIRE(io->images && io->ray_o && io->ray_d && io->t, "NULL input");
   DGS_REQUIRE(io->xyz && io->features && io->scaling && io->rotation && io->opacity, "NULL output");
-  cudaStream_t st = (cudaStream_t)stream;
   const int B = io->B, V = io->V, H = io->H, W = io->W, D = w->width, L = w->layers, G = w->n_gaussians, p = w->patch;
   const int T = V * (H / p) * (W / p), N = T + G, Kin = p * p * 9, Ndec = p * p * 14;
   DitWorkspace ws(workspace, w, B, V, H, W);
-  DGS_REQUIRE(workspace && workspace_bytes >= ws.bytes, "workspace too small: %zu < %zu", workspace_bytes, ws.bytes);
+  Fp8Workspace ws8(workspace ? (char*)workspace + ws.bytes : nullptr, w, B, V, H, W);
+  const size_t need = ws.bytes + (w8 ? ws8.bytes : 0);
+  DGS_REQUIRE(workspace && workspace_bytes >= need, "workspace too small: %zu < %zu", workspace_bytes, need);
   const int mod_stride = L * 6 * D + 4 * D;
   const bool train = io->train_state != nullptr;
   const bool recompute = train && io->train_mode == DGS_TRAIN_RECOMPUTE;
@@ -269,7 +328,11 @@ int dgs_dit_forward(const dgs_dit_weights* w, const dgs_dit_io* io, void* worksp
       bb.h1 = ws.h; bb.h2 = ws.h; bb.qkv = ws.qkv; bb.attn = ws.attn; bb.u = ws.u;
       bb.proj_out = bb.fc2_out = bb.u_pre = nullptr; bb.lse = nullptr; bb.distinct = false;
     }
-    DGS_TRY(block_forward(w, l, m, mod_stride, B, N, bb, st));
+    if (w8)
+      DGS_TRY(block_forward_fp8(w, w8, l, m, mod_stride, B, N, ws.x, (uint8_t*)ws.h, ws8.sa_h, ws.qkv, ws.attn,
+                                (uint8_t*)ws.u, ws8.sa_u, st));
+    else
+      DGS_TRY(block_forward(w, l, m, mod_stride, B, N, bb, st));
   }
   float* x_fin = (train && !recompute) ? ts.x_all + (size_t)L * MD : ws.x;
   if (recompute) DGS_CUDA_OK(cudaMemcpyAsync(ts.x_all + (size_t)L * MD, ws.x, MD * sizeof(float), cudaMemcpyDeviceToDevice, st));
@@ -299,6 +362,54 @@ int dgs_dit_forward(const dgs_dit_weights* w, const dgs_dit_io* io, void* worksp
   DGS_TRY(gaussians_epilogue(ws.gs_tok, ws.img_gs, io->ray_o, io->ray_d, go, B, G, V, H, W, p, io->scene_depth,
                              io->range_near, io->range_far, st));
   return DGS_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t dgs_dit_workspace_bytes(const dgs_dit_weights* w, int B, int V, int H, int W) {
+  if (check_dit(w, B, V, H, W)) return 0;
+  return DitWorkspace(nullptr, w, B, V, H, W).bytes;
+}
+
+int dgs_dit_forward(const dgs_dit_weights* w, const dgs_dit_io* io, void* workspace, size_t workspace_bytes,
+                    void* stream) {
+  return dit_forward(w, nullptr, io, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+size_t dgs_dit_workspace_bytes_fp8(const dgs_dit_weights* w, int B, int V, int H, int W) {
+  if (check_dit(w, B, V, H, W)) return 0;
+  return DitWorkspace(nullptr, w, B, V, H, W).bytes + Fp8Workspace(nullptr, w, B, V, H, W).bytes;
+}
+
+int dgs_dit_forward_fp8(const dgs_dit_weights* w, const dgs_dit_weights_fp8* w8, const dgs_dit_io* io, void* workspace,
+                        size_t workspace_bytes, void* stream) {
+  DGS_REQUIRE(w8 && w8->qkv_w && w8->qkv_s && w8->fc1_w && w8->fc1_s && w8->fc2_w && w8->fc2_s, "NULL FP8 weight or scale");
+  DGS_REQUIRE(io == nullptr || io->train_state == nullptr,
+              "dgs_dit_forward_fp8 is inference only (io->train_state must be NULL; training runs bf16)");
+  return dit_forward(w, w8, io, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int dgs_quantize_rows_e4m3(const float* x, int rows, int cols, void* q, float* scale, void* stream) {
+  DGS_REQUIRE(x && q && scale, "NULL pointer");
+  return quantize_rows_e4m3(x, rows, cols, (uint8_t*)q, scale, (cudaStream_t)stream);
+}
+
+int dgs_ln_modulate_fp8(const float* x, const float* shift, const float* scale, int mod_stride, void* q, float* q_scale,
+                        int B, int rows, int width, float eps, void* stream) {
+  DGS_REQUIRE(x && shift && scale && q && q_scale, "NULL pointer");
+  return ln_modulate_fp8(x, shift, scale, mod_stride, (uint8_t*)q, q_scale, B, rows, width, eps, (cudaStream_t)stream);
+}
+
+int dgs_gemm_fp8(const void* A, const float* sa, const void* W, const float* sw, const float* bias, const float* gate,
+                 void* out, float* out_scale, int M, int N, int K, int epi, int ldc, int gate_stride,
+                 int rows_per_sample, void* stream) {
+  DGS_REQUIRE(epi != EPI_GATE_RESID_F32 || (gate && rows_per_sample > 0), "gate epilogue needs gate and rows_per_sample");
+  GemmEpilogue ep;
+  ep.out = out; ep.ldc = ldc; ep.bias = bias; ep.gate = gate; ep.gate_stride = gate_stride;
+  ep.rows_per_sample = rows_per_sample > 0 ? rows_per_sample : 1;
+  return gemm_fp8(A, sa, W, sw, M, N, K, epi, ep, out_scale, (cudaStream_t)stream);
 }
 
 size_t dgs_dit_train_state_bytes(const dgs_dit_weights* w, int B, int V, int H, int W) {

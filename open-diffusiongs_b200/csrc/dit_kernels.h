@@ -8,7 +8,7 @@
 namespace dgs {
 
 enum GemmEpi { EPI_BIAS_BF16 = 0, EPI_BIAS_GELU_BF16 = 1, EPI_GATE_RESID_F32 = 2, EPI_F32 = 3, EPI_DGELU_BF16 = 4,
-               EPI_BIAS_RELU_BF16 = 5 };
+               EPI_BIAS_RELU_BF16 = 5, EPI_BIAS_GELU_E4M3 = 6 };
 
 struct GemmEpilogue {
   void* out = nullptr;          // bf16 or fp32 [M, ldc]
@@ -31,6 +31,14 @@ int gemm_bf16(const void* A, const void* W, int M, int N, int K, int epi, const 
 // C[M,N] fp32 = A^T W for A [K,M], W [K,N] bf16 row-major (MN-major wgmma operands; ep.lda/ldb = row strides, 0 = M/N)
 int gemm_bf16_tn(const void* A, const void* W, int M, int N, int K, const GemmEpilogue& ep, cudaStream_t st);
 
+// FP8 operands (gemm_sm90.cu): A e4m3 [M, K] with group scales sa [K/128][fp8_scale_stride(M)] (one per row and
+// 128-column group), W e4m3 [N, K] with per-row scales sw [N].  C = epi(sw[n] * sum_kb sa[kb][m] * (A_kb W_kb^T)).
+// epi: EPI_BIAS_BF16, EPI_GATE_RESID_F32 (in place only), EPI_F32, or EPI_BIAS_GELU_E4M3 (out e4m3 [M, ldc] plus its
+// group scales out_scale [N/128][fp8_scale_stride(M)]).  K % 128 == 0, N % 128 == 0.
+inline int fp8_scale_stride(int M) { return (M + 3) / 4 * 4; }
+int gemm_fp8(const void* A, const float* sa, const void* W, const float* sw, int M, int N, int K, int epi,
+             const GemmEpilogue& ep, float* out_scale, cudaStream_t st);
+
 
 // softmax(Q K^T / sqrt(64)) V over qkv [B, N, 3, H, 64] (bf16) -> out [B, N, H*64] (bf16) (attention_sm90.cu)
 // lse2 (optional, training): [B, H, attention_lse_stride(N)] fp32, log2-domain log-sum-exp of the scaled scores
@@ -48,6 +56,12 @@ int attention_bwd(const void* qkv, const void* out, const void* dout, float* lse
 int ln_modulate(const float* x, const float* ln_weight, const float* shift, const float* scale, int mod_stride,
                 __nv_bfloat16* h, int B, int rows_in, int row_off, int rows_out, int D, float eps, int split,
                 cudaStream_t st);
+// the same LayerNorm + modulate (no LN weight, no gather) -> e4m3 q [B*rows, D] with one power-of-two scale per row
+// and 128-column group, q_scale [D/128][fp8_scale_stride(B*rows)]
+int ln_modulate_fp8(const float* x, const float* shift, const float* scale, int mod_stride, uint8_t* q, float* q_scale,
+                    int B, int rows, int D, float eps, cudaStream_t st);
+// q [rows, cols] e4m3 = x / scale[r] with one power-of-two scale per row (the FP8 weight format)
+int quantize_rows_e4m3(const float* x, int rows, int cols, uint8_t* q, float* scale, cudaStream_t st);
 // plain LayerNorm with weight (no bias), fp32 -> fp32, in place over [rows, D]
 int ln_weight_inplace(float* x, const float* w, int rows, int D, float eps, cudaStream_t st);
 // out[b, n] = act_in(in[b,:]) . W[n,:] + bias[n], W fp32 [N,K]; act_in: 0 none, 1 SiLU

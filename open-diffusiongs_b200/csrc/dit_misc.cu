@@ -5,6 +5,7 @@
 //       diffusionGS/models/transformers/utils_transformer.py:26-27,246-290.
 #include "dgs_internal.h"
 #include "dit_kernels.h"
+#include "sm90_ptx.cuh"
 
 namespace dgs {
 
@@ -18,6 +19,26 @@ __device__ __forceinline__ float warp_sum_f(float v) {
 // LayerNorm (+ optional weight) + adaLN modulate -> bf16.  One warp per row, D = 32 * 4 * VEC.
 // Two-pass statistics in registers (mean, then centred variance) = torch's LayerNorm numerics.
 // ---------------------------------------------------------------------------------------------
+// one warp loads row xr into v (lane l holds float4 number i of the row at columns 4 (32 i + l) .. + 3) and returns
+// its mean and 1 / sqrt(var + eps)
+template <int D>
+__device__ __forceinline__ void ln_row_stats(const float* xr, int lane, float (&v)[D / 32], float eps, float& mean,
+                                             float& rstd) {
+  constexpr int PER_LANE = D / 32;
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < PER_LANE / 4; i++) {
+    const float4 t = *reinterpret_cast<const float4*>(xr + (i * 32 + lane) * 4);
+    v[4 * i] = t.x; v[4 * i + 1] = t.y; v[4 * i + 2] = t.z; v[4 * i + 3] = t.w;
+    s += t.x + t.y + t.z + t.w;
+  }
+  mean = warp_sum_f(s) * (1.0f / D);
+  float q = 0.f;
+#pragma unroll
+  for (int i = 0; i < PER_LANE; i++) { const float d = v[i] - mean; q += d * d; }
+  rstd = rsqrtf(warp_sum_f(q) * (1.0f / D) + eps);
+}
+
 template <int D>
 __global__ void __launch_bounds__(256) ln_modulate_kernel(const float* __restrict__ x, const float* __restrict__ lnw,
                                                           const float* __restrict__ shift,
@@ -32,18 +53,8 @@ __global__ void __launch_bounds__(256) ln_modulate_kernel(const float* __restric
   const int b = warp / rows_out, r = warp - b * rows_out;
   const float* xr = x + ((size_t)b * rows_in + row_off + r) * D;
   float v[PER_LANE];
-  float s = 0.f;
-#pragma unroll
-  for (int i = 0; i < PER_LANE / 4; i++) {
-    const float4 t = *reinterpret_cast<const float4*>(xr + (i * 32 + lane) * 4);
-    v[4 * i] = t.x; v[4 * i + 1] = t.y; v[4 * i + 2] = t.z; v[4 * i + 3] = t.w;
-    s += t.x + t.y + t.z + t.w;
-  }
-  const float mean = warp_sum_f(s) * (1.0f / D);
-  float q = 0.f;
-#pragma unroll
-  for (int i = 0; i < PER_LANE; i++) { const float d = v[i] - mean; q += d * d; }
-  const float rstd = rsqrtf(warp_sum_f(q) * (1.0f / D) + eps);
+  float mean, rstd;
+  ln_row_stats<D>(xr, lane, v, eps, mean, rstd);
   const float* sh = shift + (size_t)b * mod_stride;
   const float* sc = scale + (size_t)b * mod_stride;
   __nv_bfloat16* hr = h + (size_t)warp * D * (split ? 3 : 1);
@@ -83,6 +94,87 @@ int ln_modulate(const float* x, const float* ln_weight, const float* shift, cons
   const int blocks = (int)((warps * 32 + 255) / 256);
   DGS_CUDA_OK(launch_pdl(ln_modulate_kernel<1024>, dim3(blocks), dim3(256), 0, st, x, ln_weight, shift, scale, mod_stride, h,
                          B, rows_in, row_off, rows_out, eps, split));
+  DGS_POST_LAUNCH();
+  return DGS_OK;
+}
+
+// LayerNorm + modulate -> e4m3 with 1 x 128 group scales (the FP8 GEMMs' A operand).  The LayerNorm and modulate
+// arithmetic is ln_modulate_kernel's; lane l's float4 number i lies in column group i, so each group's amax is one warp
+// reduction.
+template <int D>
+__global__ void __launch_bounds__(256) ln_modulate_fp8_kernel(const float* __restrict__ x,
+                                                              const float* __restrict__ shift,
+                                                              const float* __restrict__ scale, int mod_stride,
+                                                              uint8_t* __restrict__ q, float* __restrict__ q_scale,
+                                                              int lds, int B, int rows, float eps) {
+  constexpr int PER_LANE = D / 32, GROUPS = D / 128;
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  if (warp >= B * rows) return;
+  const int b = warp / rows;
+  float v[PER_LANE];
+  float mean, rstd;
+  ln_row_stats<D>(x + (size_t)warp * D, lane, v, eps, mean, rstd);
+  const float* sh = shift + (size_t)b * mod_stride;
+  const float* sc = scale + (size_t)b * mod_stride;
+  uint8_t* qr = q + (size_t)warp * D;
+#pragma unroll
+  for (int i = 0; i < GROUPS; i++) {
+    const int c = (i * 32 + lane) * 4;
+    const float4 s4 = __ldg(reinterpret_cast<const float4*>(sc + c));
+    const float4 h4 = __ldg(reinterpret_cast<const float4*>(sh + c));
+    const float o0 = (v[4 * i] - mean) * rstd * (1.f + s4.x) + h4.x;
+    const float o1 = (v[4 * i + 1] - mean) * rstd * (1.f + s4.y) + h4.y;
+    const float o2 = (v[4 * i + 2] - mean) * rstd * (1.f + s4.z) + h4.z;
+    const float o3 = (v[4 * i + 3] - mean) * rstd * (1.f + s4.w) + h4.w;
+    float amax = fmaxf(fmaxf(fabsf(o0), fabsf(o1)), fmaxf(fabsf(o2), fabsf(o3)));
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+    const int e = ptx::e4m3_scale_exp(amax);
+    const float inv = ptx::exp2_int(-e);
+    const uint32_t packed = (uint32_t)ptx::pack2_e4m3(o0 * inv, o1 * inv) | ((uint32_t)ptx::pack2_e4m3(o2 * inv, o3 * inv) << 16);
+    *reinterpret_cast<uint32_t*>(qr + c) = packed;
+    if (lane == 0) q_scale[(size_t)i * lds + warp] = ptx::exp2_int(e);
+  }
+}
+
+int ln_modulate_fp8(const float* x, const float* shift, const float* scale, int mod_stride, uint8_t* q, float* q_scale,
+                    int B, int rows, int D, float eps, cudaStream_t st) {
+  DGS_REQUIRE(D == 1024, "ln_modulate_fp8: width %d not supported (1024 only)", D);
+  DGS_REQUIRE(B > 0 && rows > 0, "ln_modulate_fp8: bad shape B=%d rows=%d", B, rows);
+  const long long warps = (long long)B * rows;
+  const int blocks = (int)((warps * 32 + 255) / 256);
+  DGS_CUDA_OK(launch_pdl(ln_modulate_fp8_kernel<1024>, dim3(blocks), dim3(256), 0, st, x, shift, scale, mod_stride, q,
+                         q_scale, fp8_scale_stride(B * rows), B, rows, eps));
+  DGS_POST_LAUNCH();
+  return DGS_OK;
+}
+
+// One block per row: amax, then the row times 2^-e rounded to e4m3 (the FP8 weight format, one scale per row).
+__global__ void __launch_bounds__(256) quantize_rows_e4m3_kernel(const float* __restrict__ x, int cols,
+                                                                 uint8_t* __restrict__ q, float* __restrict__ scale) {
+  __shared__ float red[8];
+  const float* xr = x + (size_t)blockIdx.x * cols;
+  float amax = 0.f;
+  for (int c = threadIdx.x; c < cols; c += blockDim.x) amax = fmaxf(amax, fabsf(xr[c]));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = amax;
+  __syncthreads();
+  amax = red[0];
+#pragma unroll
+  for (int w = 1; w < 8; w++) amax = fmaxf(amax, red[w]);
+  const int e = ptx::e4m3_scale_exp(amax);
+  const float inv = ptx::exp2_int(-e);
+  uint8_t* qr = q + (size_t)blockIdx.x * cols;
+  for (int c = threadIdx.x; c < cols; c += blockDim.x) qr[c] = (uint8_t)(ptx::pack2_e4m3(xr[c] * inv, 0.f) & 0xffu);
+  if (threadIdx.x == 0) scale[blockIdx.x] = ptx::exp2_int(e);
+}
+
+int quantize_rows_e4m3(const float* x, int rows, int cols, uint8_t* q, float* scale, cudaStream_t st) {
+  DGS_REQUIRE(rows > 0 && cols > 0, "quantize_rows_e4m3: bad shape %dx%d", rows, cols);
+  quantize_rows_e4m3_kernel<<<rows, 256, 0, st>>>(x, cols, q, scale);
   DGS_POST_LAUNCH();
   return DGS_OK;
 }

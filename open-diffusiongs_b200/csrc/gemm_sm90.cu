@@ -18,6 +18,7 @@
 //   EPI_F32             y = acc (+ b), fp32                 (tokenizer, decoder head, weight gradients)
 //   EPI_DGELU_BF16      y = acc * gelu'(u)                  (backward of mlp.fc2 -> act: u = saved pre-activation)
 //   EPI_BIAS_RELU_BF16  y = max(acc + b, 0)                 (the LPIPS VGG convolutions, lpips.cu)
+//   EPI_BIAS_GELU_E4M3  y = e4m3(gelu_tanh(acc + b)) + scales (FP8 mlp.fc1 -> fc2's operand; gemm_fp8_kernel only)
 // Training mode (GemmEpilogue::aux / resid): fc1 also stores its pre-activation, the gate epilogues also store the
 // pre-gate branch output and may read the residual from a different buffer than they write.
 #include <cstdlib>
@@ -159,7 +160,9 @@ __device__ __forceinline__ void epilogue_fragment(const GemmEpilogue& ep, const 
 
 // The output element type of the epilogues that stage their tile for a TMA store (see epilogue_tma).
 template <int EPI>
-constexpr int epi_out_bytes() { return (EPI == EPI_GATE_RESID_F32 || EPI == EPI_F32) ? 4 : 2; }
+constexpr int epi_out_bytes() {
+  return (EPI == EPI_GATE_RESID_F32 || EPI == EPI_F32) ? 4 : (EPI == EPI_BIAS_GELU_E4M3 ? 1 : 2);
+}
 
 // Epilogue of one warpgroup's 64 x BN fragment through shared memory: the values are computed in registers as in
 // epilogue_fragment, written to this warpgroup's staging buffer, and one thread hands the buffer to the TMA unit, which
@@ -331,6 +334,185 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 }
 
 // ---------------------------------------------------------------------------------------------
+// FP8 (e4m3) variant: same producer / two-consumer structure, ring and PDL as gemm_bf16_kernel, with
+//   * BK = 128 e4m3 = one 128-byte swizzle row (a stage has the bf16 kernel's byte size), 128 x 128 tiles (a 128 x 256
+//     tile would need 128 + 128 accumulator registers per thread: over the consumers' 232);
+//   * four wgmma m64n128k32 per k-block into a fresh partial tile, which is then added into the fp32 accumulator times
+//     its rows' activation scales sa[kb][m] (the producer brings the k-block's 128 row scales in with the stage).  This
+//     applies the 1 x 128 group scales and keeps the tensor core's reduced-precision FP8 accumulation to one 128-term
+//     partial sum;
+//   * the per-output-channel weight scale sw[n] multiplies the accumulator before the (shared) epilogue.
+// ---------------------------------------------------------------------------------------------
+constexpr int BK8 = 128, BN8 = 128;
+
+template <int OUT_BYTES>
+struct Fp8Cfg {
+  static constexpr int SMEM_LIMIT = 227 * 1024;
+  static constexpr int A_BYTES = BM * BK8, B_BYTES = BN8 * BK8, S_BYTES = BM * 4;
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int OUT_TILE_BYTES = BM * BN8 * OUT_BYTES;
+  static constexpr int EXTRA = 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int FIT = (SMEM_LIMIT - EXTRA - OUT_TILE_BYTES) / (STAGE_BYTES + S_BYTES);
+  static constexpr int STAGES = FIT < 6 ? FIT : 6;
+  static constexpr int SMEM_BYTES = STAGES * (STAGE_BYTES + S_BYTES) + OUT_TILE_BYTES + EXTRA;
+  static_assert(STAGES >= 3 && SMEM_BYTES <= SMEM_LIMIT, "FP8 GEMM configuration does not fit in shared memory");
+};
+
+struct Fp8Scales {
+  const float* sa;   // [K/128][lds] activation group scales
+  const float* sw;   // [N] weight scales
+  float* out_scale;  // EPI_BIAS_GELU_E4M3: [N/128][lds] group scales of the output
+  int lds;           // fp8_scale_stride(M)
+};
+
+// bias + GELU -> e4m3 of one warpgroup's 64 x 128 fragment: the tile's 128 columns are one scale group, so a row's
+// amax is a reduction over the 4 lanes that hold the row.  The bytes are staged (128-byte swizzled, like the TMA box
+// that stores them) and written by one TMA store; the row scales go straight to out_scale.
+__device__ __forceinline__ void epilogue_gelu_e4m3(const GemmEpilogue& ep, const Fp8Scales& fs, float (&acc)[64],
+                                                   uint8_t* stage, const CUtensorMap* tmC, int m0, int n0, int M,
+                                                   int wg, int wq, int lane) {
+  const bool leader = wq == 0 && lane == 0;
+  if (leader) bulk_wait_read<0>();
+  named_bar_sync(1 + wg, 128);
+#pragma unroll
+  for (int i = 0; i < 2; i++) {
+    const int r = 16 * wq + (lane >> 2) + 8 * i;
+    float amax = 0.f;
+#pragma unroll
+    for (int j = 0; j < BN8 / 8; j++) {
+      const int n = n0 + 8 * j + 2 * (lane & 3);
+      float2 v = make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+      if (ep.bias) {
+        const float2 b = __ldg(reinterpret_cast<const float2*>(ep.bias + n));
+        v.x += b.x; v.y += b.y;
+      }
+      v.x = epi_gelu_tanh(v.x); v.y = epi_gelu_tanh(v.y);
+      acc[4 * j + 2 * i] = v.x; acc[4 * j + 2 * i + 1] = v.y;
+      amax = fmaxf(amax, fmaxf(fabsf(v.x), fabsf(v.y)));
+    }
+    amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
+    amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
+    const int e = e4m3_scale_exp(amax);
+    const float inv = exp2_int(-e);
+    if ((lane & 3) == 0 && m0 + r < M) fs.out_scale[(size_t)(n0 / 128) * fs.lds + m0 + r] = exp2_int(e);
+#pragma unroll
+    for (int j = 0; j < BN8 / 8; j++) {
+      const int byte = 8 * j + 2 * (lane & 3);
+      uint8_t* p = stage + r * 128 + ((((byte >> 4) ^ (lane >> 2)) << 4) | (byte & 15));
+      *reinterpret_cast<uint16_t*>(p) = pack2_e4m3(acc[4 * j + 2 * i] * inv, acc[4 * j + 2 * i + 1] * inv);
+    }
+  }
+  fence_proxy_async();
+  named_bar_sync(1 + wg, 128);
+  if (leader) {
+    tma_store_2d(tmC, stage, n0, m0);
+    bulk_commit();
+  }
+}
+
+// TMA_EPI: the epilogue stages the tile for a TMA store (EPI_BIAS_BF16, EPI_BIAS_GELU_E4M3) or reduce-add
+// (EPI_GATE_RESID_F32, in place); else it writes from registers (EPI_F32).
+template <int EPI, bool TMA_EPI>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                const __grid_constant__ CUtensorMap tmC, GemmEpilogue ep, Fp8Scales fs, int M, int N, int K) {
+  using Cfg = Fp8Cfg<TMA_EPI ? epi_out_bytes<EPI>() : 0>;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw = smem_u32(smem_raw);
+  uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
+  uint8_t* sA = smem;
+  uint8_t* sB = smem + Cfg::STAGES * Cfg::A_BYTES;
+  uint8_t* sC = smem + Cfg::STAGES * Cfg::STAGE_BYTES;
+  float* sS = reinterpret_cast<float*>(sC + Cfg::OUT_TILE_BYTES);  // [STAGES][BM] row scales of the stage's k-block
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sS + Cfg::STAGES * BM);
+  uint64_t* empty_bar = full_bar + Cfg::STAGES;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int num_n = N / BN8, num_tiles = ((M + BM - 1) / BM) * num_n, num_k = K / BK8;
+
+  if (threadIdx.x == 0) {
+    prefetch_tmap(&tmA);
+    prefetch_tmap(&tmB);
+    for (int s = 0; s < Cfg::STAGES; s++) { mbar_init(full_bar + s, 1); mbar_init(empty_bar + s, 8); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  griddep_launch_dependents();
+  griddep_wait();
+
+  if (warp >= 8) {
+    // ===================== TMA producer =====================
+    ws_producer_regs();
+    if (warp == 8 && lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int m0 = (tile / num_n) * BM, n0 = (tile % num_n) * BN8;
+        // the scale rows [m0, min(m0 + 128, lds)): lds % 4 == 0, so a multiple of 16 bytes that stays inside sa
+        const uint32_t sbytes = (uint32_t)min(BM, fs.lds - m0) * 4u;
+        for (int kb = 0; kb < num_k; kb++) {
+          mbar_wait(empty_bar + stage, phase ^ 1);
+          mbar_arrive_expect_tx(full_bar + stage, Cfg::STAGE_BYTES + sbytes);
+          tma_load_2d(sA + stage * Cfg::A_BYTES, &tmA, full_bar + stage, kb * BK8, m0);
+          tma_load_2d(sB + stage * Cfg::B_BYTES, &tmB, full_bar + stage, kb * BK8, n0);
+          bulk_load_1d(sS + stage * BM, fs.sa + (size_t)kb * fs.lds + m0, sbytes, full_bar + stage);
+          if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+  } else {
+    // ===================== consumer warpgroups 0, 1: rows [64 wg, 64 wg + 64) of each tile =====================
+    ws_consumer_regs();
+    const int wg = warp >> 2;
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // the thread's rows r0, r0 + 8 of the tile
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[64], part[64];
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const int m0 = (tile / num_n) * BM, n0 = (tile % num_n) * BN8;
+#pragma unroll
+      for (int i = 0; i < 64; i++) acc[i] = 0.f;
+      for (int kb = 0; kb < num_k; kb++) {
+        mbar_wait(full_bar + stage, phase);
+        const uint64_t adesc = wg_desc_sw128(smem_u32(sA + stage * Cfg::A_BYTES + wg * 8192), 16, 1024);
+        const uint64_t bdesc = wg_desc_sw128(smem_u32(sB + stage * Cfg::B_BYTES), 16, 1024);
+        wg_fence();
+#pragma unroll
+        for (int k = 0; k < BK8 / 32; k++) wgmma_m64n128k32_e4m3(part, adesc + 2 * k, bdesc + 2 * k, k);
+        wg_commit();
+        wg_wait<0>();
+        wg_fence_regs(part);
+        const float s0 = sS[stage * BM + r0], s1 = sS[stage * BM + r0 + 8];
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty_bar + stage);
+#pragma unroll
+        for (int j = 0; j < 16; j++) {
+          acc[4 * j] = fmaf(s0, part[4 * j], acc[4 * j]);
+          acc[4 * j + 1] = fmaf(s0, part[4 * j + 1], acc[4 * j + 1]);
+          acc[4 * j + 2] = fmaf(s1, part[4 * j + 2], acc[4 * j + 2]);
+          acc[4 * j + 3] = fmaf(s1, part[4 * j + 3], acc[4 * j + 3]);
+        }
+        if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+      }
+#pragma unroll
+      for (int j = 0; j < 16; j++) {
+        const float2 w = __ldg(reinterpret_cast<const float2*>(fs.sw + n0 + 8 * j + 2 * (lane & 3)));
+        acc[4 * j] *= w.x; acc[4 * j + 1] *= w.y; acc[4 * j + 2] *= w.x; acc[4 * j + 3] *= w.y;
+      }
+      uint8_t* stg = sC + wg * (Cfg::OUT_TILE_BYTES / 2);
+      if constexpr (EPI == EPI_BIAS_GELU_E4M3) {
+        epilogue_gelu_e4m3(ep, fs, acc, stg, &tmC, m0 + wg * 64, n0, M, wg, warp & 3, lane);
+      } else if constexpr (TMA_EPI) {
+        epilogue_tma<EPI, BN8>(ep, acc, stg, &tmC, m0 + wg * 64, n0, M, N, wg, warp & 3, lane);
+      } else {
+        epilogue_fragment<EPI, BN8>(ep, acc, m0 + r0, n0 + 2 * (lane & 3), M, N, false);
+      }
+    }
+    if (TMA_EPI && (warp & 3) == 0 && lane == 0) bulk_wait<0>();
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
 // host launcher
 // ---------------------------------------------------------------------------------------------
 static int num_sms() {
@@ -471,6 +653,77 @@ int gemm_bf16_tn(const void* A, const void* W, int M, int N, int K, const GemmEp
   if (splits > 1) DGS_CUDA_OK(cudaMemset2DAsync(ep.out, (size_t)ldc * 4, 0, (size_t)N * 4, (size_t)M, st));
   return wide ? launch_gemm<256, EPI_F32, true, false>(tmA, tmB, tmC, e2, M, N, K, st, splits)
               : launch_gemm<128, EPI_F32, true, false>(tmA, tmB, tmC, e2, M, N, K, st, splits);
+}
+
+template <int EPI, bool TMA_EPI>
+static int launch_fp8(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const GemmEpilogue& ep,
+                      const Fp8Scales& fs, int M, int N, int K, cudaStream_t st) {
+  using Cfg = Fp8Cfg<TMA_EPI ? epi_out_bytes<EPI>() : 0>;
+  auto kern = gemm_fp8_kernel<EPI, TMA_EPI>;
+  static bool configured = false;
+  if (!configured) {
+    DGS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    configured = true;
+  }
+  const int sms = num_sms();
+  DGS_REQUIRE(sms > 0, "gemm_fp8: cannot query the device's SM count");
+  const int tiles = ceil_div(M, BM) * (N / BN8);
+  DGS_CUDA_OK(launch_pdl(kern, dim3(tiles < sms ? tiles : sms), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, st, tmA, tmB, tmC, ep,
+                         fs, M, N, K));
+  DGS_POST_LAUNCH();
+  return DGS_OK;
+}
+
+int gemm_fp8(const void* A, const float* sa, const void* W, const float* sw, int M, int N, int K, int epi,
+             const GemmEpilogue& ep, float* out_scale, cudaStream_t st) {
+  DGS_REQUIRE(M > 0 && N > 0 && K > 0, "gemm_fp8: bad shape %dx%dx%d", M, N, K);
+  DGS_REQUIRE(K % 128 == 0 && N % 128 == 0, "gemm_fp8: need K %% 128 == 0 and N %% 128 == 0 (got N=%d K=%d)", N, K);
+  DGS_REQUIRE(epi == EPI_BIAS_BF16 || epi == EPI_GATE_RESID_F32 || epi == EPI_F32 || epi == EPI_BIAS_GELU_E4M3,
+              "gemm_fp8: unsupported epilogue %d (0 bias -> bf16, 2 gate + residual, 3 fp32, 6 bias + GELU -> e4m3)", epi);
+  DGS_REQUIRE(A && W && ep.out, "gemm_fp8: NULL operand or output");
+  DGS_REQUIRE(sa && sw, "gemm_fp8: NULL scales (activation group scales and weight scales are required)");
+  DGS_REQUIRE(epi != EPI_BIAS_GELU_E4M3 || out_scale, "gemm_fp8: the GELU -> e4m3 epilogue needs out_scale");
+  DGS_REQUIRE(epi != EPI_GATE_RESID_F32 || (ep.gate && !ep.resid && !ep.aux),
+              "gemm_fp8: the gate epilogue needs gate and runs in place only");
+  DGS_REQUIRE(((uintptr_t)A % 16) == 0 && ((uintptr_t)W % 16) == 0 && ((uintptr_t)sa % 16) == 0 &&
+                  ((uintptr_t)(out_scale) % 16) == 0 && ((uintptr_t)ep.out % 16) == 0,
+              "gemm_fp8: operands, scales and output must be 16-byte aligned");
+  const bool tma_epi = epi != EPI_F32;
+  const int ob = tma_epi ? (epi == EPI_GATE_RESID_F32 ? 4 : (epi == EPI_BIAS_GELU_E4M3 ? 1 : 2)) : 4;
+  DGS_REQUIRE(ep.ldc >= N && ((size_t)ep.ldc * ob) % 16 == 0, "gemm_fp8: output row stride %d must be >= N and 16-byte "
+              "aligned", ep.ldc);
+  const int sms = num_sms();
+  DGS_REQUIRE(sms > 0, "gemm_fp8: cannot query the device's SM count");
+  Fp8Scales fs;
+  fs.sa = sa; fs.sw = sw; fs.out_scale = out_scale; fs.lds = fp8_scale_stride(M);
+  CUtensorMap tmA, tmB, tmC;
+  memset(&tmC, 0, sizeof(tmC));
+  {
+    uint64_t dims[2] = {(uint64_t)K, (uint64_t)M}, str[1] = {(uint64_t)K};
+    uint32_t box[2] = {BK8, BM};
+    int rc = make_tmap(&tmA, CU_TENSOR_MAP_DATA_TYPE_UINT8, A, 2, dims, str, box);
+    if (rc) return rc;
+  }
+  {
+    uint64_t dims[2] = {(uint64_t)K, (uint64_t)N}, str[1] = {(uint64_t)K};
+    uint32_t box[2] = {BK8, BN8};
+    int rc = make_tmap(&tmB, CU_TENSOR_MAP_DATA_TYPE_UINT8, W, 2, dims, str, box);
+    if (rc) return rc;
+  }
+  if (tma_epi) {  // one box = one 128-byte column block x the 64 rows of a consumer warpgroup
+    const CUtensorMapDataType type = ob == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                     : (ob == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_UINT8);
+    uint64_t dims[2] = {(uint64_t)N, (uint64_t)M}, str[1] = {(uint64_t)ep.ldc * ob};
+    uint32_t box[2] = {(uint32_t)(128 / ob), 64};
+    int rc = make_tmap(&tmC, type, ep.out, 2, dims, str, box);
+    if (rc) return rc;
+  }
+  switch (epi) {
+    case EPI_BIAS_BF16: return launch_fp8<EPI_BIAS_BF16, true>(tmA, tmB, tmC, ep, fs, M, N, K, st);
+    case EPI_GATE_RESID_F32: return launch_fp8<EPI_GATE_RESID_F32, true>(tmA, tmB, tmC, ep, fs, M, N, K, st);
+    case EPI_BIAS_GELU_E4M3: return launch_fp8<EPI_BIAS_GELU_E4M3, true>(tmA, tmB, tmC, ep, fs, M, N, K, st);
+    default: return launch_fp8<EPI_F32, false>(tmA, tmB, tmC, ep, fs, M, N, K, st);
+  }
 }
 
 }  // namespace dgs

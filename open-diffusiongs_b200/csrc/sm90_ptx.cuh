@@ -134,6 +134,24 @@ __device__ __forceinline__ uint32_t pack2_bf16(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&v);
 }
 
+// ---- e4m3 (FP8) quantization with power-of-two scales ----------------------------------------------
+// A group with absolute maximum amax gets the scale s = 2^e, e = ceil(log2(amax / 448)) (the smallest e with
+// amax <= 448 * 2^e, clamped to [-126, 126]; e = 0 when amax is 0).  amax = f * 2^(E-1), f in [1, 2): 448 * 2^(E-10)
+// = 0.875 * 2^E >= amax iff f <= 1.75, so e is read off amax's exponent and mantissa bits, with no division.
+__device__ __forceinline__ int e4m3_scale_exp(float amax) {
+  if (!(amax > 0.f)) return 0;
+  const uint32_t b = __float_as_uint(amax);
+  const int e = (int)((b >> 23) & 0xffu) - 135 + ((b & 0x7fffffu) > 0x600000u ? 1 : 0);
+  return e < -126 ? -126 : (e > 126 ? 126 : e);
+}
+__device__ __forceinline__ float exp2_int(int e) { return __int_as_float((e + 127) << 23); }  // e in [-126, 127]
+// two values -> two e4m3 bytes (lo at the lower address), round to nearest even, saturating to +-448
+__device__ __forceinline__ uint16_t pack2_e4m3(float lo, float hi) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+
 // ---- wgmma ------------------------------------------------------------------------------------
 // Shared-memory matrix descriptor, 128-byte swizzle, tile rows of exactly 128 bytes (64 bf16), tile base 1024-byte
 // aligned.  bits: [0,14) addr>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [62,64) layout (1 = SWIZZLE_128B).
@@ -187,6 +205,24 @@ __device__ __forceinline__ void wgmma_m64n64_ss(float (&d)[32], uint64_t da, uin
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, 1, 1, 1, %34, %35;"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
       : "l"(da), "l"(db), "n"(TA), "n"(TB));
+}
+// e4m3 x e4m3 -> fp32, both operands K-major from shared memory (the only layout wgmma takes for 8-bit types).  One
+// k32 step is 32 bytes along the swizzle row, the same descriptor step as a bf16 k16.  accumulate = 0: D = A x B
+// (D's previous contents are ignored, so a fresh partial-sum tile needs no zeroing).
+__device__ __forceinline__ void wgmma_m64n128k32_e4m3(float (&d)[64], uint64_t da, uint64_t db, int accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(accumulate));
+}
+// non-tensor bulk copy global -> shared (16-byte aligned, bytes % 16 == 0), completing on an mbarrier's tx count
+__device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* src, uint32_t bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
+                   smem_u32(smem_dst)),
+               "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(smem_u32(bar))
+               : "memory");
 }
 template <int TB>
 __device__ __forceinline__ void wgmma_m64n64_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t db) {

@@ -45,6 +45,13 @@ class DitIO(C.Structure):
 TRAIN_STORE, TRAIN_RECOMPUTE = 0, 1  # dgs_dit_io.train_mode
 
 
+class DitWeightsFp8(C.Structure):  # dgs_dit_weights_fp8
+    _fields_ = [(n, C.c_void_p) for n in ("qkv_w", "qkv_s", "fc1_w", "fc1_s", "fc2_w", "fc2_s")]
+
+
+FP8_EPI_BIAS_BF16, FP8_EPI_GATE_RESID_F32, FP8_EPI_F32, FP8_EPI_BIAS_GELU_E4M3 = 0, 2, 3, 6  # dgs_gemm_fp8 epi
+
+
 class DitBwdOpts(C.Structure):  # dgs_dit_bwd_opts
     _fields_ = [("block_done", C.POINTER(C.c_void_p))]
 
@@ -166,6 +173,13 @@ def lib():
         L.dgs_ssim_forward.argtypes = [C.c_int, C.c_int, C.c_int, vp, vp, C.c_float, C.c_int, vp, vp, vp, vp, C.c_size_t,
                                        vp]
         L.dgs_ssim_backward.argtypes = [C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]
+        L.dgs_dit_workspace_bytes_fp8.restype = C.c_size_t
+        L.dgs_dit_workspace_bytes_fp8.argtypes = [C.POINTER(DitWeights), C.c_int, C.c_int, C.c_int, C.c_int]
+        L.dgs_dit_forward_fp8.argtypes = [C.POINTER(DitWeights), C.POINTER(DitWeightsFp8), C.POINTER(DitIO), vp, C.c_size_t,
+                                          vp]
+        L.dgs_quantize_rows_e4m3.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp]
+        L.dgs_ln_modulate_fp8.argtypes = [vp, vp, vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_float, vp]
+        L.dgs_gemm_fp8.argtypes = [vp] * 8 + [C.c_int] * 7 + [vp]
         _lib = L
     return _lib
 
@@ -203,4 +217,5 @@ EXPORTED = [  # every symbol include/dgs_b200.h declares (checked by tests/test_
     "dgs_adamw_ema_step", "dgs_render_batch_forward_mse", "dgs_render_batch_backward_mse", "dgs_dit_export_state",
     "dgs_dit_export_ends", "dgs_lpips_workspace_bytes", "dgs_lpips_state_bytes", "dgs_lpips_forward", "dgs_lpips_backward",
     "dgs_ssim_workspace_bytes", "dgs_ssim_state_bytes", "dgs_ssim_forward", "dgs_ssim_backward",
+    "dgs_dit_workspace_bytes_fp8", "dgs_dit_forward_fp8", "dgs_quantize_rows_e4m3", "dgs_ln_modulate_fp8", "dgs_gemm_fp8",
 ]

@@ -15,7 +15,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from ._lib import DitIO, DitWeights, check
+from ._lib import DitIO, DitWeights, DitWeightsFp8, check
 from .renderer import Renderer
 
 _REGISTRY = {}
@@ -139,6 +139,9 @@ class DGSDenoiser(nn.Module):
         self.register_buffer("_dummy", torch.zeros(0, dtype=torch.float32), persistent=False)  # dGS/utils/base.py:115
         self._packed = None
         self._packed_key = None
+        self._packed_fp8 = None
+        self._packed_fp8_key = None
+        self._precision = "bf16"
         if c.pretrained_model_name_or_path:
             sd = torch.load(c.pretrained_model_name_or_path, map_location="cpu", weights_only=False)
             if "model" in sd:  # denoiser.py:259-268
@@ -196,6 +199,41 @@ class DGSDenoiser(nn.Module):
         self._packed, self._packed_key = (w, t), key
         return self._packed
 
+    def packed_weights_fp8(self):
+        """The qkv / fc1 / fc2 weights of every block in the FP8 format of dgs_dit_weights_fp8 (e4m3 + one power-of-two
+        scale per output channel, quantized by dgs_quantize_rows_e4m3), re-packed when any parameter changed."""
+        key = self._pack_key()
+        if self._packed_fp8 is not None and self._packed_fp8_key == key:
+            return self._packed_fp8
+        L = _lib.lib()
+        stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        w8, t = DitWeightsFp8(), {}
+        for name, get in (("qkv", lambda b: b.attn.qkv.weight), ("fc1", lambda b: b.mlp.fc1.weight),
+                          ("fc2", lambda b: b.mlp.fc2.weight)):
+            src = torch.stack([get(b).detach().float() for b in self.transformer]).contiguous()
+            n_layers, n, k = src.shape
+            q = torch.empty(n_layers, n, k, dtype=torch.uint8, device=src.device)
+            s = torch.empty(n_layers, n, dtype=torch.float32, device=src.device)
+            check(L.dgs_quantize_rows_e4m3(src.data_ptr(), n_layers * n, k, q.data_ptr(), s.data_ptr(), stream))
+            t[name + "_w"], t[name + "_s"] = q, s
+            setattr(w8, name + "_w", q.data_ptr())
+            setattr(w8, name + "_s", s.data_ptr())
+        self._packed_fp8, self._packed_fp8_key = (w8, t), key
+        return self._packed_fp8
+
+    # ---- inference precision ----
+    def set_inference_precision(self, precision):
+        """"bf16" (default): every GEMM on bf16 operands.  "fp8": inference runs the qkv, mlp.fc1 and mlp.fc2 GEMMs of
+        every block on e4m3 operands with power-of-two scales (dgs_dit_forward_fp8); training refuses to run."""
+        if precision not in ("bf16", "fp8"):
+            raise ValueError(f"inference precision {precision!r} (expected 'bf16' or 'fp8')")
+        self._precision = precision
+        return self
+
+    @property
+    def inference_precision(self):
+        return self._precision
+
     # ---- reference API ----
     @property
     def dtype(self):
@@ -210,6 +248,9 @@ class DGSDenoiser(nn.Module):
         in train() mode that has a DitTrainer attached (dgs_b200/train.py), the call is recorded as ONE autograd node
         whose backward is dgs_dit_backward (activations stored, not recomputed)."""
         if torch.is_grad_enabled() and self.training and getattr(self, "_trainer", None) is not None:
+            if self._precision == "fp8":
+                raise RuntimeError("DGSDenoiser: FP8 is an inference precision; training runs bf16 "
+                                   "(set_inference_precision('bf16') before a training forward)")
             from .train import dit_train_forward
             out, img_xyz = dit_train_forward(self, images, ray_o, ray_d, t)
             return (out, img_xyz, None) if return_tokens else (out, img_xyz)
@@ -244,7 +285,8 @@ class DGSDenoiser(nn.Module):
             n_tok = c.n_gaussians + V * (H // c.patch_size) * (W // c.patch_size)
             tokens = new(B, n_tok, c.width) if return_tokens else None
             L = _lib.lib()
-            nbytes = L.dgs_dit_workspace_bytes(C.byref(w), B, V, H, W)
+            fp8 = self._precision == "fp8" and train_state is None
+            nbytes = (L.dgs_dit_workspace_bytes_fp8 if fp8 else L.dgs_dit_workspace_bytes)(C.byref(w), B, V, H, W)
             if nbytes == 0:
                 raise _lib.DgsError(L.dgs_last_error().decode())
             ws = getattr(self, "_workspace", None)  # grow-only, re-used step after step
@@ -258,8 +300,12 @@ class DGSDenoiser(nn.Module):
                        rotation=out.rotation.data_ptr(), opacity=out.opacity.data_ptr(),
                        img_aligned_xyz=img_xyz.data_ptr(), tokens_out=None if tokens is None else tokens.data_ptr(),
                        train_state=None if train_state is None else train_state.data_ptr(), train_mode=int(train_mode))
-            check(L.dgs_dit_forward(C.byref(w), C.byref(io), ws.data_ptr(), nbytes,
-                                    C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+            stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            if fp8:
+                w8, _keep8 = self.packed_weights_fp8()
+                check(L.dgs_dit_forward_fp8(C.byref(w), C.byref(w8), C.byref(io), ws.data_ptr(), nbytes, stream))
+            else:
+                check(L.dgs_dit_forward(C.byref(w), C.byref(io), ws.data_ptr(), nbytes, stream))
         keep = (io, ws, nbytes, images, ray_o, ray_d, tf, w, _keep)  # what a later dgs_dit_backward needs alive
         return out, img_xyz, tokens, keep
 
