@@ -328,9 +328,29 @@ int dgs_dit_backward(const dgs_dit_weights* w, const dgs_dit_weights_t* wT, cons
  * parameter gradient of transformer block l is final (the blocks are differentiated in reverse order), block_done[layers]
  * when the remaining gradients (tokenizer, embedder, heads) are.  A side stream that waits on block_done[l]
  * (dgs_stream_wait_event) can all-reduce block l's contiguous bucket while blocks l-1 .. 0 are still running.
- * Entries may be NULL; events come from dgs_event_create. */
+ * Entries may be NULL; events come from dgs_event_create.
+ *
+ * trace (NULL: none) reads out the backward's per-block gradients for the per-block parity tests: each field is NULL or
+ * the DEVICE base of a caller buffer stacked over the layers (slice l of a [layers, ...] field belongs to block l), which
+ * the backward fills by cudaMemcpyAsync on `stream` at the point where that tensor is final.  M = B*N rows,
+ * Np = round_up(N, 128).  The names are the gradients of the tensors dgs_dit_export_state reads out:
+ *   dx [layers + 1, M, width] fp32: the gradient of the residual stream; slice layers right after the heads, slice l
+ *   once block l is differentiated (the gradient of the stream entering it);
+ *   dx_mid [layers, M, width] fp32: of x_mid (after the MLP branch's LayerNorm + modulate backward);
+ *   d_fc2_out, d_proj_out [layers, M, width] bf16: gate * dx of the two branches (the pre-gate branch outputs);
+ *   du_pre [layers, M, mlp_hidden] bf16: of u_pre (the fc2 dgrad times gelu'(u_pre));
+ *   dh2, dh1 [layers, M, width] bf16: of h2 / h1 (the fc1 / qkv dgrad);
+ *   d_attn [layers, M, width] bf16: of attn (the attn.proj dgrad);
+ *   dsum [layers, B, heads, Np] fp32: rowsum(attn * d_attn) per head (pad entries 0);  dqkv [layers, M, 3*width] bf16.
+ * Kernels and results do not depend on the trace. */
 typedef struct {
-  void** block_done;   /* NULL or [layers + 1] events */
+  float* dx; float* dx_mid;
+  void* d_fc2_out; void* du_pre; void* dh2; void* d_proj_out; void* d_attn;
+  float* dsum; void* dqkv; void* dh1;
+} dgs_dit_bwd_trace;
+typedef struct {
+  void** block_done;                /* NULL or [layers + 1] events */
+  const dgs_dit_bwd_trace* trace;   /* NULL or the per-block read-out above */
 } dgs_dit_bwd_opts;
 int dgs_dit_backward_ex(const dgs_dit_weights* w, const dgs_dit_weights_t* wT, const dgs_dit_io* io,
                         const dgs_dit_out_grads* dout, const dgs_dit_grads* grads, const dgs_dit_bwd_opts* opts,

@@ -71,6 +71,7 @@ struct TrainState {
   float* dsum;              // [B, heads, Np]
   float* dcond;             // [3][B, w]   dsilu(c) / dtemb1 / pre1
   float* ln_stats;          // [M, 2]      (mean, rstd) of the LayerNorm being differentiated
+  float* skb_part;          // per-CTA partial sums of the adaLN / timestep-MLP input gradients (skinny_linear_bwd)
   float* d_gs_tok;          // [B*G, 14]
   __nv_bfloat16* dyb;       // [M, w]      gated branch gradient / generic [M, w] bf16
   __nv_bfloat16* dh;        // [M, w]
@@ -107,6 +108,7 @@ struct TrainState {
     dsum = c.take<float>((size_t)B * w->heads * Np);
     dcond = c.take<float>((size_t)3 * B * D);
     ln_stats = c.take<float>(2 * M);
+    skb_part = c.take<float>(skinny_linear_bwd_part_floats(B, (int)(6 * D), (int)D));  // the widest: a block's 6w rows
     d_gs_tok = c.take<float>((size_t)B * w->n_gaussians * 14 + 16);
     dyb = c.take<__nv_bfloat16>(M * D);
     dh = c.take<__nv_bfloat16>(M * D);
@@ -523,6 +525,14 @@ int dgs_dit_backward_ex(const dgs_dit_weights* w, const dgs_dit_weights_t* wT, c
   const size_t MD = (size_t)M * D, MU = (size_t)M * U;
   const int Np = attention_lse_stride(N);
   void** done_ev = opts ? opts->block_done : nullptr;
+  const dgs_dit_bwd_trace no_trace = {};
+  const dgs_dit_bwd_trace& tr = opts && opts->trace ? *opts->trace : no_trace;
+  // trace read-out: slice `slice` of the stacked caller buffer `base` <- `bytes` of src (NULL field: nothing)
+  auto trace = [&](void* base, int slice, const void* src, size_t bytes) -> int {
+    if (base) DGS_CUDA_OK(cudaMemcpyAsync((char*)base + (size_t)slice * bytes, src, bytes, cudaMemcpyDeviceToDevice, st));
+    return DGS_OK;
+  };
+  const size_t f4 = sizeof(float), b2 = sizeof(__nv_bfloat16);
 
   // gradients accumulated by atomics start from zero; GEMM-produced ones are overwritten
   DGS_CUDA_OK(cudaMemsetAsync(ts.dmod, 0, (size_t)B * mod_stride * sizeof(float), st));
@@ -578,6 +588,7 @@ int dgs_dit_backward_ex(const dgs_dit_weights* w, const dgs_dit_weights_t* wT, c
                               g->ups_ln_w, ts.ln_stats, st));
     }
   }
+  DGS_TRY(trace(tr.dx, L, ts.dx, MD * f4));
 
   // ---- L x DiTBlock, reversed ----
   for (int l = L - 1; l >= 0; l--) {
@@ -597,6 +608,7 @@ int dgs_dit_backward_ex(const dgs_dit_weights* w, const dgs_dit_weights_t* wT, c
       DGS_TRY(gate_bwd(ts.dx, ts.fc2_out + sl * MD, m + 5 * D, mod_stride, N, M, D, ts.dyb, nullptr, dm + 5 * D,
                        g->fc2_b + l * LS, st));
     }
+    DGS_TRY(trace(tr.d_fc2_out, l, ts.dyb, MD * b2));
     {
       ProfScope ps(st, PROF_DIT_BWD_WGRAD);
       DGS_TRY(wgrad_tn(ts.dyb, D, ts.u + sl * MU, U, g->fc2_w + l * LS, D, U, M));
@@ -606,6 +618,7 @@ int dgs_dit_backward_ex(const dgs_dit_weights* w, const dgs_dit_weights_t* wT, c
       DGS_TRY(dgrad(ts.dyb, (const __nv_bfloat16*)wT->fc2_wT + (size_t)l * D * U, ts.big0, M, U, D, EPI_DGELU_BF16,
                     ts.u_pre + sl * MU));  // du_pre = (dy W2) * gelu'(u_pre)
     }
+    DGS_TRY(trace(tr.du_pre, l, ts.big0, MU * b2));
     {
       ProfScope ps(st, PROF_DIT_BWD_ELEM);
       DGS_TRY(colsum_bf16(ts.big0, M, U, g->fc1_b + l * LS, st));
@@ -618,14 +631,17 @@ int dgs_dit_backward_ex(const dgs_dit_weights* w, const dgs_dit_weights_t* wT, c
       ProfScope ps(st, PROF_DIT_BWD_DGRAD);
       DGS_TRY(dgrad(ts.big0, (const __nv_bfloat16*)wT->fc1_wT + (size_t)l * D * U, ts.dh, M, D, U, EPI_BIAS_BF16, nullptr));
     }
+    DGS_TRY(trace(tr.dh2, l, ts.dh, MD * b2));
     {
       ProfScope ps(st, PROF_DIT_BWD_ELEM);
       DGS_TRY(ln_modulate_bwd(x_mid, ts.dh, 0, nullptr, m + 4 * D, mod_stride, B, N, 0, N, D, 1e-6f, ts.dx, 1, dm + 3 * D,
                               dm + 4 * D, nullptr, ts.ln_stats, st));
+      DGS_TRY(trace(tr.dx_mid, l, ts.dx, MD * f4));
       // -- attention branch: x_mid = x_in + gate_msa * proj(attn(qkv(h1)))
       DGS_TRY(gate_bwd(ts.dx, ts.proj_out + sl * MD, m + 2 * D, mod_stride, N, M, D, ts.dyb, nullptr, dm + 2 * D,
                        g->proj_b + l * LS, st));
     }
+    DGS_TRY(trace(tr.d_proj_out, l, ts.dyb, MD * b2));
     {
       ProfScope ps(st, PROF_DIT_BWD_WGRAD);
       DGS_TRY(wgrad_tn(ts.dyb, D, ts.attn + sl * MD, D, g->proj_w + l * LS, D, D, M));
@@ -634,11 +650,14 @@ int dgs_dit_backward_ex(const dgs_dit_weights* w, const dgs_dit_weights_t* wT, c
       ProfScope ps(st, PROF_DIT_BWD_DGRAD);
       DGS_TRY(dgrad(ts.dyb, (const __nv_bfloat16*)wT->proj_wT + (size_t)l * D * D, ts.dh, M, D, D, EPI_BIAS_BF16, nullptr));
     }
+    DGS_TRY(trace(tr.d_attn, l, ts.dh, MD * b2));
     {
       ProfScope ps(st, PROF_DIT_BWD_ATTN);
       DGS_TRY(attention_bwd(ts.qkv + sl * 3 * MD, ts.attn + sl * MD, ts.dh,
                             ts.lse + sl * B * w->heads * Np, ts.dsum, ts.big0, B, N, w->heads, st));
     }
+    DGS_TRY(trace(tr.dsum, l, ts.dsum, (size_t)B * w->heads * Np * f4));
+    DGS_TRY(trace(tr.dqkv, l, ts.big0, 3 * MD * b2));
     {
       ProfScope ps(st, PROF_DIT_BWD_ELEM);
       DGS_TRY(colsum_bf16(ts.big0, M, 3 * D, g->qkv_b + l * LS, st));
@@ -651,14 +670,16 @@ int dgs_dit_backward_ex(const dgs_dit_weights* w, const dgs_dit_weights_t* wT, c
       ProfScope ps(st, PROF_DIT_BWD_DGRAD);
       DGS_TRY(dgrad(ts.big0, (const __nv_bfloat16*)wT->qkv_wT + (size_t)l * 3 * D * D, ts.dh, M, D, 3 * D, EPI_BIAS_BF16, nullptr));
     }
+    DGS_TRY(trace(tr.dh1, l, ts.dh, MD * b2));
     {
       ProfScope ps(st, PROF_DIT_BWD_ELEM);
       DGS_TRY(ln_modulate_bwd(x_in, ts.dh, 0, nullptr, m + D, mod_stride, B, N, 0, N, D, 1e-6f, ts.dx, 1, dm, dm + D, nullptr, ts.ln_stats, st));
+      DGS_TRY(trace(tr.dx, l, ts.dx, MD * f4));
       // this block's adaLN linear (6w x w, a third of the block's parameters): d mod_l is complete now, so its weight /
       // bias gradient is produced HERE -- every gradient of block l is final at this point and its all-reduce can start
       // while blocks l-1 .. 0 are still being differentiated (block_done event); d silu(c) accumulates across blocks
       DGS_TRY(skinny_linear_bwd(ws.c, w->adaln_w + (size_t)l * 6 * D * D, dm, mod_stride, B, 6 * D, D, 1, g->adaln_w + l * LS,
-                                g->adaln_b + l * LS, ts.dcond, st));
+                                g->adaln_b + l * LS, ts.dcond, ts.skb_part, st));
     }
     if (done_ev && done_ev[l]) DGS_CUDA_OK(cudaEventRecord((cudaEvent_t)done_ev[l], st));
   }
@@ -682,13 +703,13 @@ int dgs_dit_backward_ex(const dgs_dit_weights* w, const dgs_dit_weights_t* wT, c
     segs.tail_rows[0] = 2 * D; segs.tail_dW[0] = g->ups_adaln_w; segs.tail_db[0] = g->ups_adaln_b;
     segs.tail_rows[1] = 2 * D; segs.tail_dW[1] = g->dec_adaln_w; segs.tail_db[1] = g->dec_adaln_b;
     DGS_TRY(skinny_linear_bwd_segs(ws.c, w->adaln_w + (size_t)L * 6 * D * D, ts.dmod + (size_t)L * 6 * D, mod_stride, B, 4 * D, D,
-                                   1, segs, dsc, st));
+                                   1, segs, dsc, ts.skb_part, st));
   }
   DGS_TRY(silu_bwd_inplace(dsc, ws.c, B * D, st));
-  DGS_TRY(skinny_linear_bwd(ws.temb1, w->t2_w, dsc, D, B, D, D, 0, g->t2_w, g->t2_b, dt1, st));
+  DGS_TRY(skinny_linear_bwd(ws.temb1, w->t2_w, dsc, D, B, D, D, 0, g->t2_w, g->t2_b, dt1, ts.skb_part, st));
   DGS_TRY(skinny_linear(ws.temb0, w->t0_w, w->t0_b, pre1, B, D, 256, 0, 0, st));
   DGS_TRY(silu_bwd_inplace(dt1, pre1, B * D, st));
-  DGS_TRY(skinny_linear_bwd(ws.temb0, w->t0_w, dt1, D, B, D, 256, 0, g->t0_w, g->t0_b, nullptr, st));
+  DGS_TRY(skinny_linear_bwd(ws.temb0, w->t0_w, dt1, D, B, D, 256, 0, g->t0_w, g->t0_b, nullptr, nullptr, st));
   if (done_ev && done_ev[L]) DGS_CUDA_OK(cudaEventRecord((cudaEvent_t)done_ev[L], st));
   return DGS_OK;
 }

@@ -343,7 +343,9 @@ __global__ void __launch_bounds__(256) colsum_kernel(const __nv_bfloat16* __rest
 // ---------------------------------------------------------------------------------------------------------------
 // Backward of the skinny linear  out[b, n] = a[b, :] . W[n, :] + bias[n],  a = act_in(in)  (skinny_linear_kernel):
 //   dW[n, k] = sum_b dout[b, n] a[b, k]     dbias[n] = sum_b dout[b, n]     da[b, k] += sum_n dout[b, n] W[n, k]
-// One CTA per 256 output rows n; a thread owns 4 consecutive k.  W is read once, dW written once.
+// One CTA per SKB_ROWS output rows n; a thread owns 4 consecutive k.  W is read once, dW written once.  Each CTA writes
+// its partial da to part[cta] and skinny_da_reduce_kernel adds the partials into da in CTA order, so da does not depend
+// on the order in which the CTAs finish (fp32 atomics did: run-to-run noise in every gradient behind da).
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int SKB_MAXB = 8, SKB_ROWS = 128;
 __device__ __forceinline__ float silu_f(float v) { return v / (1.0f + __expf(-v)); }
@@ -351,7 +353,7 @@ __device__ __forceinline__ float silu_f(float v) { return v / (1.0f + __expf(-v)
 __global__ void __launch_bounds__(256) skinny_linear_bwd_kernel(const float* __restrict__ in, const float* __restrict__ W,
                                                                 const float* __restrict__ dout, int ldo, int B, int N,
                                                                 int K, int act_in, SkinnySegs segs,
-                                                                float* __restrict__ da) {
+                                                                float* __restrict__ part) {
   extern __shared__ float sm[];
   float* s_a = sm;               // [B, K]
   float* s_do = sm + B * K;      // [B, SKB_ROWS]
@@ -407,16 +409,23 @@ __global__ void __launch_bounds__(256) skinny_linear_bwd_kernel(const float* __r
       }
       *reinterpret_cast<float4*>(dW + (size_t)r * K + k) = g4;
     }
-    if (da) {
+    if (part) {
+      float* pc = part + (size_t)blockIdx.x * B * K;
 #pragma unroll
       for (int b = 0; b < SKB_MAXB; b++) {
-        if (b < B) {
-#pragma unroll
-          for (int e = 0; e < 4; e++) atomicAdd(da + (size_t)b * K + k + e, acc[b][e]);
-        }
+        if (b < B) *reinterpret_cast<float4*>(pc + (size_t)b * K + k) = make_float4(acc[b][0], acc[b][1], acc[b][2], acc[b][3]);
       }
     }
   }
+}
+
+// da[i] += sum_c part[c][i], c = 0 .. n_part-1 in order (i < n = B*K)
+__global__ void skinny_da_reduce_kernel(const float* __restrict__ part, int n_part, int n, float* __restrict__ da) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float s = 0.f;
+  for (int c = 0; c < n_part; c++) s += part[(size_t)c * n + i];
+  da[i] += s;
 }
 
 // dpre = dpost * silu'(pre)  (elementwise, in place on dpost)
@@ -623,8 +632,9 @@ int ln_modulate_bwd(const float* x, const void* dh, int dh_is_f32, const float* 
 }
 
 int skinny_linear_bwd_segs(const float* in, const float* W, const float* dout, int ldo, int B, int N, int K, int act_in,
-                           const SkinnySegs& segs, float* da, cudaStream_t st) {
+                           const SkinnySegs& segs, float* da, float* part, cudaStream_t st) {
   DGS_REQUIRE(B >= 1 && B <= SKB_MAXB && K % 4 == 0, "skinny_linear_bwd: bad shape B=%d K=%d (B <= 8)", B, K);
+  DGS_REQUIRE(!da || part, "skinny_linear_bwd: da needs the partial-sum scratch");
   DGS_REQUIRE(segs.seg_rows % SKB_ROWS == 0 && segs.tail_rows[0] % SKB_ROWS == 0 &&
                   segs.seg_rows * segs.n_seg + segs.tail_rows[0] + segs.tail_rows[1] == N,
               "skinny_linear_bwd: segments must be multiples of %d rows and cover N", SKB_ROWS);
@@ -635,19 +645,26 @@ int skinny_linear_bwd_segs(const float* in, const float* W, const float* dout, i
     configured = true;
   }
   DGS_REQUIRE(smem <= 96 * 1024, "skinny_linear_bwd: B*K too large");
-  skinny_linear_bwd_kernel<<<ceil_div(N, SKB_ROWS), 256, smem, st>>>(in, W, dout, ldo, B, N, K, act_in, segs, da);
+  const int n_part = ceil_div(N, SKB_ROWS);
+  skinny_linear_bwd_kernel<<<n_part, 256, smem, st>>>(in, W, dout, ldo, B, N, K, act_in, segs, da ? part : nullptr);
   DGS_POST_LAUNCH();
+  if (da) {
+    skinny_da_reduce_kernel<<<ceil_div(B * K, 256), 256, 0, st>>>(part, n_part, B * K, da);
+    DGS_POST_LAUNCH();
+  }
   return DGS_OK;
 }
 
+size_t skinny_linear_bwd_part_floats(int B, int N, int K) { return (size_t)ceil_div(N, SKB_ROWS) * B * K; }
+
 int skinny_linear_bwd(const float* in, const float* W, const float* dout, int ldo, int B, int N, int K, int act_in,
-                      float* dW, float* dbias, float* da, cudaStream_t st) {
+                      float* dW, float* dbias, float* da, float* part, cudaStream_t st) {
   SkinnySegs segs;
   segs.seg_rows = N; segs.n_seg = 1; segs.seg_stride = 0; segs.dW0 = dW; segs.db0 = dbias;
   if (N % SKB_ROWS) {  // a single ragged segment: express it as a tail (no alignment requirement on the last one)
     segs.seg_rows = 0; segs.n_seg = 0; segs.tail_rows[0] = 0; segs.tail_rows[1] = N; segs.tail_dW[1] = dW; segs.tail_db[1] = dbias;
   }
-  return skinny_linear_bwd_segs(in, W, dout, ldo, B, N, K, act_in, segs, da, st);
+  return skinny_linear_bwd_segs(in, W, dout, ldo, B, N, K, act_in, segs, da, part, st);
 }
 
 int silu_bwd_inplace(float* d, const float* pre, int n, cudaStream_t st) {

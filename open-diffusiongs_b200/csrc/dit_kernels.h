@@ -104,11 +104,13 @@ struct SkinnySegs {
   float* tail_dW[2] = {nullptr, nullptr}; float* tail_db[2] = {nullptr, nullptr};
 };
 int colsum_bf16(const __nv_bfloat16* in, int M, int C, float* colsum, cudaStream_t st);
+// da (optional) += dout W, summed in a fixed order through `part`, a scratch of skinny_linear_bwd_part_floats(B, N, K)
 int skinny_linear_bwd_segs(const float* in, const float* W, const float* dout, int ldo, int B, int N, int K, int act_in,
-                           const SkinnySegs& segs, float* da, cudaStream_t st);
+                           const SkinnySegs& segs, float* da, float* part, cudaStream_t st);
+size_t skinny_linear_bwd_part_floats(int B, int N, int K);
 // dout [B, ldo] (row stride ldo >= N): rows n of this linear are columns [0, N) of dout
 int skinny_linear_bwd(const float* in, const float* W, const float* dout, int ldo, int B, int N, int K, int act_in,
-                      float* dW, float* dbias, float* da, cudaStream_t st);
+                      float* dW, float* dbias, float* da, float* part, cudaStream_t st);
 int silu_bwd_inplace(float* d, const float* pre, int n, cudaStream_t st);
 int gaussians_epilogue_bwd(const float* gs_tok, const float* img_gs, const float* ray_d, const float* dxyz,
                            const float* dfeatures, const float* dscaling, const float* drotation, const float* dopacity,

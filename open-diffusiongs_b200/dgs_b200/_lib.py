@@ -52,8 +52,15 @@ class DitWeightsFp8(C.Structure):  # dgs_dit_weights_fp8
 FP8_EPI_BIAS_BF16, FP8_EPI_GATE_RESID_F32, FP8_EPI_F32, FP8_EPI_BIAS_GELU_E4M3 = 0, 2, 3, 6  # dgs_gemm_fp8 epi
 
 
+BWD_TRACE_FIELDS = ("dx", "dx_mid", "d_fc2_out", "du_pre", "dh2", "d_proj_out", "d_attn", "dsum", "dqkv", "dh1")
+
+
+class DitBwdTrace(C.Structure):  # dgs_dit_bwd_trace
+    _fields_ = [(n, C.c_void_p) for n in BWD_TRACE_FIELDS]
+
+
 class DitBwdOpts(C.Structure):  # dgs_dit_bwd_opts
-    _fields_ = [("block_done", C.POINTER(C.c_void_p))]
+    _fields_ = [("block_done", C.POINTER(C.c_void_p)), ("trace", C.POINTER(DitBwdTrace))]
 
 
 class RenderMse(C.Structure):  # dgs_render_mse

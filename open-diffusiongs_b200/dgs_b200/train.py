@@ -77,6 +77,7 @@ class DitTrainer:
         self._micro = 0           # backward passes since the last optimizer step
         self._reduced = False     # the overlapped all-reduce of this step has been issued
         self._events = None
+        self._trace = None        # (names, dict) armed by trace_backward for the next backward
         self._group = gradient_group()  # CTA-capped communicator for the gradient exchange (None: default group / 1 rank)
         self._grads = self._grad_struct()
         self.anchor = torch.zeros(1, device=dev, requires_grad=True)  # makes autograd call our backward
@@ -219,6 +220,36 @@ class DitTrainer:
             check(_lib.lib().dgs_dit_export_ends(C.byref(w), B, V, H, W, self.train_mode, self._state.data_ptr(),
                                                  ws.data_ptr(), ws.numel(), *args, _stream(dev)))
         return out
+
+    def trace_backward(self, names=_lib.BWD_TRACE_FIELDS):
+        """Arms the next backward to read out its per-block gradients (dgs_dit_bwd_opts.trace) and returns a dict that
+        this backward fills with {name: tensor} for `names` out of BWD_TRACE_FIELDS, stacked over the layers (M = B*N
+        rows as [B, N]): dx [L+1, B, N, width] fp32 (dx[l]: the gradient of the residual stream entering block l,
+        dx[L]: the one the heads hand to the blocks), dx_mid [L, B, N, width] fp32, dsum [L, B, heads, round_up(N, 128)]
+        fp32, du_pre [L, B, N, 4*width] bf16, dqkv [L, B, N, 3*width] bf16 and d_fc2_out, dh2, d_proj_out, d_attn, dh1
+        [L, B, N, width] bf16.  In both train modes; one call traces one backward."""
+        unknown = set(names) - set(_lib.BWD_TRACE_FIELDS)
+        if unknown:
+            raise ValueError(f"unknown backward trace tensors {sorted(unknown)}; expected a subset of {_lib.BWD_TRACE_FIELDS}")
+        out = {}
+        self._trace = (tuple(names), out)
+        return out
+
+    def _take_trace(self, B, V, H, W):
+        """The armed trace's buffers for a backward at shape (B, V, H, W) -> DitBwdTrace (None: not armed); disarms."""
+        if self._trace is None:
+            return None
+        names, out = self._trace
+        self._trace = None
+        c = self.model.cfg
+        L, D = c.num_layers, c.width
+        N = c.n_gaussians + V * (H // c.patch_size) * (W // c.patch_size)
+        shapes = dict(dx=(L + 1, B, N, D), du_pre=(L, B, N, 4 * D), dqkv=(L, B, N, 3 * D),
+                      dsum=(L, B, D // c.dim_heads, (N + 127) // 128 * 128))
+        for k in names:
+            dt = torch.float32 if k in ("dx", "dx_mid", "dsum") else torch.bfloat16
+            out[k] = torch.empty(shapes.get(k, (L, B, N, D)), dtype=dt, device=self.master.device)
+        return _lib.DitBwdTrace(**{k: out[k].data_ptr() for k in names})
 
     def zero_grad(self):
         self.arena.zero_()
@@ -375,12 +406,17 @@ class _DitFunction(torch.autograd.Function):
               z(d_opacity, B, P, 1)]
         dout = DitOutGrads(*(g.data_ptr() for g in gs))
         opts = tr._bwd_opts()
+        overlapped = opts is not None
+        trace = tr._take_trace(B, V, H, W)
+        if trace is not None:
+            opts = opts or DitBwdOpts()
+            opts.trace = C.pointer(trace)
         with torch.cuda.device(dev):
             check(_lib.lib().dgs_dit_backward_ex(C.byref(w), C.byref(tr._wT), C.byref(io), C.byref(dout),
                                                  C.byref(tr._grads), None if opts is None else C.byref(opts),
                                                  ws.data_ptr(), nbytes, _stream(dev)))
         ctx.keep = None
-        tr._end_backward(overlapped=opts is not None)
+        tr._end_backward(overlapped=overlapped)
         # parameter gradients were written straight into the arena (p.grad views); nothing to hand to autograd
         return None, None, None, None, None, torch.zeros_like(tr.anchor)
 

@@ -197,6 +197,133 @@ def dit_block_matched(blk, x, mod, feed=None, rounding=True, softmax_scale=None,
     return out
 
 
+# named defects of the block backward (see dit_block_backward_matched); tests/test_dit_block_bwd_power_cpu.py shows the GPU
+# checks would see each one; the product path never sets one
+BWD_DEFECTS = ("gate_sample0_everywhere", "wgrad_tail_dropped", "last_key_dropped", "gelu_erf_grad", "ln_bwd_no_mean",
+               "dscale_sample1_into_0")
+
+
+def _gelu_tanh_grad(x):
+    k0, k1 = math.sqrt(2.0 / math.pi), 0.044715
+    t = torch.tanh(k0 * (x + k1 * x ** 3))
+    return 0.5 * (1.0 + t) + 0.5 * x * (1.0 - t * t) * k0 * (1.0 + 3.0 * k1 * x * x)
+
+
+def _gelu_erf_grad(x):
+    return 0.5 * (1.0 + torch.erf(x / math.sqrt(2.0))) + x * torch.exp(-0.5 * x * x) / math.sqrt(2.0 * math.pi)
+
+
+@torch.no_grad()
+def dit_block_backward_matched(blk, fwd, mod, c, dx_out, feed=None, rounding=True, head_chunk=None, defects=()):
+    """Backward of one DiTBlock in fp64 from the forward tensors `fwd` and the gradient dx_out [B, N, w] of its output,
+    rounding to bf16 where the backward kernels round:
+      d_fc2_out = bf16(gate_mlp dx) and d_proj_out = bf16(gate_msa dx_mid) (gate_bwd);
+      du_pre = bf16((d_fc2_out W2) gelu'(u_pre)) with the tanh GELU (the fc2 dgrad's dGELU epilogue);
+      dh2, d_attn, dh1 = bf16 of the fc1 / attn.proj / qkv dgrads, the weights in bf16 (the transposed copies);
+      attention: P = exp2(S log2(e) / 8 - lse2) from the forward's lse2, Dsum = rowsum(attn d_attn), dV = bf16(P)^T dO,
+      dS = P (dP - Dsum) / 8 rounded to bf16 before dQ = dS K and dK = dS^T Q, dqkv stored in bf16.
+    The weight and bias gradients are fp64 sums of the same bf16 operands the kernels multiply; dx_mid and dx (fp32 in the
+    kernels) are not rounded.  rounding=False: the plain fp64 backward (then `fwd` should be the plain forward's).
+
+    blk: a DiTBlock-shaped module (its fp32 weights are read); fwd: {x, x_mid, h1, qkv, attn, lse, proj_out, h2, u_pre, u,
+    fc2_out} as dgs_dit_export_state / dit_block_matched give them (lse [B, heads, >= N] in log2 units); mod [B, 6w] the
+    block's adaLN modulation, c [B, w] the conditioning before the SiLU.  feed: {name: tensor} replaces this function's
+    own value of an intermediate gradient by the given one before it is used downstream (teacher forcing), keys out of
+    d_fc2_out, du_pre, dh2, dx_mid, d_proj_out, d_attn, dqkv, dh1.  head_chunk: heads per attention pass (bounds the fp64
+    score memory).  defects: names out of BWD_DEFECTS.
+    Returns every gradient (fp64): d_fc2_out, du_pre, dh2, dx_mid, d_proj_out, d_attn, dsum [B, heads, N], dqkv, dh1, dx,
+    dmod [B, 6w], and the parameter gradients under the block's parameter names (attn.qkv.weight, ...,
+    adaLN_modulation.1.bias)."""
+    feed = feed or {}
+    rnd = _bf16 if rounding else (lambda t: t)
+    f = {k: v.double() for k, v in fwd.items()}
+    dx = dx_out.double()
+    B, N, D = dx.shape
+    heads = blk.attn.num_heads if hasattr(blk.attn, "num_heads") else D // 64
+    hd = D // heads
+    scale = hd ** -0.5
+    mod = mod.double()
+    s1, c1, g1, s2, c2, g2 = (m[:, None, :] for m in mod.chunk(6, dim=1))
+    W = lambda lin: rnd(lin.weight.detach().double())  # noqa: E731
+    get = lambda k, v: feed[k].double() if k in feed else v  # noqa: E731
+    M = B * N
+    keep = (M // 128) * 128 if "wgrad_tail_dropped" in defects else M
+    out, dmod = {}, torch.zeros(B, 6 * D, dtype=torch.float64, device=dx.device)
+
+    def linear_grads(name, dy, a):  # dW = dy^T a, db = sum dy over the rows
+        dy2, a2 = dy.reshape(M, -1), a.reshape(M, -1)
+        out[name + ".weight"] = dy2[:keep].t() @ a2[:keep]
+        out[name + ".bias"] = dy2.sum(0)
+
+    def gate(g, t):
+        return rnd((g[:1] if "gate_sample0_everywhere" in defects else g) * t)
+
+    def ln_modulate_bwd(x, dh, c_):  # -> dx, dshift, dscale of h = LN(x; 1e-6) (1 + c_) + shift
+        mu = x.mean(-1, keepdim=True)
+        rstd = 1.0 / torch.sqrt((x - mu).pow(2).mean(-1, keepdim=True) + 1e-6)
+        xh = (x - mu) * rstd
+        dxh = dh * (1 + c_)
+        m1 = 0.0 if "ln_bwd_no_mean" in defects else dxh.mean(-1, keepdim=True)
+        dscale = (dh * xh).sum(1)
+        if "dscale_sample1_into_0" in defects and B > 1:
+            dscale = torch.cat([dscale[:1] + dscale[1:2], torch.zeros_like(dscale[1:2]), dscale[2:]])
+        return rstd * (dxh - m1 - xh * (dxh * xh).mean(-1, keepdim=True)), dh.sum(1), dscale
+
+    # -- MLP branch: x_out = x_mid + gate_mlp * fc2(gelu(fc1(h2)))
+    out["d_fc2_out"] = gate(g2, dx)
+    d_fc2 = get("d_fc2_out", out["d_fc2_out"])
+    dmod[:, 5 * D:] = (dx * f["fc2_out"]).sum(1)
+    linear_grads("mlp.fc2", d_fc2, f["u"])
+    dgelu = _gelu_erf_grad if "gelu_erf_grad" in defects else _gelu_tanh_grad
+    out["du_pre"] = rnd((d_fc2 @ W(blk.mlp.fc2)) * dgelu(f["u_pre"]))
+    du_pre = get("du_pre", out["du_pre"])
+    linear_grads("mlp.fc1", du_pre, f["h2"])
+    out["dh2"] = rnd(du_pre @ W(blk.mlp.fc1))
+    ddx, dmod[:, 3 * D:4 * D], dmod[:, 4 * D:5 * D] = ln_modulate_bwd(f["x_mid"], get("dh2", out["dh2"]), c2)
+    out["dx_mid"] = dx + ddx
+    dx_mid = get("dx_mid", out["dx_mid"])
+    # -- attention branch: x_mid = x_in + gate_msa * proj(attention(qkv(h1)))
+    out["d_proj_out"] = gate(g1, dx_mid)
+    d_proj = get("d_proj_out", out["d_proj_out"])
+    dmod[:, 2 * D:3 * D] = (dx_mid * f["proj_out"]).sum(1)
+    linear_grads("attn.proj", d_proj, f["attn"])
+    out["d_attn"] = rnd(d_proj @ W(blk.attn.proj))
+    d_attn = get("d_attn", out["d_attn"])
+    split = lambda t: t.reshape(B, N, heads, hd).permute(0, 2, 1, 3)  # noqa: E731  [B, H, N, hd]
+    q, k, v = f["qkv"].reshape(B, N, 3, heads, hd).permute(2, 0, 3, 1, 4)
+    o, do = split(f["attn"]), split(d_attn)
+    dsum = (o * do).sum(-1)
+    out["dsum"] = dsum
+    lse2 = f["lse"][:, :, :N]
+    dqkv = torch.empty(3, B, heads, N, hd, dtype=torch.float64, device=dx.device)
+    step = head_chunk or heads
+    for h0 in range(0, heads, step):
+        hs = slice(h0, h0 + step)
+        s = q[:, hs] @ k[:, hs].transpose(-1, -2)
+        p = torch.exp2(s * (scale / math.log(2.0)) - lse2[:, hs, :, None])
+        del s
+        ds = p * (do[:, hs] @ v[:, hs].transpose(-1, -2) - dsum[:, hs, :, None]) * scale
+        dqkv[2, :, hs] = rnd(p).transpose(-1, -2) @ do[:, hs]
+        del p
+        ds = rnd(ds)
+        dqkv[0, :, hs] = ds @ k[:, hs]
+        dqkv[1, :, hs] = ds.transpose(-1, -2) @ q[:, hs]
+        del ds
+    if "last_key_dropped" in defects:
+        dqkv[1:, :, :, N - 1] = 0.0
+    out["dqkv"] = rnd(dqkv.permute(1, 3, 0, 2, 4).reshape(B, N, 3 * D))
+    dqkv = get("dqkv", out["dqkv"])
+    linear_grads("attn.qkv", dqkv, f["h1"])
+    out["dh1"] = rnd(dqkv @ W(blk.attn.qkv))
+    ddx, dmod[:, :D], dmod[:, D:2 * D] = ln_modulate_bwd(f["x"], get("dh1", out["dh1"]), c1)
+    out["dx"] = dx_mid + ddx
+    # -- adaLN: mod = Linear(silu(c))
+    out["dmod"] = dmod
+    out["adaLN_modulation.1.weight"] = dmod.t() @ F.silu(c.double())
+    out["adaLN_modulation.1.bias"] = dmod.sum(0)
+    return out
+
+
 # ---- the stages on either side of the blocks, in fp64 and differentiable (fp64 autograd gives their backward) ----
 # matched=True rounds where the kernels round; plain fp64 otherwise.  `defects` plants a named defect (END_DEFECTS) so
 # that tests/test_dit_ends_power_cpu.py can show the GPU checks would see it; the product path never sets one.

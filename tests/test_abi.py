@@ -34,6 +34,22 @@ def test_library_exports_every_declared_symbol():
     assert sorted(_lib.EXPORTED) == names
 
 
+def _struct_fields(name):
+    """Field names of the typedef struct `name` in include/dgs_b200.h, in declaration order."""
+    txt = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "dgs_b200.h")).read(), flags=re.S)
+    body = re.search(r"typedef struct \{([^{}]*)\}\s*" + name + r"\s*;", txt).group(1)
+    return [m.group(1) for decl in body.split(";") if (m := re.search(r"(\w+)\s*$", decl.strip()))]
+
+
+def test_backward_trace_structs_mirror_the_header():
+    """dgs_b200._lib's ctypes mirrors of dgs_dit_bwd_trace / dgs_dit_bwd_opts: same fields, same order, all pointers."""
+    assert _struct_fields("dgs_dit_bwd_trace") == [n for n, _ in _lib.DitBwdTrace._fields_] == list(_lib.BWD_TRACE_FIELDS)
+    assert _struct_fields("dgs_dit_bwd_opts") == [n for n, _ in _lib.DitBwdOpts._fields_] == ["block_done", "trace"]
+    assert ctypes.sizeof(_lib.DitBwdTrace) == len(_lib.BWD_TRACE_FIELDS) * ctypes.sizeof(ctypes.c_void_p)
+    assert _lib.DitBwdOpts.trace.offset == ctypes.sizeof(ctypes.c_void_p)
+    assert not _lib.DitBwdOpts().trace  # zero-filled: no trace unless one is attached
+
+
 def test_version_and_error_string():
     _ensure_built()
     L = _lib.lib()
@@ -78,6 +94,20 @@ def test_argument_validation_without_gpu():
     assert ends(nbytes=ws_bytes - 1, mod=fake) == 1 and b"workspace too small" in L.dgs_last_error()
     assert ends(ws=None, dx0=fake) == 1 and b"workspace too small" in L.dgs_last_error()
     assert ends(mode=7, dmod=fake) == 1 and b"train_mode" in L.dgs_last_error()
+    # a backward with the trace armed still rejects bad arguments before any device work (the trace is never read)
+    trace = _lib.DitBwdTrace(**{k: 256 for k in _lib.BWD_TRACE_FIELDS})
+    opts = _lib.DitBwdOpts(trace=ctypes.pointer(trace))
+    io = _lib.DitIO(B=9, V=4, H=32, W=32, train_state=256, train_mode=STORE)
+    wT = _lib.DitWeightsT(**{n: 256 for n, _ in _lib.DitWeightsT._fields_})
+    dout = _lib.DitOutGrads(*([256] * 5))
+    grads = _lib.DitGrads()
+
+    def backward(io):
+        return L.dgs_dit_backward_ex(ctypes.byref(w), ctypes.byref(wT), ctypes.byref(io), ctypes.byref(dout),
+                                     ctypes.byref(grads), ctypes.byref(opts), fake, 1 << 40, None)
+    assert backward(io) == 1 and b"batch 9 > 8" in L.dgs_last_error()
+    io.B, io.train_state = 1, None
+    assert backward(io) == 1 and b"train_state is NULL" in L.dgs_last_error()
     w.width = 512
     assert export(STORE, 0, x=fake) == 1 and b"width" in L.dgs_last_error()
     assert ends(x_pre=fake) == 1 and b"width" in L.dgs_last_error()
