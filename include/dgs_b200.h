@@ -506,6 +506,40 @@ int dgs_ssim_backward(int n, int H, int W, const float* x, const float* y, const
                       float* d_x, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * B2d. Mesh extraction after the sampler loop: GaussianModel.extract_fields / extract_mesh
+ * (diffusionGS/models/gsrenderer/gs_core.py:786-869).
+ * ---------------------------------------------------------------------------------------------- */
+/* The block-truncated opacity field of extract_fields(resolution, num_blocks, relax_ratio).  Inputs are the RAW fp32
+ * tensors xyz [P,3], scaling [P,3], rotation [P,4] (not normalised), opacity [P,1]; scale_modifier is 1 when the model
+ * has none; center (device fp32 [3]) and scale are the caller's mesh_center and fp32 mesh_scale; lin (device fp32
+ * [resolution]) is torch.linspace(-1, 1, resolution), whose values decide membership.  Each axis is cut into chunks of
+ * resolution / num_blocks points (the last one shorter); a Gaussian belongs to a block of three chunks iff on every axis
+ * vmin < (x - center) * scale < vmax, with vmin / vmax the chunk's first / last coordinate -/+ fp32((2 / num_blocks) *
+ * relax_ratio), all fp32 as in the reference.  occ [resolution^3] (x-major, fp32) = per point the sum over the block's
+ * Gaussians, in Gaussian order, of opacity * exp(power) (0 where power > 0); blocks without Gaussians are 0.  The sum
+ * order is fixed: the result does not change from run to run.
+ * block_counts (NULL, or device int [chunks^3]) receives each block's number of Gaussians; *num_pairs (NULL or host)
+ * the total.  scratch_alloc is called once for per-Gaussian and per-block scratch and, after the one host sync that
+ * reads the pair count, once more for the pairs (16 B each plus the sort's temporary storage); both are free after
+ * the call.  More than 2^31 - 1 pairs is DGS_ERR_OVERFLOW. */
+int dgs_mesh_field(int P, const float* xyz, const float* scaling, const float* rotation, const float* opacity,
+                   float scale_modifier, const float* center, float scale, int resolution, int num_blocks,
+                   double relax_ratio, const float* lin, float* occ, int* block_counts, long long* num_pairs,
+                   dgs_alloc_fn scratch_alloc, void* scratch_user, void* stream);
+/* Marching cubes over field [nx, ny, nz] (C order, fp32, every size >= 2).  A grid point is inside iff value > iso; every
+ * grid edge with exactly one inside end gets one vertex, at a + (iso - va) / (vb - va) (b - a) in index coordinates,
+ * shared by the triangles of the (up to four) voxels around it, so the mesh is welded.  Vertices are ordered by owning
+ * edge (grid point in C order, then axis x, y, z), triangles by voxel, then case-table order (mc_tables.h, generated by
+ * gen_mc_tables.py); each triangle's right-hand-rule normal points from inside to outside.  On faces with two diagonally
+ * opposite inside corners the inside corners are kept apart, so the surface is closed.
+ * alloc is called once for scratch (10 B per grid point plus the scans' temporary storage, free after the call), then,
+ * after the one host sync that reads the totals, for *vertices (fp32 [V, 3]) and *triangles (int32 [F, 3]) when V > 0.
+ * An empty surface returns V = F = 0 and NULL outputs. */
+int dgs_marching_cubes(const float* field, int nx, int ny, int nz, float iso, dgs_alloc_fn alloc, void* alloc_user,
+                       float** vertices, int** triangles, long long* num_vertices, long long* num_triangles,
+                       void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * B3. The elementwise callers either side of the path.
  * ---------------------------------------------------------------------------------------------- */
 /* TransformInput (diffusionGS/systems/utils.py:621-757, patch_size=None): per-pixel world-space rays.

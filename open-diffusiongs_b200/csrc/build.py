@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.abspath(os.path.join(HERE, "..", ".."))
 OUT_DIR = os.path.join(HERE, "..", "dgs_b200", "lib")
 OUT = os.path.abspath(os.path.join(OUT_DIR, "libdgs_b200.so"))
-SOURCES = ["core.cu", "raster.cu", "dit_misc.cu", "gemm_sm90.cu", "attention_sm90.cu", "attention_bwd_sm90.cu", "dit_bwd_misc.cu", "dit_api.cu", "diffusion_steps.cu", "lpips.cu", "ssim.cu"]
+SOURCES = ["core.cu", "raster.cu", "dit_misc.cu", "gemm_sm90.cu", "attention_sm90.cu", "attention_bwd_sm90.cu", "dit_bwd_misc.cu", "dit_api.cu", "diffusion_steps.cu", "lpips.cu", "ssim.cu", "mesh.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-O3"]
 

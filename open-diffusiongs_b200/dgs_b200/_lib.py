@@ -187,6 +187,10 @@ def lib():
         L.dgs_quantize_rows_e4m3.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp]
         L.dgs_ln_modulate_fp8.argtypes = [vp, vp, vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_float, vp]
         L.dgs_gemm_fp8.argtypes = [vp] * 8 + [C.c_int] * 7 + [vp]
+        L.dgs_mesh_field.argtypes = [C.c_int, vp, vp, vp, vp, C.c_float, vp, C.c_float, C.c_int, C.c_int, C.c_double,
+                                     vp, vp, vp, C.POINTER(C.c_longlong), ALLOC_FN, vp, vp]
+        L.dgs_marching_cubes.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_float, ALLOC_FN, vp, C.POINTER(C.c_void_p),
+                                         C.POINTER(C.c_void_p), C.POINTER(C.c_longlong), C.POINTER(C.c_longlong), vp]
         _lib = L
     return _lib
 
@@ -225,4 +229,5 @@ EXPORTED = [  # every symbol include/dgs_b200.h declares (checked by tests/test_
     "dgs_dit_export_ends", "dgs_lpips_workspace_bytes", "dgs_lpips_state_bytes", "dgs_lpips_forward", "dgs_lpips_backward",
     "dgs_ssim_workspace_bytes", "dgs_ssim_state_bytes", "dgs_ssim_forward", "dgs_ssim_backward",
     "dgs_dit_workspace_bytes_fp8", "dgs_dit_forward_fp8", "dgs_quantize_rows_e4m3", "dgs_ln_modulate_fp8", "dgs_gemm_fp8",
+    "dgs_mesh_field", "dgs_marching_cubes",
 ]

@@ -105,8 +105,9 @@ deferred_gaussian_render = batched_gaussian_render  # reference name (gs_core.py
 
 
 class GaussianModel:
-    """Minimal parameter holder with the reference's activations (gs_core.py:323-373, 545-575); the
-    PLY / mesh / filter methods of the reference class are out of scope."""
+    """Parameter holder with the reference's activations (gs_core.py:323-373, 545-575), its post-sampler filters
+    (386-475), PLY export and import (577-785) and mesh extraction (786-869): `extract_fields` and `extract_mesh` run
+    on the sm_90a kernels of dgs_b200.mesh and need CUDA tensors."""
 
     def __init__(self, sh_degree: int, scaling_modifier=None):
         self.sh_degree = sh_degree
@@ -148,7 +149,12 @@ class GaussianModel:
         return self._features_dc
 
 
-    # ---- post-processing after the sampler loop: gs_core.py:386-475 filters, 577-713 PLY export ----
+    def get_covariance(self, scaling_modifier=1):
+        """gs_core.py:572-575: (R S)(R S)^T of the scales times scaling_modifier and the raw rotation over its Euclidean
+        norm, as [P, 6] = (xx, xy, xz, yy, yz, zz)."""
+        return _covariance6(scaling_modifier * self.get_scaling, self._rotation)
+
+    # ---- post-processing after the sampler loop: gs_core.py:386-475 filters, 577-785 PLY, 786-869 mesh ----
     def to(self, device):
         for k in ("_xyz", "_features_dc", "_features_rest", "_scaling", "_rotation", "_opacity"):
             v = getattr(self, k)
@@ -246,6 +252,111 @@ class GaussianModel:
             f.write(("\n".join(header) + "\n").encode("ascii"))
             f.write(elements.astype(elements.dtype.newbyteorder("<")).tobytes())
         return path
+
+
+    def load_ply(self, path):
+        """gs_core.py:716-785: the inverse of save_ply (xyz, f_dc, f_rest when sh_degree > 0, raw opacity / log-scale /
+        rotation) into CPU fp32 tensors; read with numpy from binary PLY (plyfile is not installed here)."""
+        import numpy as np
+        v = _read_ply_vertices(path)
+        n = len(v)
+        xyz = np.stack([v["x"], v["y"], v["z"]], axis=1)
+        opacities = np.asarray(v["opacity"])[..., np.newaxis]
+        features_dc = np.stack([v["f_dc_0"], v["f_dc_1"], v["f_dc_2"]], axis=1)[..., np.newaxis]  # [P, 3, 1]
+
+        def group(prefix):
+            names = sorted((k for k in v.dtype.names if k.startswith(prefix)), key=lambda k: int(k.split("_")[-1]))
+            return np.stack([v[k] for k in names], axis=1) if names else np.zeros((n, 0))
+        if self.sh_degree > 0:
+            extra = group("f_rest_")
+            assert extra.shape[1] == 3 * (self.sh_degree + 1) ** 2 - 3
+            extra = extra.reshape(n, 3, (self.sh_degree + 1) ** 2 - 1)
+            self._features_rest = torch.from_numpy(extra.astype(np.float32)).transpose(1, 2).contiguous()
+        else:
+            self._features_rest = None
+        self._xyz = torch.from_numpy(xyz.astype(np.float32))
+        self._features_dc = torch.from_numpy(features_dc.astype(np.float32)).transpose(1, 2).contiguous()
+        self._opacity = torch.from_numpy(opacities.astype(np.float32)).contiguous()
+        self._scaling = torch.from_numpy(group("scale_").astype(np.float32)).contiguous()
+        self._rotation = torch.from_numpy(group("rot").astype(np.float32)).contiguous()
+        return self
+
+    def extract_fields(self, resolution=128, num_blocks=16, relax_ratio=1.5):
+        """gs_core.py:786-852: the opacity field [resolution]^3 (fp32, on the model's CUDA device, indexed [x][y][z]) on
+        the grid linspace(-1, 1, resolution) after normalising the centres to about [-0.9, 0.9]^3; sets mesh_center and
+        mesh_scale.  Each point sums only the Gaussians whose centre lies within relax_ratio block sizes of its block, as
+        the reference does.  With no Gaussians the field is 0 (mesh_center 0, mesh_scale 1)."""
+        from . import mesh as _mesh
+        occ, self.mesh_center, self.mesh_scale = _mesh.opacity_field(
+            self._xyz, self._scaling, self._rotation, self._opacity, self.scaling_modifier, resolution, num_blocks,
+            relax_ratio)
+        return occ
+
+    def extract_mesh(self, density_thresh=0.005, resolution=256, decimate_target=1e5, postprocess=None):
+        """gs_core.py:855-869: extract_fields(resolution, num_blocks=64), marching cubes at density_thresh on the GPU,
+        vertices mapped by v / (resolution - 1) * 2 - 1 (in the normalised frame: not mapped back by mesh_center /
+        mesh_scale, as in the reference) -> dgs_b200.mesh.Mesh (vertices float32 [V, 3], faces int64 [F, 3]).
+        The reference then cleans, remeshes and decimates with pymeshlab; that is not done here: without `postprocess`
+        the raw marching-cubes mesh is returned and `decimate_target` is unused.  `postprocess(vertices, faces,
+        decimate_target) -> (vertices, faces)` runs on the numpy arrays, e.g. a wrapper of the reference's clean_mesh /
+        decimate_mesh."""
+        from . import mesh as _mesh
+        occ = self.extract_fields(resolution, num_blocks=64)
+        return _mesh.extract_mesh(occ, density_thresh, resolution, postprocess, decimate_target)
+
+
+def _covariance6(stds, r):
+    """build_covariance_from_scaling_rotation (gs_core.py:112-147, 324-328) in elementwise fp32 ops."""
+    norm = torch.sqrt(r[:, 0] * r[:, 0] + r[:, 1] * r[:, 1] + r[:, 2] * r[:, 2] + r[:, 3] * r[:, 3])
+    q = r / norm[:, None]
+    w, x, y, z = q[:, 0], q[:, 1], q[:, 2], q[:, 3]
+    R = [[1 - 2 * (y * y + z * z), 2 * (x * y - w * z), 2 * (x * z + w * y)],
+         [2 * (x * y + w * z), 1 - 2 * (x * x + z * z), 2 * (y * z - w * x)],
+         [2 * (x * z - w * y), 2 * (y * z + w * x), 1 - 2 * (x * x + y * y)]]
+    L = [[R[i][j] * stds[:, j] for j in range(3)] for i in range(3)]
+    dot = lambda i, k: (L[i][0] * L[k][0] + L[i][1] * L[k][1]) + L[i][2] * L[k][2]  # noqa: E731
+    return torch.stack([dot(0, 0), dot(0, 1), dot(0, 2), dot(1, 1), dot(1, 2), dot(2, 2)], dim=1)
+
+
+_PLY_TYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short": "i2", "int16": "i2", "ushort": "u2",
+              "uint16": "u2", "int": "i4", "int32": "i4", "uint": "u4", "uint32": "u4", "float": "f4", "float32": "f4",
+              "double": "f8", "float64": "f8"}
+
+
+def _read_ply_vertices(path):
+    """The `vertex` element of a binary PLY whose first element it is, as a numpy structured array."""
+    import numpy as np
+    with open(path, "rb") as f:
+        if f.readline().strip() != b"ply":
+            raise ValueError(f"{path}: not a PLY file")
+        fmt, n, props, in_vertex = None, None, [], False
+        while True:
+            line = f.readline()
+            if not line:
+                raise ValueError(f"{path}: PLY header without end_header")
+            tok = line.decode("ascii").split()
+            if not tok:
+                continue
+            if tok[0] == "end_header":
+                break
+            if tok[0] == "format":
+                fmt = tok[1]
+            elif tok[0] == "element":
+                in_vertex = tok[1] == "vertex" and n is None
+                if in_vertex:
+                    n = int(tok[2])
+                elif n is None:
+                    raise ValueError(f"{path}: the vertex element must come first")
+            elif tok[0] == "property" and in_vertex:
+                if tok[1] == "list":
+                    raise ValueError(f"{path}: list properties in the vertex element are not supported")
+                props.append((tok[2], _PLY_TYPES[tok[1]]))
+        if fmt not in ("binary_little_endian", "binary_big_endian") or n is None:
+            raise ValueError(f"{path}: need a binary PLY with a vertex element (format {fmt})")
+        order = "<" if fmt == "binary_little_endian" else ">"
+        dtype = np.dtype([(name, order + t) for name, t in props])
+        data = np.frombuffer(f.read(dtype.itemsize * n), dtype=dtype, count=n)
+    return data
 
 
 class Renderer(nn.Module):

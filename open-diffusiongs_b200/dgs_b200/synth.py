@@ -58,6 +58,18 @@ def make_gaussians(P, seed=0, dist="trained", extent=1.0):
     return dict(xyz=xyz, features=features, scaling=scaling, rotation=rotation, opacity=opacity)
 
 
+def make_shell_gaussians(P, seed=0, dist="trained", radii=(0.6, 0.45, 0.5), thickness=0.02):
+    """make_gaussians with the centres on a thin ellipsoidal shell (semi-axes `radii`, relative thickness `thickness`):
+    an object-like point set, whose opacity field is a closed surface with empty space inside and out."""
+    g = make_gaussians(P, seed, dist)
+    rng = np.random.default_rng(seed + 7919)
+    d = rng.normal(0, 1, (P, 3))
+    d /= np.linalg.norm(d, axis=1, keepdims=True)
+    r = 1.0 + rng.normal(0, thickness, (P, 1))
+    g["xyz"] = (d * r * np.asarray(radii)).astype(np.float32)
+    return g
+
+
 def activate(g):
     """Host-side activations -> the tensors `GaussianRasterizer.forward` receives."""
     return dict(means3D=g["xyz"], shs=g["features"], scales=np.exp(g["scaling"]),
