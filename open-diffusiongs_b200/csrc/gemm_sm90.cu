@@ -73,14 +73,19 @@ constexpr int BM = 128, BK = 64;
 constexpr int GEMM_THREADS = WS_THREADS;
 
 // OUT_BYTES: element size of the output tile staged in shared memory for the TMA-store epilogue (0: the epilogue
-// writes from registers).  The staging buffer takes what would otherwise be operand stages.
+// writes from registers).  The staging buffer takes what would otherwise be operand stages.  It holds RING column
+// blocks (128 bytes x 64 rows, 8 KB) per consumer warpgroup: the whole 64 x BN fragment, except for a 128 x 256 fp32
+// tile (128 KB staged whole, which would leave two operand stages), which goes out two column blocks at a time and
+// keeps four stages.
 template <int BN, int OUT_BYTES>
 struct GemmCfg {
   static constexpr int SMEM_LIMIT = 227 * 1024;
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int OUT_TILE_BYTES = BM * BN * OUT_BYTES;
+  static constexpr int OUT_BLOCKS = BN * OUT_BYTES / 128;  // column blocks of a warpgroup's fragment
+  static constexpr int RING = OUT_BLOCKS > 4 ? 2 : OUT_BLOCKS;
+  static constexpr int OUT_TILE_BYTES = 2 * RING * 8192;
   static constexpr int EXTRA = 1024 /*align slack*/ + 256 /*barriers*/;
   static constexpr int FIT = (SMEM_LIMIT - EXTRA - OUT_TILE_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = FIT < (BN == 256 ? 4 : 6) ? FIT : (BN == 256 ? 4 : 6);
@@ -172,53 +177,63 @@ constexpr int epi_out_bytes() {
 // makes the fragment writes free of bank conflicts.
 // EPI_GATE_RESID_F32 (in place, no ep.resid) stages gate * (acc + b) and adds it into x with a TMA reduce-add, so x is
 // never read by the SM.  The result is x + round(g * v) rather than fmaf(g, v, x): one more fp32 rounding per update.
-template <int EPI, int BN>
+// RING < the fragment's column blocks: the fragment goes out in batches of RING blocks, each written once the previous
+// batch's stores have read the buffer.
+template <int EPI, int BN, int RING>
 __device__ __forceinline__ void epilogue_tma(const GemmEpilogue& ep, const float (&acc)[BN / 2], uint8_t* stage,
                                              const CUtensorMap* tmC, int m0, int n0, int M, int N, int wg, int wq, int lane) {
   constexpr int OB = epi_out_bytes<EPI>();
-  constexpr int COLS = 128 / OB;  // columns per staging row
+  constexpr int COLS = 128 / OB;            // columns per staging row
+  constexpr int JB = RING * COLS / 8;       // 8-column groups per batch
   const bool leader = wq == 0 && lane == 0;
-  if (leader) bulk_wait_read<0>();  // the stores of this warpgroup's previous tile have read the buffer
-  named_bar_sync(1 + wg, 128);
+  const float* gate_row[2] = {nullptr, nullptr};
+  if (EPI == EPI_GATE_RESID_F32) {
 #pragma unroll
-  for (int i = 0; i < 2; i++) {
-    const int r = 16 * wq + (lane >> 2) + 8 * i;  // row in the warpgroup's 64-row slice; r % 8 == lane / 4
-    const float* gate_row = nullptr;
-    if (EPI == EPI_GATE_RESID_F32) {
-      const int row = min(m0 + r, M - 1);  // rows >= M are clipped by the store, but must not index past the gates
-      gate_row = ep.gate + (size_t)(row / ep.rows_per_sample) * ep.gate_stride;
-    }
-#pragma unroll
-    for (int j = 0; j < BN / 8; j++) {
-      const int n = n0 + 8 * j + 2 * (lane & 3);
-      if (n0 + 8 * j >= N) break;  // N % 32 == 0: whole 8-column groups are in or out
-      float2 v = make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
-      if (ep.bias) {
-        const float2 b = __ldg(reinterpret_cast<const float2*>(ep.bias + n));
-        v.x += b.x; v.y += b.y;
-      }
-      if (EPI == EPI_BIAS_GELU_BF16) { v.x = epi_gelu_tanh(v.x); v.y = epi_gelu_tanh(v.y); }
-      if (EPI == EPI_BIAS_RELU_BF16) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); }
-      if (EPI == EPI_GATE_RESID_F32) {
-        const float2 g = __ldg(reinterpret_cast<const float2*>(gate_row + n));
-        v.x *= g.x; v.y *= g.y;
-      }
-      const int byte = ((8 * j) % COLS + 2 * (lane & 3)) * OB;  // within the 128-byte staging row
-      uint8_t* p = stage + (8 * j / COLS) * 8192 + r * 128 + ((((byte >> 4) ^ (lane >> 2)) << 4) | (byte & 15));
-      if (OB == 2) *reinterpret_cast<uint32_t*>(p) = pack2_bf16(v.x, v.y);
-      else *reinterpret_cast<float2*>(p) = v;
+    for (int i = 0; i < 2; i++) {
+      const int row = min(m0 + 16 * wq + (lane >> 2) + 8 * i, M - 1);  // rows >= M are clipped by the store, but must
+      gate_row[i] = ep.gate + (size_t)(row / ep.rows_per_sample) * ep.gate_stride;  // not index past the gates
     }
   }
-  fence_proxy_async();  // make the generic-proxy writes visible to the TMA unit
-  named_bar_sync(1 + wg, 128);
-  if (leader) {
 #pragma unroll
-    for (int b = 0; b < BN / COLS; b++) {
-      if (n0 + b * COLS >= N) break;
-      if (EPI == EPI_GATE_RESID_F32) tma_reduce_add_2d(tmC, stage + b * 8192, n0 + b * COLS, m0);
-      else tma_store_2d(tmC, stage + b * 8192, n0 + b * COLS, m0);
+  for (int j0 = 0; j0 < BN / 8; j0 += JB) {
+    if (n0 + 8 * j0 >= N) break;
+    if (leader) bulk_wait_read<0>();  // the stores of the previous batch (or tile) have read the buffer
+    named_bar_sync(1 + wg, 128);
+#pragma unroll
+    for (int i = 0; i < 2; i++) {
+      const int r = 16 * wq + (lane >> 2) + 8 * i;  // row in the warpgroup's 64-row slice; r % 8 == lane / 4
+#pragma unroll
+      for (int j = j0; j < j0 + JB; j++) {
+        const int n = n0 + 8 * j + 2 * (lane & 3);
+        if (n0 + 8 * j >= N) break;  // N % 32 == 0: whole 8-column groups are in or out
+        float2 v = make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+        if (ep.bias) {
+          const float2 b = __ldg(reinterpret_cast<const float2*>(ep.bias + n));
+          v.x += b.x; v.y += b.y;
+        }
+        if (EPI == EPI_BIAS_GELU_BF16) { v.x = epi_gelu_tanh(v.x); v.y = epi_gelu_tanh(v.y); }
+        if (EPI == EPI_BIAS_RELU_BF16) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); }
+        if (EPI == EPI_GATE_RESID_F32) {
+          const float2 g = __ldg(reinterpret_cast<const float2*>(gate_row[i] + n));
+          v.x *= g.x; v.y *= g.y;
+        }
+        const int byte = ((8 * j) % COLS + 2 * (lane & 3)) * OB;  // within the 128-byte staging row
+        uint8_t* p = stage + (8 * j / COLS % RING) * 8192 + r * 128 + ((((byte >> 4) ^ (lane >> 2)) << 4) | (byte & 15));
+        if (OB == 2) *reinterpret_cast<uint32_t*>(p) = pack2_bf16(v.x, v.y);
+        else *reinterpret_cast<float2*>(p) = v;
+      }
     }
-    bulk_commit();
+    fence_proxy_async();  // make the generic-proxy writes visible to the TMA unit
+    named_bar_sync(1 + wg, 128);
+    if (leader) {
+#pragma unroll
+      for (int b = 8 * j0 / COLS; b < 8 * j0 / COLS + RING; b++) {
+        if (n0 + b * COLS >= N) break;
+        if (EPI == EPI_GATE_RESID_F32) tma_reduce_add_2d(tmC, stage + (b % RING) * 8192, n0 + b * COLS, m0);
+        else tma_store_2d(tmC, stage + (b % RING) * 8192, n0 + b * COLS, m0);
+      }
+      bulk_commit();
+    }
   }
 }
 
@@ -322,8 +337,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       wg_fence_regs(acc);
       if (prev >= 0 && lane == 0) mbar_arrive(empty_bar + prev);
       if constexpr (TMA_EPI) {
-        epilogue_tma<EPI, BN>(ep, acc, sC + wg * (Cfg::OUT_TILE_BYTES / 2), &tmC, m0 + wg * 64, n0, M, N, wg, warp & 3,
-                              lane);
+        epilogue_tma<EPI, BN, Cfg::RING>(ep, acc, sC + wg * (Cfg::OUT_TILE_BYTES / 2), &tmC, m0 + wg * 64, n0, M, N, wg,
+                                         warp & 3, lane);
       } else {
         const int row0 = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
         epilogue_fragment<EPI, BN>(ep, acc, row0, n0 + 2 * (lane & 3), M, N, splits > 1);
@@ -503,7 +518,8 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       if constexpr (EPI == EPI_BIAS_GELU_E4M3) {
         epilogue_gelu_e4m3(ep, fs, acc, stg, &tmC, m0 + wg * 64, n0, M, wg, warp & 3, lane);
       } else if constexpr (TMA_EPI) {
-        epilogue_tma<EPI, BN8>(ep, acc, stg, &tmC, m0 + wg * 64, n0, M, N, wg, warp & 3, lane);
+        constexpr int whole = BN8 * epi_out_bytes<EPI>() / 128;  // the fragment is staged whole
+        epilogue_tma<EPI, BN8, whole>(ep, acc, stg, &tmC, m0 + wg * 64, n0, M, N, wg, warp & 3, lane);
       } else {
         epilogue_fragment<EPI, BN8>(ep, acc, m0 + r0, n0 + 2 * (lane & 3), M, N, false);
       }
@@ -549,7 +565,7 @@ static int launch_epi(bool wide, bool tma_epi, const CUtensorMap& tmA, const CUt
                       const GemmEpilogue& ep, int M, int N, int K, cudaStream_t st) {
   if constexpr (EPI != EPI_DGELU_BF16) {  // dGELU reads the saved pre-activation per element: register epilogue only
     if (tma_epi) {
-      if constexpr (epi_out_bytes<EPI>() == 2)
+      if constexpr (epi_out_bytes<EPI>() == 2 || EPI == EPI_GATE_RESID_F32)
         if (wide) return launch_gemm<256, EPI, false, true>(tmA, tmB, tmC, ep, M, N, K, st);
       return launch_gemm<128, EPI, false, true>(tmA, tmB, tmC, ep, M, N, K, st);
     }
@@ -574,10 +590,13 @@ int gemm_bf16(const void* A, const void* W, int M, int N, int K, int epi, const 
   const int ob = out_f32 ? 4 : 2;
   const bool tma_epi = epi != EPI_DGELU_BF16 && !ep.aux && !ep.resid && ep.ldc >= N && ((size_t)ep.ldc * ob) % 16 == 0 &&
                        ((uintptr_t)ep.out % 16) == 0;
-  // 128 x 256 tiles only when every CTA of the persistent grid gets at least two of them, so that each tile's epilogue
-  // drains under the next tile's mainloop; else 128 x 128 tiles.  A staged fp32 tile of 128 x 256 (128 KB) would leave
-  // room for two operand stages only, so staged fp32 outputs always use 128 x 128 tiles.
-  const bool wide = (N % 256 == 0) && (ceil_div(M, BM) * (N / 256) >= 2 * sms) && !(tma_epi && out_f32);
+  // 128 x 256 tiles when every CTA of the persistent grid gets at least two of them, so that each tile's epilogue
+  // drains under the next tile's mainloop; else 128 x 128 tiles.  The in-place gate + residual update (staged two column
+  // blocks at a time, four operand stages) takes 128 x 256 tiles at any M: at attn.proj / mlp.fc2 (4098 tokens, one
+  // tile per CTA) they are faster than two 128 x 128 tiles per CTA, which stream 1.33x the operand bytes per FLOP from
+  // L2.  Other staged fp32 outputs (whole 128 x 256 tiles would leave two operand stages) use 128 x 128 tiles.
+  const bool gate_tma = tma_epi && epi == EPI_GATE_RESID_F32;
+  const bool wide = (N % 256 == 0) && (gate_tma || (ceil_div(M, BM) * (N / 256) >= 2 * sms && !(tma_epi && out_f32)));
   const int BN = wide ? 256 : 128;
   CUtensorMap tmA, tmB, tmC;
   memset(&tmC, 0, sizeof(tmC));
