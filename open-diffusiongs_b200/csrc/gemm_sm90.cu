@@ -3,12 +3,19 @@
 //   C[M,N] = epilogue( A[M,K] (bf16, row-major) x W[N,K]^T (bf16, row-major = nn.Linear weight) )
 //
 // One CTA per SM, 384 threads: warps 0..7 = two consumer warpgroups (64 rows of the 128-row tile each, fp32
-// accumulators in registers), warp 8 = TMA producer (its warpgroup gives its registers to the consumers).  Operands are staged by TMA into a 128-byte-swizzled
-// shared-memory ring (BK = 64 bf16 = one swizzle row) that runs continuously across the CTA's tiles, so the producer
-// loads the next tile while the consumers run the epilogue of the current one.  Tile = 128 x BN (BN = 256 or 128),
+// accumulators in registers), warp 8 = TMA producer (its warpgroup gives its registers to the consumers).  Operands are
+// staged by TMA into a 128-byte-swizzled shared-memory ring (a k-block of K = one 128-byte swizzle row) that runs
+// continuously across the CTA's tiles, so the producer loads the next tile while the consumers run the epilogue of the
+// current one.  Tile = 128 x BN (BN = 256 or 128),
 // wgmma m64nBNk16, one k-block group kept in flight while the next is issued.  The inference epilogues stage the
 // finished tile in shared memory and hand it to the TMA unit (a store, or for the in-place residual update a reduce-add
 // in L2), so the consumers go on to the next tile's mainloop while the tile is written out.
+//
+// Operand modes (GemmOp): bf16 K-major (the forward and dgrad GEMMs), bf16 MN-major (the weight gradients, gemm_bf16_tn)
+// and e4m3 (the FP8 inference path, gemm_fp8).  The e4m3 mode is the K-major kernel at BN = 128 with a k-block of 128
+// e4m3 elements, the k-block's 128 activation row scales loaded with each stage, four wgmma m64n128k32 per k-block into
+// a fresh partial tile that is added into the accumulator times its rows' scales, and the per-channel weight scale
+// applied before the epilogue.
 //
 // Fused epilogues = the elementwise tails of the reference DiT block
 // (diffusionGS/models/transformers/utils_transformer.py:270-290, timm Attention/Mlp):
@@ -18,7 +25,7 @@
 //   EPI_F32             y = acc (+ b), fp32                 (tokenizer, decoder head, weight gradients)
 //   EPI_DGELU_BF16      y = acc * gelu'(u)                  (backward of mlp.fc2 -> act: u = saved pre-activation)
 //   EPI_BIAS_RELU_BF16  y = max(acc + b, 0)                 (the LPIPS VGG convolutions, lpips.cu)
-//   EPI_BIAS_GELU_E4M3  y = e4m3(gelu_tanh(acc + b)) + scales (FP8 mlp.fc1 -> fc2's operand; gemm_fp8_kernel only)
+//   EPI_BIAS_GELU_E4M3  y = e4m3(gelu_tanh(acc + b)) + scales (FP8 mlp.fc1 -> fc2's operand; e4m3 mode only)
 // Training mode (GemmEpilogue::aux / resid): fc1 also stores its pre-activation, the gate epilogues also store the
 // pre-gate branch output and may read the residual from a different buffer than they write.
 #include <cstdlib>
@@ -69,28 +76,49 @@ int make_tmap(CUtensorMap* out, CUtensorMapDataType dtype, const void* base, int
 // ---------------------------------------------------------------------------------------------
 // device
 // ---------------------------------------------------------------------------------------------
-constexpr int BM = 128, BK = 64;
+constexpr int BM = 128, BK = 64, BK8 = 128;  // BK / BK8: the bf16 / e4m3 elements of a k-block (one 128-byte row)
 constexpr int GEMM_THREADS = WS_THREADS;
+
+enum GemmOp { OP_BF16_K = 0, OP_BF16_MN = 1, OP_E4M3 = 2 };
 
 // OUT_BYTES: element size of the output tile staged in shared memory for the TMA-store epilogue (0: the epilogue
 // writes from registers).  The staging buffer takes what would otherwise be operand stages.  It holds RING column
 // blocks (128 bytes x 64 rows, 8 KB) per consumer warpgroup: the whole 64 x BN fragment, except for a 128 x 256 fp32
 // tile (128 KB staged whole, which would leave two operand stages), which goes out two column blocks at a time and
-// keeps four stages.
-template <int BN, int OUT_BYTES>
+// keeps four stages.  SCALE_BYTES: the row scales a stage carries besides its operands (e4m3: BM fp32, else 0).
+template <int BN, int OUT_BYTES, int SCALE_BYTES>
 struct GemmCfg {
   static constexpr int SMEM_LIMIT = 227 * 1024;
-  static constexpr int A_BYTES = BM * BK * 2;
-  static constexpr int B_BYTES = BN * BK * 2;
+  static constexpr int S_BYTES = SCALE_BYTES;
+  static constexpr int A_BYTES = BM * 128;
+  static constexpr int B_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int OUT_BLOCKS = BN * OUT_BYTES / 128;  // column blocks of a warpgroup's fragment
   static constexpr int RING = OUT_BLOCKS > 4 ? 2 : OUT_BLOCKS;
   static constexpr int OUT_TILE_BYTES = 2 * RING * 8192;
   static constexpr int EXTRA = 1024 /*align slack*/ + 256 /*barriers*/;
-  static constexpr int FIT = (SMEM_LIMIT - EXTRA - OUT_TILE_BYTES) / STAGE_BYTES;
+  static constexpr int FIT = (SMEM_LIMIT - EXTRA - OUT_TILE_BYTES) / (STAGE_BYTES + S_BYTES);
   static constexpr int STAGES = FIT < (BN == 256 ? 4 : 6) ? FIT : (BN == 256 ? 4 : 6);
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + OUT_TILE_BYTES + EXTRA;
+  static constexpr int SMEM_BYTES = STAGES * (STAGE_BYTES + S_BYTES) + OUT_TILE_BYTES + EXTRA;
   static_assert(STAGES >= 3 && SMEM_BYTES <= SMEM_LIMIT, "GEMM configuration does not fit in shared memory");
+  static_assert(S_BYTES % 16 == 0, "the row scales are one bulk copy per stage: 16-byte multiples");
+};
+static_assert(GemmCfg<256, 4, 0>::RING == 2 && GemmCfg<256, 4, 0>::STAGES == 4,
+              "the in-place gate + residual update on 128 x 256 tiles keeps four operand stages");
+static_assert(GemmCfg<128, 1, BM * 4>::STAGES == 6 && GemmCfg<128, 4, BM * 4>::STAGES == 4,
+              "FP8 stage counts: 6 for fc1 (e4m3 out), 4 for fc2 (in-place fp32)");
+
+// The element size of the output tile of each epilogue when it is staged for a TMA store (see epilogue_tma).
+constexpr int epi_out_bytes(int epi) {
+  return (epi == EPI_GATE_RESID_F32 || epi == EPI_F32) ? 4 : (epi == EPI_BIAS_GELU_E4M3 ? 1 : 2);
+}
+
+// FP8 scales (gemm_fp8; unused in the bf16 modes)
+struct Fp8Scales {
+  const float* sa = nullptr;         // [K/128][lds] activation group scales
+  const float* sw = nullptr;         // [N] weight scales
+  float* out_scale = nullptr;        // EPI_BIAS_GELU_E4M3: [N/128][lds] group scales of the output
+  int lds = 0;                       // fp8_scale_stride(M)
 };
 
 __device__ __forceinline__ float epi_gelu_tanh(float x) {  // nn.GELU(approximate="tanh"), tanh on the MUFU pipe
@@ -108,6 +136,21 @@ __device__ __forceinline__ float epi_dgelu_tanh(float x) {  // d/dx of the above
   asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(u));
   const float du = k0 * (1.0f + 3.0f * k1 * x2);
   return 0.5f * (1.0f + t) + 0.5f * x * (1.0f - t * t) * du;
+}
+
+// The per-element part every epilogue shares, on one thread's column pair (n, n+1) of output row offset ro: acc + b
+// (with keep_pre, training mode, also stored to ep.aux as bf16), then the GELU or ReLU of the epilogues that have one.
+template <int EPI>
+__device__ __forceinline__ float2 epi_bias_act(const GemmEpilogue& ep, float2 v, int n, bool keep_pre = false,
+                                               size_t ro = 0) {
+  if (ep.bias) {
+    const float2 b = __ldg(reinterpret_cast<const float2*>(ep.bias + n));
+    v.x += b.x; v.y += b.y;
+  }
+  if (keep_pre) *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(ep.aux) + ro + n) = pack2_bf16(v.x, v.y);
+  if (EPI == EPI_BIAS_GELU_BF16 || EPI == EPI_BIAS_GELU_E4M3) { v.x = epi_gelu_tanh(v.x); v.y = epi_gelu_tanh(v.y); }
+  if (EPI == EPI_BIAS_RELU_BF16) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); }
+  return v;
 }
 
 template <int BN, bool MN>
@@ -132,16 +175,9 @@ __device__ __forceinline__ void epilogue_fragment(const GemmEpilogue& ep, const 
     for (int j = 0; j < BN / 8; j++) {
       const int n = n0 + 8 * j;
       if (n >= N) break;  // N % 32 == 0: whole 8-column groups are in or out
-      float2 v = make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
-      if (ep.bias) {
-        const float2 b = __ldg(reinterpret_cast<const float2*>(ep.bias + n));
-        v.x += b.x; v.y += b.y;
-      }
-      if ((EPI == EPI_BIAS_GELU_BF16 || EPI == EPI_GATE_RESID_F32) && ep.aux)  // training: keep acc + b (bf16)
-        *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(ep.aux) + ro + n) = pack2_bf16(v.x, v.y);
+      const bool keep_pre = (EPI == EPI_BIAS_GELU_BF16 || EPI == EPI_GATE_RESID_F32) && ep.aux;
+      float2 v = epi_bias_act<EPI>(ep, make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]), n, keep_pre, ro);
       if (EPI == EPI_BIAS_BF16 || EPI == EPI_BIAS_GELU_BF16 || EPI == EPI_DGELU_BF16 || EPI == EPI_BIAS_RELU_BF16) {
-        if (EPI == EPI_BIAS_GELU_BF16) { v.x = epi_gelu_tanh(v.x); v.y = epi_gelu_tanh(v.y); }
-        if (EPI == EPI_BIAS_RELU_BF16) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); }
         if (EPI == EPI_DGELU_BF16) {
           const __nv_bfloat162 u = *reinterpret_cast<const __nv_bfloat162*>(reinterpret_cast<const __nv_bfloat16*>(ep.aux) + ro + n);
           const float2 uf = __bfloat1622float2(u);
@@ -163,28 +199,27 @@ __device__ __forceinline__ void epilogue_fragment(const GemmEpilogue& ep, const 
   }
 }
 
-// The output element type of the epilogues that stage their tile for a TMA store (see epilogue_tma).
-template <int EPI>
-constexpr int epi_out_bytes() {
-  return (EPI == EPI_GATE_RESID_F32 || EPI == EPI_F32) ? 4 : (EPI == EPI_BIAS_GELU_E4M3 ? 1 : 2);
-}
-
 // Epilogue of one warpgroup's 64 x BN fragment through shared memory: the values are computed in registers as in
 // epilogue_fragment, written to this warpgroup's staging buffer, and one thread hands the buffer to the TMA unit, which
 // writes it out while the warpgroup goes on with its next tile's mainloop.  Rows >= M and columns >= N are clipped by
-// the TMA unit.  The staging buffer holds column blocks of 128 bytes (64 bf16 / 32 fp32 columns) x 64 rows, 8 KB each,
-// 128-byte swizzled like the TMA box that stores it: the 16-byte chunk c of row r sits at chunk c ^ (r % 8), which also
-// makes the fragment writes free of bank conflicts.
+// the TMA unit.  The staging buffer holds column blocks of 128 bytes (64 bf16 / 32 fp32 / 128 e4m3 columns) x 64 rows,
+// 8 KB each, 128-byte swizzled like the TMA box that stores it: the 16-byte chunk c of row r sits at chunk c ^ (r % 8),
+// which also makes the fragment writes free of bank conflicts.
 // EPI_GATE_RESID_F32 (in place, no ep.resid) stages gate * (acc + b) and adds it into x with a TMA reduce-add, so x is
 // never read by the SM.  The result is x + round(g * v) rather than fmaf(g, v, x): one more fp32 rounding per update.
+// EPI_BIAS_GELU_E4M3 (BN = 128): the tile's 128 columns are one scale group, so a row's amax is a reduction over the 4
+// lanes that hold the row; a pass over the row applies bias + GELU and writes the row's scale straight to out_scale
+// before the row is staged.
 // RING < the fragment's column blocks: the fragment goes out in batches of RING blocks, each written once the previous
 // batch's stores have read the buffer.
 template <int EPI, int BN, int RING>
-__device__ __forceinline__ void epilogue_tma(const GemmEpilogue& ep, const float (&acc)[BN / 2], uint8_t* stage,
-                                             const CUtensorMap* tmC, int m0, int n0, int M, int N, int wg, int wq, int lane) {
-  constexpr int OB = epi_out_bytes<EPI>();
+__device__ __forceinline__ void epilogue_tma(const GemmEpilogue& ep, const Fp8Scales& fs, float (&acc)[BN / 2],
+                                             uint8_t* stage, const CUtensorMap* tmC, int m0, int n0, int M, int N, int wg,
+                                             int wq, int lane) {
+  constexpr int OB = epi_out_bytes(EPI);
   constexpr int COLS = 128 / OB;            // columns per staging row
   constexpr int JB = RING * COLS / 8;       // 8-column groups per batch
+  constexpr bool WHOLE = EPI == EPI_BIAS_GELU_E4M3;  // gemm_fp8 checks N % 128 == 0: the tile has no columns >= N
   const bool leader = wq == 0 && lane == 0;
   const float* gate_row[2] = {nullptr, nullptr};
   if (EPI == EPI_GATE_RESID_F32) {
@@ -196,30 +231,47 @@ __device__ __forceinline__ void epilogue_tma(const GemmEpilogue& ep, const float
   }
 #pragma unroll
   for (int j0 = 0; j0 < BN / 8; j0 += JB) {
-    if (n0 + 8 * j0 >= N) break;
+    if (!WHOLE && n0 + 8 * j0 >= N) break;
     if (leader) bulk_wait_read<0>();  // the stores of the previous batch (or tile) have read the buffer
     named_bar_sync(1 + wg, 128);
 #pragma unroll
     for (int i = 0; i < 2; i++) {
       const int r = 16 * wq + (lane >> 2) + 8 * i;  // row in the warpgroup's 64-row slice; r % 8 == lane / 4
+      float inv;  // EPI_BIAS_GELU_E4M3: 1 / the row's scale
+      if constexpr (EPI == EPI_BIAS_GELU_E4M3) {  // bias + GELU into acc, then the row's amax and scale
+        static_assert(BN == 128 && JB == BN / 8, "one e4m3 scale group per tile row, staged in one batch");
+        float amax = 0.f;
+#pragma unroll
+        for (int j = 0; j < BN / 8; j++) {
+          const float2 v = epi_bias_act<EPI>(ep, make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]),
+                                             n0 + 8 * j + 2 * (lane & 3));
+          acc[4 * j + 2 * i] = v.x; acc[4 * j + 2 * i + 1] = v.y;
+          amax = fmaxf(amax, fmaxf(fabsf(v.x), fabsf(v.y)));
+        }
+        amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
+        amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
+        const int e = e4m3_scale_exp(amax);
+        inv = exp2_int(-e);
+        if ((lane & 3) == 0 && m0 + r < M) fs.out_scale[(size_t)(n0 / 128) * fs.lds + m0 + r] = exp2_int(e);
+      }
 #pragma unroll
       for (int j = j0; j < j0 + JB; j++) {
         const int n = n0 + 8 * j + 2 * (lane & 3);
-        if (n0 + 8 * j >= N) break;  // N % 32 == 0: whole 8-column groups are in or out
+        if (!WHOLE && n0 + 8 * j >= N) break;  // N % 32 == 0: whole 8-column groups are in or out
         float2 v = make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
-        if (ep.bias) {
-          const float2 b = __ldg(reinterpret_cast<const float2*>(ep.bias + n));
-          v.x += b.x; v.y += b.y;
+        if constexpr (EPI == EPI_BIAS_GELU_E4M3) {
+          v.x *= inv; v.y *= inv;
+        } else {
+          v = epi_bias_act<EPI>(ep, v, n);
         }
-        if (EPI == EPI_BIAS_GELU_BF16) { v.x = epi_gelu_tanh(v.x); v.y = epi_gelu_tanh(v.y); }
-        if (EPI == EPI_BIAS_RELU_BF16) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); }
         if (EPI == EPI_GATE_RESID_F32) {
           const float2 g = __ldg(reinterpret_cast<const float2*>(gate_row[i] + n));
           v.x *= g.x; v.y *= g.y;
         }
         const int byte = ((8 * j) % COLS + 2 * (lane & 3)) * OB;  // within the 128-byte staging row
         uint8_t* p = stage + (8 * j / COLS % RING) * 8192 + r * 128 + ((((byte >> 4) ^ (lane >> 2)) << 4) | (byte & 15));
-        if (OB == 2) *reinterpret_cast<uint32_t*>(p) = pack2_bf16(v.x, v.y);
+        if (OB == 1) *reinterpret_cast<uint16_t*>(p) = pack2_e4m3(v.x, v.y);
+        else if (OB == 2) *reinterpret_cast<uint32_t*>(p) = pack2_bf16(v.x, v.y);
         else *reinterpret_cast<float2*>(p) = v;
       }
     }
@@ -228,7 +280,7 @@ __device__ __forceinline__ void epilogue_tma(const GemmEpilogue& ep, const float
     if (leader) {
 #pragma unroll
       for (int b = 8 * j0 / COLS; b < 8 * j0 / COLS + RING; b++) {
-        if (n0 + b * COLS >= N) break;
+        if (!WHOLE && n0 + b * COLS >= N) break;
         if (EPI == EPI_GATE_RESID_F32) tma_reduce_add_2d(tmC, stage + (b % RING) * 8192, n0 + b * COLS, m0);
         else tma_store_2d(tmC, stage + (b % RING) * 8192, n0 + b * COLS, m0);
       }
@@ -237,32 +289,39 @@ __device__ __forceinline__ void epilogue_tma(const GemmEpilogue& ep, const float
   }
 }
 
-// MN = false:  C = A[M,K] x W[N,K]^T, both operands K-major (rows of 64 K elements = one 128-byte swizzle row).
-// MN = true :  C = A^T x W   for A [K, M], W [K, N] row-major, i.e. both operands MN-major (the weight-gradient GEMM
-//              dW = dY^T X with K = tokens: neither operand has to be transposed in memory).  A stage then holds
+// OP = OP_BF16_K:  C = A[M,K] x W[N,K]^T, both operands K-major (rows of 64 K elements = one 128-byte swizzle row).
+// OP = OP_BF16_MN: C = A^T x W   for A [K, M], W [K, N] row-major, i.e. both operands MN-major (the weight-gradient
+//              GEMM dW = dY^T X with K = tokens: neither operand has to be transposed in memory).  A stage then holds
 //              BM/64 (resp. BN/64) swizzle atoms of [64 K rows x 64 M/N elements]; the descriptors use LBO = 8192 B
 //              (atom to atom along M/N), SBO = 1024 B (8 K rows), and step 16 K rows = 2048 B per wgmma.
-// splits > 1 (split-K, EPI_F32 only): work unit u = (tile u % num_tiles, K range u / num_tiles); every unit adds its
-// partial product into the (pre-zeroed) output.
+// OP = OP_E4M3:    C = sw[n] * sum_kb sa[kb][m] * (A_kb W_kb^T), e4m3 operands K-major (rows of 128 K elements), BN = 128
+//              (a 128 x 256 tile would need 128 + 128 accumulator registers per thread: over the consumers' 232).  The
+//              partial tile of each k-block keeps the tensor core's reduced-precision FP8 accumulation to one 128-term sum.
+// splits > 1 (split-K, bf16 EPI_F32 only): work unit u = (tile u % num_tiles, K range u / num_tiles); every unit adds
+// its partial product into the (pre-zeroed) output.
 // TMA_EPI: the epilogue goes through shared memory and a TMA store into tmC (epilogue_tma); otherwise it writes from
 // registers (epilogue_fragment) and tmC is unused.
-template <int BN, int EPI, bool MN, bool TMA_EPI>
+template <int BN, int EPI, int OP, bool TMA_EPI>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const __grid_constant__ CUtensorMap tmC, GemmEpilogue ep, int M, int N, int K, int splits) {
-  using Cfg = GemmCfg<BN, TMA_EPI ? epi_out_bytes<EPI>() : 0>;
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+            const __grid_constant__ CUtensorMap tmC, GemmEpilogue ep, int M, int N, int K, int splits, Fp8Scales fs) {
+  constexpr bool MN = OP == OP_BF16_MN, E4M3 = OP == OP_E4M3;
+  constexpr int KB = E4M3 ? BK8 : BK;
+  static_assert(!E4M3 || BN == 128, "the e4m3 mode runs 128 x 128 tiles");
+  using Cfg = GemmCfg<BN, TMA_EPI ? epi_out_bytes(EPI) : 0, E4M3 ? BM * 4 : 0>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
   uint8_t* sA = smem;
   uint8_t* sB = smem + Cfg::STAGES * Cfg::A_BYTES;
   uint8_t* sC = smem + Cfg::STAGES * Cfg::STAGE_BYTES;  // TMA_EPI: one 64 x BN staging buffer per consumer warpgroup
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sC + Cfg::OUT_TILE_BYTES);
+  float* sS = reinterpret_cast<float*>(sC + Cfg::OUT_TILE_BYTES);  // e4m3: [STAGES][BM] row scales of the k-block
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sC + Cfg::OUT_TILE_BYTES + Cfg::STAGES * Cfg::S_BYTES);
   uint64_t* empty_bar = full_bar + Cfg::STAGES;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_m = (M + BM - 1) / BM, num_n = (N + BN - 1) / BN;
-  const int num_tiles = num_m * num_n, num_k = (K + BK - 1) / BK;
+  const int num_tiles = num_m * num_n, num_k = (K + KB - 1) / KB;
   const int num_units = num_tiles * splits, kpb = (num_k + splits - 1) / splits;  // k-blocks per unit
 
   if (threadIdx.x == 0) {
@@ -282,14 +341,17 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       int stage = 0;
       uint32_t phase = 0;
       for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
-        const int tile = unit % num_tiles, kb0 = (unit / num_tiles) * kpb, kb1 = min(num_k, kb0 + kpb);
+        const int tile = E4M3 ? unit : unit % num_tiles;  // the e4m3 mode does not split K
+        const int kb0 = E4M3 ? 0 : (unit / num_tiles) * kpb, kb1 = E4M3 ? num_k : min(num_k, kb0 + kpb);
         const int m0 = (tile / num_n) * BM, n0 = (tile % num_n) * BN;
+        // e4m3: the scale rows [m0, min(m0 + 128, lds)): lds % 4 == 0, so a multiple of 16 bytes that stays inside sa
+        const uint32_t sbytes = E4M3 ? (uint32_t)min(BM, fs.lds - m0) * 4u : 0u;
         for (int kb = kb0; kb < kb1; kb++) {
           mbar_wait(empty_bar + stage, phase ^ 1);
-          mbar_arrive_expect_tx(full_bar + stage, Cfg::STAGE_BYTES);
+          mbar_arrive_expect_tx(full_bar + stage, Cfg::STAGE_BYTES + sbytes);
           if (!MN) {
-            tma_load_2d(sA + stage * Cfg::A_BYTES, &tmA, full_bar + stage, kb * BK, m0);
-            tma_load_2d(sB + stage * Cfg::B_BYTES, &tmB, full_bar + stage, kb * BK, n0);
+            tma_load_2d(sA + stage * Cfg::A_BYTES, &tmA, full_bar + stage, kb * KB, m0);
+            tma_load_2d(sB + stage * Cfg::B_BYTES, &tmB, full_bar + stage, kb * KB, n0);
           } else {  // one [64 K x 64 MN] box per swizzle atom
 #pragma unroll
             for (int a = 0; a < BM / 64; a++)
@@ -298,6 +360,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             for (int a = 0; a < BN / 64; a++)
               tma_load_2d(sB + stage * Cfg::B_BYTES + a * 8192, &tmB, full_bar + stage, n0 + a * 64, kb * BK);
           }
+          if constexpr (E4M3) bulk_load_1d(sS + stage * BM, fs.sa + (size_t)kb * fs.lds + m0, sbytes, full_bar + stage);
           if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
         }
       }
@@ -310,7 +373,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     uint32_t phase = 0;
     float acc[BN / 2];
     for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
-      const int tile = unit % num_tiles, kb0 = (unit / num_tiles) * kpb, kb1 = min(num_k, kb0 + kpb);
+      const int tile = E4M3 ? unit : unit % num_tiles;  // the e4m3 mode does not split K
+      const int kb0 = E4M3 ? 0 : (unit / num_tiles) * kpb, kb1 = E4M3 ? num_k : min(num_k, kb0 + kpb);
       const int m0 = (tile / num_n) * BM, n0 = (tile % num_n) * BN;
 #pragma unroll
       for (int i = 0; i < BN / 2; i++) acc[i] = 0.f;
@@ -321,210 +385,60 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         const uint64_t adesc = wg_desc_sw128(smem_u32(sA + stage * Cfg::A_BYTES + wg * 8192), MN ? 8192 : 16, 1024);
         const uint64_t bdesc = wg_desc_sw128(smem_u32(sB + stage * Cfg::B_BYTES), MN ? 8192 : 16, 1024);
         wg_fence();
+        if constexpr (E4M3) {
+          // k32 steps (32 bytes along the swizzle row) into a fresh partial tile, which is added into acc times its
+          // rows' activation scales once it is complete; the stage is released as soon as the scales are read
+          float part[64];
 #pragma unroll
-        for (int k = 0; k < BK / 16; k++) {
-          // K-major: 16 bf16 = 32 bytes along the swizzle row (+2 in the >>4 address field); MN-major: 16 K rows = 2048 B
-          const uint64_t adv = MN ? (uint64_t)(128 * k) : (uint64_t)(2 * k);
-          wg_mma_k16<BN, MN>(acc, adesc + adv, bdesc + adv);
+          for (int k = 0; k < BK8 / 32; k++) wgmma_m64n128k32_e4m3(part, adesc + 2 * k, bdesc + 2 * k, k);
+          wg_commit();
+          wg_wait<0>();
+          wg_fence_regs(part);
+          const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // the thread's rows r0, r0 + 8 of the tile
+          const float s0 = sS[stage * BM + r0], s1 = sS[stage * BM + r0 + 8];
+          __syncwarp();
+          if (lane == 0) mbar_arrive(empty_bar + stage);
+#pragma unroll
+          for (int j = 0; j < 16; j++) {
+            acc[4 * j] = fmaf(s0, part[4 * j], acc[4 * j]);
+            acc[4 * j + 1] = fmaf(s0, part[4 * j + 1], acc[4 * j + 1]);
+            acc[4 * j + 2] = fmaf(s1, part[4 * j + 2], acc[4 * j + 2]);
+            acc[4 * j + 3] = fmaf(s1, part[4 * j + 3], acc[4 * j + 3]);
+          }
+        } else {
+#pragma unroll
+          for (int k = 0; k < BK / 16; k++) {
+            // K-major: 16 bf16 = 32 bytes along the swizzle row (+2 in the >>4 address field); MN-major: 16 K rows = 2048 B
+            const uint64_t adv = MN ? (uint64_t)(128 * k) : (uint64_t)(2 * k);
+            wg_mma_k16<BN, MN>(acc, adesc + adv, bdesc + adv);
+          }
+          wg_commit();
+          wg_wait<1>();  // the group of the previous k-block has retired: its stage may be refilled
+          if (prev >= 0 && lane == 0) mbar_arrive(empty_bar + prev);
+          prev = stage;
         }
-        wg_commit();
-        wg_wait<1>();  // the group of the previous k-block has retired: its stage may be refilled
-        if (prev >= 0 && lane == 0) mbar_arrive(empty_bar + prev);
-        prev = stage;
         if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
       }
-      wg_wait<0>();
-      wg_fence_regs(acc);
-      if (prev >= 0 && lane == 0) mbar_arrive(empty_bar + prev);
+      if constexpr (E4M3) {  // the per-output-channel weight scales
+#pragma unroll
+        for (int j = 0; j < 16; j++) {
+          const float2 w = __ldg(reinterpret_cast<const float2*>(fs.sw + n0 + 8 * j + 2 * (lane & 3)));
+          acc[4 * j] *= w.x; acc[4 * j + 1] *= w.y; acc[4 * j + 2] *= w.x; acc[4 * j + 3] *= w.y;
+        }
+      } else {  // the last k-block's group is still in flight
+        wg_wait<0>();
+        wg_fence_regs(acc);
+        if (prev >= 0 && lane == 0) mbar_arrive(empty_bar + prev);
+      }
       if constexpr (TMA_EPI) {
-        epilogue_tma<EPI, BN, Cfg::RING>(ep, acc, sC + wg * (Cfg::OUT_TILE_BYTES / 2), &tmC, m0 + wg * 64, n0, M, N, wg,
-                                         warp & 3, lane);
+        epilogue_tma<EPI, BN, Cfg::RING>(ep, fs, acc, sC + wg * (Cfg::OUT_TILE_BYTES / 2), &tmC, m0 + wg * 64, n0, M, N,
+                                         wg, warp & 3, lane);
       } else {
         const int row0 = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
         epilogue_fragment<EPI, BN>(ep, acc, row0, n0 + 2 * (lane & 3), M, N, splits > 1);
       }
     }
     if (TMA_EPI && (warp & 3) == 0 && lane == 0) bulk_wait<0>();  // the output is written before the grid completes
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// FP8 (e4m3) variant: same producer / two-consumer structure, ring and PDL as gemm_bf16_kernel, with
-//   * BK = 128 e4m3 = one 128-byte swizzle row (a stage has the bf16 kernel's byte size), 128 x 128 tiles (a 128 x 256
-//     tile would need 128 + 128 accumulator registers per thread: over the consumers' 232);
-//   * four wgmma m64n128k32 per k-block into a fresh partial tile, which is then added into the fp32 accumulator times
-//     its rows' activation scales sa[kb][m] (the producer brings the k-block's 128 row scales in with the stage).  This
-//     applies the 1 x 128 group scales and keeps the tensor core's reduced-precision FP8 accumulation to one 128-term
-//     partial sum;
-//   * the per-output-channel weight scale sw[n] multiplies the accumulator before the (shared) epilogue.
-// ---------------------------------------------------------------------------------------------
-constexpr int BK8 = 128, BN8 = 128;
-
-template <int OUT_BYTES>
-struct Fp8Cfg {
-  static constexpr int SMEM_LIMIT = 227 * 1024;
-  static constexpr int A_BYTES = BM * BK8, B_BYTES = BN8 * BK8, S_BYTES = BM * 4;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int OUT_TILE_BYTES = BM * BN8 * OUT_BYTES;
-  static constexpr int EXTRA = 1024 /*align slack*/ + 256 /*barriers*/;
-  static constexpr int FIT = (SMEM_LIMIT - EXTRA - OUT_TILE_BYTES) / (STAGE_BYTES + S_BYTES);
-  static constexpr int STAGES = FIT < 6 ? FIT : 6;
-  static constexpr int SMEM_BYTES = STAGES * (STAGE_BYTES + S_BYTES) + OUT_TILE_BYTES + EXTRA;
-  static_assert(STAGES >= 3 && SMEM_BYTES <= SMEM_LIMIT, "FP8 GEMM configuration does not fit in shared memory");
-};
-
-struct Fp8Scales {
-  const float* sa;   // [K/128][lds] activation group scales
-  const float* sw;   // [N] weight scales
-  float* out_scale;  // EPI_BIAS_GELU_E4M3: [N/128][lds] group scales of the output
-  int lds;           // fp8_scale_stride(M)
-};
-
-// bias + GELU -> e4m3 of one warpgroup's 64 x 128 fragment: the tile's 128 columns are one scale group, so a row's
-// amax is a reduction over the 4 lanes that hold the row.  The bytes are staged (128-byte swizzled, like the TMA box
-// that stores them) and written by one TMA store; the row scales go straight to out_scale.
-__device__ __forceinline__ void epilogue_gelu_e4m3(const GemmEpilogue& ep, const Fp8Scales& fs, float (&acc)[64],
-                                                   uint8_t* stage, const CUtensorMap* tmC, int m0, int n0, int M,
-                                                   int wg, int wq, int lane) {
-  const bool leader = wq == 0 && lane == 0;
-  if (leader) bulk_wait_read<0>();
-  named_bar_sync(1 + wg, 128);
-#pragma unroll
-  for (int i = 0; i < 2; i++) {
-    const int r = 16 * wq + (lane >> 2) + 8 * i;
-    float amax = 0.f;
-#pragma unroll
-    for (int j = 0; j < BN8 / 8; j++) {
-      const int n = n0 + 8 * j + 2 * (lane & 3);
-      float2 v = make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
-      if (ep.bias) {
-        const float2 b = __ldg(reinterpret_cast<const float2*>(ep.bias + n));
-        v.x += b.x; v.y += b.y;
-      }
-      v.x = epi_gelu_tanh(v.x); v.y = epi_gelu_tanh(v.y);
-      acc[4 * j + 2 * i] = v.x; acc[4 * j + 2 * i + 1] = v.y;
-      amax = fmaxf(amax, fmaxf(fabsf(v.x), fabsf(v.y)));
-    }
-    amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
-    amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
-    const int e = e4m3_scale_exp(amax);
-    const float inv = exp2_int(-e);
-    if ((lane & 3) == 0 && m0 + r < M) fs.out_scale[(size_t)(n0 / 128) * fs.lds + m0 + r] = exp2_int(e);
-#pragma unroll
-    for (int j = 0; j < BN8 / 8; j++) {
-      const int byte = 8 * j + 2 * (lane & 3);
-      uint8_t* p = stage + r * 128 + ((((byte >> 4) ^ (lane >> 2)) << 4) | (byte & 15));
-      *reinterpret_cast<uint16_t*>(p) = pack2_e4m3(acc[4 * j + 2 * i] * inv, acc[4 * j + 2 * i + 1] * inv);
-    }
-  }
-  fence_proxy_async();
-  named_bar_sync(1 + wg, 128);
-  if (leader) {
-    tma_store_2d(tmC, stage, n0, m0);
-    bulk_commit();
-  }
-}
-
-// TMA_EPI: the epilogue stages the tile for a TMA store (EPI_BIAS_BF16, EPI_BIAS_GELU_E4M3) or reduce-add
-// (EPI_GATE_RESID_F32, in place); else it writes from registers (EPI_F32).
-template <int EPI, bool TMA_EPI>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                const __grid_constant__ CUtensorMap tmC, GemmEpilogue ep, Fp8Scales fs, int M, int N, int K) {
-  using Cfg = Fp8Cfg<TMA_EPI ? epi_out_bytes<EPI>() : 0>;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
-  uint8_t* sA = smem;
-  uint8_t* sB = smem + Cfg::STAGES * Cfg::A_BYTES;
-  uint8_t* sC = smem + Cfg::STAGES * Cfg::STAGE_BYTES;
-  float* sS = reinterpret_cast<float*>(sC + Cfg::OUT_TILE_BYTES);  // [STAGES][BM] row scales of the stage's k-block
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sS + Cfg::STAGES * BM);
-  uint64_t* empty_bar = full_bar + Cfg::STAGES;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int num_n = N / BN8, num_tiles = ((M + BM - 1) / BM) * num_n, num_k = K / BK8;
-
-  if (threadIdx.x == 0) {
-    prefetch_tmap(&tmA);
-    prefetch_tmap(&tmB);
-    for (int s = 0; s < Cfg::STAGES; s++) { mbar_init(full_bar + s, 1); mbar_init(empty_bar + s, 8); }
-    fence_barrier_init();
-  }
-  __syncthreads();
-  griddep_launch_dependents();
-  griddep_wait();
-
-  if (warp >= 8) {
-    // ===================== TMA producer =====================
-    ws_producer_regs();
-    if (warp == 8 && lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m0 = (tile / num_n) * BM, n0 = (tile % num_n) * BN8;
-        // the scale rows [m0, min(m0 + 128, lds)): lds % 4 == 0, so a multiple of 16 bytes that stays inside sa
-        const uint32_t sbytes = (uint32_t)min(BM, fs.lds - m0) * 4u;
-        for (int kb = 0; kb < num_k; kb++) {
-          mbar_wait(empty_bar + stage, phase ^ 1);
-          mbar_arrive_expect_tx(full_bar + stage, Cfg::STAGE_BYTES + sbytes);
-          tma_load_2d(sA + stage * Cfg::A_BYTES, &tmA, full_bar + stage, kb * BK8, m0);
-          tma_load_2d(sB + stage * Cfg::B_BYTES, &tmB, full_bar + stage, kb * BK8, n0);
-          bulk_load_1d(sS + stage * BM, fs.sa + (size_t)kb * fs.lds + m0, sbytes, full_bar + stage);
-          if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else {
-    // ===================== consumer warpgroups 0, 1: rows [64 wg, 64 wg + 64) of each tile =====================
-    ws_consumer_regs();
-    const int wg = warp >> 2;
-    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // the thread's rows r0, r0 + 8 of the tile
-    int stage = 0;
-    uint32_t phase = 0;
-    float acc[64], part[64];
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int m0 = (tile / num_n) * BM, n0 = (tile % num_n) * BN8;
-#pragma unroll
-      for (int i = 0; i < 64; i++) acc[i] = 0.f;
-      for (int kb = 0; kb < num_k; kb++) {
-        mbar_wait(full_bar + stage, phase);
-        const uint64_t adesc = wg_desc_sw128(smem_u32(sA + stage * Cfg::A_BYTES + wg * 8192), 16, 1024);
-        const uint64_t bdesc = wg_desc_sw128(smem_u32(sB + stage * Cfg::B_BYTES), 16, 1024);
-        wg_fence();
-#pragma unroll
-        for (int k = 0; k < BK8 / 32; k++) wgmma_m64n128k32_e4m3(part, adesc + 2 * k, bdesc + 2 * k, k);
-        wg_commit();
-        wg_wait<0>();
-        wg_fence_regs(part);
-        const float s0 = sS[stage * BM + r0], s1 = sS[stage * BM + r0 + 8];
-        __syncwarp();
-        if (lane == 0) mbar_arrive(empty_bar + stage);
-#pragma unroll
-        for (int j = 0; j < 16; j++) {
-          acc[4 * j] = fmaf(s0, part[4 * j], acc[4 * j]);
-          acc[4 * j + 1] = fmaf(s0, part[4 * j + 1], acc[4 * j + 1]);
-          acc[4 * j + 2] = fmaf(s1, part[4 * j + 2], acc[4 * j + 2]);
-          acc[4 * j + 3] = fmaf(s1, part[4 * j + 3], acc[4 * j + 3]);
-        }
-        if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-      }
-#pragma unroll
-      for (int j = 0; j < 16; j++) {
-        const float2 w = __ldg(reinterpret_cast<const float2*>(fs.sw + n0 + 8 * j + 2 * (lane & 3)));
-        acc[4 * j] *= w.x; acc[4 * j + 1] *= w.y; acc[4 * j + 2] *= w.x; acc[4 * j + 3] *= w.y;
-      }
-      uint8_t* stg = sC + wg * (Cfg::OUT_TILE_BYTES / 2);
-      if constexpr (EPI == EPI_BIAS_GELU_E4M3) {
-        epilogue_gelu_e4m3(ep, fs, acc, stg, &tmC, m0 + wg * 64, n0, M, wg, warp & 3, lane);
-      } else if constexpr (TMA_EPI) {
-        constexpr int whole = BN8 * epi_out_bytes<EPI>() / 128;  // the fragment is staged whole
-        epilogue_tma<EPI, BN8, whole>(ep, acc, stg, &tmC, m0 + wg * 64, n0, M, N, wg, warp & 3, lane);
-      } else {
-        epilogue_fragment<EPI, BN8>(ep, acc, m0 + r0, n0 + 2 * (lane & 3), M, N, false);
-      }
-    }
-    if (TMA_EPI && (warp & 3) == 0 && lane == 0) bulk_wait<0>();
   }
 }
 
@@ -541,11 +455,22 @@ static int num_sms() {
   return n;
 }
 
-template <int BN, int EPI, bool MN, bool TMA_EPI>
+// A tensor map over a row-major [rows, cols] matrix of elem_bytes-byte elements with a row stride of ld elements, read
+// or written in boxes of box_rows x box_cols (box_cols x elem_bytes = 128 bytes: one swizzle row).
+static int tmap_2d(CUtensorMap* m, const void* base, int elem_bytes, int rows, int cols, int ld, int box_rows,
+                   int box_cols) {
+  const CUtensorMapDataType type = elem_bytes == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                   : (elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_UINT8);
+  uint64_t dims[2] = {(uint64_t)cols, (uint64_t)rows}, str[1] = {(uint64_t)ld * elem_bytes};
+  uint32_t box[2] = {(uint32_t)box_cols, (uint32_t)box_rows};
+  return make_tmap(m, type, base, 2, dims, str, box);
+}
+
+template <int BN, int EPI, int OP, bool TMA_EPI>
 static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const GemmEpilogue& ep,
-                       int M, int N, int K, cudaStream_t st, int splits = 1) {
-  using Cfg = GemmCfg<BN, TMA_EPI ? epi_out_bytes<EPI>() : 0>;
-  auto kern = gemm_bf16_kernel<BN, EPI, MN, TMA_EPI>;
+                       int M, int N, int K, cudaStream_t st, int splits = 1, const Fp8Scales& fs = Fp8Scales()) {
+  using Cfg = GemmCfg<BN, TMA_EPI ? epi_out_bytes(EPI) : 0, OP == OP_E4M3 ? BM * 4 : 0>;
+  auto kern = gemm_kernel<BN, EPI, OP, TMA_EPI>;
   static bool configured = false;
   if (!configured) {
     DGS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -555,7 +480,8 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUt
   DGS_REQUIRE(sms > 0, "gemm: cannot query the device's SM count");
   const int units = ceil_div(M, BM) * ceil_div(N, BN) * splits;
   const int grid = units < sms ? units : sms;
-  DGS_CUDA_OK(launch_pdl(kern, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, st, tmA, tmB, tmC, ep, M, N, K, splits));
+  DGS_CUDA_OK(launch_pdl(kern, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, st, tmA, tmB, tmC, ep, M, N, K, splits,
+                         fs));
   DGS_POST_LAUNCH();
   return DGS_OK;
 }
@@ -565,13 +491,13 @@ static int launch_epi(bool wide, bool tma_epi, const CUtensorMap& tmA, const CUt
                       const GemmEpilogue& ep, int M, int N, int K, cudaStream_t st) {
   if constexpr (EPI != EPI_DGELU_BF16) {  // dGELU reads the saved pre-activation per element: register epilogue only
     if (tma_epi) {
-      if constexpr (epi_out_bytes<EPI>() == 2 || EPI == EPI_GATE_RESID_F32)
-        if (wide) return launch_gemm<256, EPI, false, true>(tmA, tmB, tmC, ep, M, N, K, st);
-      return launch_gemm<128, EPI, false, true>(tmA, tmB, tmC, ep, M, N, K, st);
+      if constexpr (epi_out_bytes(EPI) == 2 || EPI == EPI_GATE_RESID_F32)
+        if (wide) return launch_gemm<256, EPI, OP_BF16_K, true>(tmA, tmB, tmC, ep, M, N, K, st);
+      return launch_gemm<128, EPI, OP_BF16_K, true>(tmA, tmB, tmC, ep, M, N, K, st);
     }
   }
-  return wide ? launch_gemm<256, EPI, false, false>(tmA, tmB, tmC, ep, M, N, K, st)
-              : launch_gemm<128, EPI, false, false>(tmA, tmB, tmC, ep, M, N, K, st);
+  return wide ? launch_gemm<256, EPI, OP_BF16_K, false>(tmA, tmB, tmC, ep, M, N, K, st)
+              : launch_gemm<128, EPI, OP_BF16_K, false>(tmA, tmB, tmC, ep, M, N, K, st);
 }
 
 int gemm_bf16(const void* A, const void* W, int M, int N, int K, int epi, const GemmEpilogue& ep, cudaStream_t st) {
@@ -586,8 +512,8 @@ int gemm_bf16(const void* A, const void* W, int M, int N, int K, int epi, const 
   // The epilogue stages the tile in shared memory for a TMA store (or, in place, a TMA reduce-add) when the output rows
   // meet the TMA's 16-byte alignment.  The training variants (aux stores, a separate residual source), dGELU and
   // unaligned outputs write from registers.
-  const bool out_f32 = epi == EPI_GATE_RESID_F32 || epi == EPI_F32;
-  const int ob = out_f32 ? 4 : 2;
+  const int ob = epi_out_bytes(epi);
+  const bool out_f32 = ob == 4;
   const bool tma_epi = epi != EPI_DGELU_BF16 && !ep.aux && !ep.resid && ep.ldc >= N && ((size_t)ep.ldc * ob) % 16 == 0 &&
                        ((uintptr_t)ep.out % 16) == 0;
   // 128 x 256 tiles when every CTA of the persistent grid gets at least two of them, so that each tile's epilogue
@@ -600,25 +526,11 @@ int gemm_bf16(const void* A, const void* W, int M, int N, int K, int epi, const 
   const int BN = wide ? 256 : 128;
   CUtensorMap tmA, tmB, tmC;
   memset(&tmC, 0, sizeof(tmC));
-  {
-    uint64_t dims[2] = {(uint64_t)K, (uint64_t)M}, str[1] = {(uint64_t)(ep.lda ? ep.lda : K) * 2};
-    uint32_t box[2] = {BK, BM};
-    int rc = make_tmap_bf16(&tmA, A, 2, dims, str, box);
-    if (rc) return rc;
-  }
-  {
-    uint64_t dims[2] = {(uint64_t)K, (uint64_t)N}, str[1] = {(uint64_t)(ep.ldb ? ep.ldb : K) * 2};
-    uint32_t box[2] = {BK, (uint32_t)BN};
-    int rc = make_tmap_bf16(&tmB, W, 2, dims, str, box);
-    if (rc) return rc;
-  }
-  if (tma_epi) {  // one box = one 128-byte column block x the 64 rows of a consumer warpgroup
-    uint64_t dims[2] = {(uint64_t)N, (uint64_t)M}, str[1] = {(uint64_t)ep.ldc * ob};
-    uint32_t box[2] = {(uint32_t)(128 / ob), 64};
-    int rc = make_tmap(&tmC, out_f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, ep.out, 2,
-                       dims, str, box);
-    if (rc) return rc;
-  }
+  int rc = tmap_2d(&tmA, A, 2, M, K, ep.lda ? ep.lda : K, BM, BK);
+  if (!rc) rc = tmap_2d(&tmB, W, 2, N, K, ep.ldb ? ep.ldb : K, BN, BK);
+  // one box = one 128-byte column block x the 64 rows of a consumer warpgroup
+  if (!rc && tma_epi) rc = tmap_2d(&tmC, ep.out, ob, M, N, ep.ldc, 64, 128 / ob);
+  if (rc) return rc;
 #define DGS_GEMM_CASE(E) \
   case E: return launch_epi<E>(wide, tma_epi, tmA, tmB, tmC, ep, M, N, K, st);
   switch (epi) {
@@ -647,17 +559,10 @@ int gemm_bf16_tn(const void* A, const void* W, int M, int N, int K, const GemmEp
   const int BN = wide ? 256 : 128;
   CUtensorMap tmA, tmB, tmC;
   memset(&tmC, 0, sizeof(tmC));  // unused: split-K partial sums are added from registers
-  uint32_t box[2] = {64, BK};  // [64 contiguous M/N elements (128 B) x 64 K rows]
-  {
-    uint64_t dims[2] = {(uint64_t)M, (uint64_t)K}, str[1] = {(uint64_t)lda * 2};
-    int rc = make_tmap_bf16(&tmA, A, 2, dims, str, box);
-    if (rc) return rc;
-  }
-  {
-    uint64_t dims[2] = {(uint64_t)N, (uint64_t)K}, str[1] = {(uint64_t)ldb * 2};
-    int rc = make_tmap_bf16(&tmB, W, 2, dims, str, box);
-    if (rc) return rc;
-  }
+  // [64 contiguous M/N elements (128 B) x 64 K rows]
+  int rc = tmap_2d(&tmA, A, 2, K, M, lda, BK, 64);
+  if (!rc) rc = tmap_2d(&tmB, W, 2, K, N, ldb, BK, 64);
+  if (rc) return rc;
   // Split-K: the weight gradients have few output tiles (attn.proj: 64 of 128 x 128) but K = tokens is long, so K is cut
   // until the work units fill the SMs; every unit adds its partial sum into the zeroed output (fp32 atomics).
   const int tiles = ceil_div(M, BM) * ceil_div(N, BN), num_k = ceil_div(K, BK);
@@ -670,27 +575,8 @@ int gemm_bf16_tn(const void* A, const void* W, int M, int N, int K, const GemmEp
   GemmEpilogue e2 = ep;
   e2.ldc = ldc;
   if (splits > 1) DGS_CUDA_OK(cudaMemset2DAsync(ep.out, (size_t)ldc * 4, 0, (size_t)N * 4, (size_t)M, st));
-  return wide ? launch_gemm<256, EPI_F32, true, false>(tmA, tmB, tmC, e2, M, N, K, st, splits)
-              : launch_gemm<128, EPI_F32, true, false>(tmA, tmB, tmC, e2, M, N, K, st, splits);
-}
-
-template <int EPI, bool TMA_EPI>
-static int launch_fp8(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const GemmEpilogue& ep,
-                      const Fp8Scales& fs, int M, int N, int K, cudaStream_t st) {
-  using Cfg = Fp8Cfg<TMA_EPI ? epi_out_bytes<EPI>() : 0>;
-  auto kern = gemm_fp8_kernel<EPI, TMA_EPI>;
-  static bool configured = false;
-  if (!configured) {
-    DGS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    configured = true;
-  }
-  const int sms = num_sms();
-  DGS_REQUIRE(sms > 0, "gemm_fp8: cannot query the device's SM count");
-  const int tiles = ceil_div(M, BM) * (N / BN8);
-  DGS_CUDA_OK(launch_pdl(kern, dim3(tiles < sms ? tiles : sms), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, st, tmA, tmB, tmC, ep,
-                         fs, M, N, K));
-  DGS_POST_LAUNCH();
-  return DGS_OK;
+  return wide ? launch_gemm<256, EPI_F32, OP_BF16_MN, false>(tmA, tmB, tmC, e2, M, N, K, st, splits)
+              : launch_gemm<128, EPI_F32, OP_BF16_MN, false>(tmA, tmB, tmC, e2, M, N, K, st, splits);
 }
 
 int gemm_fp8(const void* A, const float* sa, const void* W, const float* sw, int M, int N, int K, int epi,
@@ -708,7 +594,7 @@ int gemm_fp8(const void* A, const float* sa, const void* W, const float* sw, int
                   ((uintptr_t)(out_scale) % 16) == 0 && ((uintptr_t)ep.out % 16) == 0,
               "gemm_fp8: operands, scales and output must be 16-byte aligned");
   const bool tma_epi = epi != EPI_F32;
-  const int ob = tma_epi ? (epi == EPI_GATE_RESID_F32 ? 4 : (epi == EPI_BIAS_GELU_E4M3 ? 1 : 2)) : 4;
+  const int ob = epi_out_bytes(epi);
   DGS_REQUIRE(ep.ldc >= N && ((size_t)ep.ldc * ob) % 16 == 0, "gemm_fp8: output row stride %d must be >= N and 16-byte "
               "aligned", ep.ldc);
   const int sms = num_sms();
@@ -717,31 +603,15 @@ int gemm_fp8(const void* A, const float* sa, const void* W, const float* sw, int
   fs.sa = sa; fs.sw = sw; fs.out_scale = out_scale; fs.lds = fp8_scale_stride(M);
   CUtensorMap tmA, tmB, tmC;
   memset(&tmC, 0, sizeof(tmC));
-  {
-    uint64_t dims[2] = {(uint64_t)K, (uint64_t)M}, str[1] = {(uint64_t)K};
-    uint32_t box[2] = {BK8, BM};
-    int rc = make_tmap(&tmA, CU_TENSOR_MAP_DATA_TYPE_UINT8, A, 2, dims, str, box);
-    if (rc) return rc;
-  }
-  {
-    uint64_t dims[2] = {(uint64_t)K, (uint64_t)N}, str[1] = {(uint64_t)K};
-    uint32_t box[2] = {BK8, BN8};
-    int rc = make_tmap(&tmB, CU_TENSOR_MAP_DATA_TYPE_UINT8, W, 2, dims, str, box);
-    if (rc) return rc;
-  }
-  if (tma_epi) {  // one box = one 128-byte column block x the 64 rows of a consumer warpgroup
-    const CUtensorMapDataType type = ob == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
-                                     : (ob == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_UINT8);
-    uint64_t dims[2] = {(uint64_t)N, (uint64_t)M}, str[1] = {(uint64_t)ep.ldc * ob};
-    uint32_t box[2] = {(uint32_t)(128 / ob), 64};
-    int rc = make_tmap(&tmC, type, ep.out, 2, dims, str, box);
-    if (rc) return rc;
-  }
+  int rc = tmap_2d(&tmA, A, 1, M, K, K, BM, BK8);
+  if (!rc) rc = tmap_2d(&tmB, W, 1, N, K, K, 128, BK8);
+  if (!rc && tma_epi) rc = tmap_2d(&tmC, ep.out, ob, M, N, ep.ldc, 64, 128 / ob);
+  if (rc) return rc;
   switch (epi) {
-    case EPI_BIAS_BF16: return launch_fp8<EPI_BIAS_BF16, true>(tmA, tmB, tmC, ep, fs, M, N, K, st);
-    case EPI_GATE_RESID_F32: return launch_fp8<EPI_GATE_RESID_F32, true>(tmA, tmB, tmC, ep, fs, M, N, K, st);
-    case EPI_BIAS_GELU_E4M3: return launch_fp8<EPI_BIAS_GELU_E4M3, true>(tmA, tmB, tmC, ep, fs, M, N, K, st);
-    default: return launch_fp8<EPI_F32, false>(tmA, tmB, tmC, ep, fs, M, N, K, st);
+    case EPI_BIAS_BF16: return launch_gemm<128, EPI_BIAS_BF16, OP_E4M3, true>(tmA, tmB, tmC, ep, M, N, K, st, 1, fs);
+    case EPI_GATE_RESID_F32: return launch_gemm<128, EPI_GATE_RESID_F32, OP_E4M3, true>(tmA, tmB, tmC, ep, M, N, K, st, 1, fs);
+    case EPI_BIAS_GELU_E4M3: return launch_gemm<128, EPI_BIAS_GELU_E4M3, OP_E4M3, true>(tmA, tmB, tmC, ep, M, N, K, st, 1, fs);
+    default: return launch_gemm<128, EPI_F32, OP_E4M3, false>(tmA, tmB, tmC, ep, M, N, K, st, 1, fs);
   }
 }
 
