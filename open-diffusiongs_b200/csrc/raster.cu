@@ -18,6 +18,7 @@
 #include <cub/cub.cuh>
 
 #include <cstring>
+#include <type_traits>
 
 #include "dgs_internal.h"
 
@@ -52,8 +53,19 @@ struct Problem {
   float bg[3];
 };
 
+// Counters of one forward, written by the binning and blend kernels and read back by the host at its syncs
+struct BinTotals {
+  uint32_t R;              // instances of the batch (32-bit scan: R64 tells whether it wrapped)
+  uint32_t R_near;         // two-phase: phase-A instances at the first near fraction (1/2^near_log2, adaptive 1/8)
+  uint32_t unfinished;     // two-phase: tiles that still have an unsaturated pixel after phase A
+  uint32_t longest;        // small-scene path: longest tile list
+  unsigned long long R64;  // exact instance count
+  uint32_t R_near_b;       // adaptive two-phase: phase-A instances at 1/16
+  uint32_t pad;
+};
+
 struct GeomState {
-  float4* g0;        // {x_pix, y_pix, depth, radius (int bits)}
+  float4* g0;       // {x_pix, y_pix, depth, radius (int bits)}
   float4* g1;        // {conic A, B, C, opacity}
   float4* g2;        // {r, g, b, clamped bits}
   uint32_t* tiles;   // tiles touched, indexed by (view, Gaussian)
@@ -66,8 +78,9 @@ struct GeomState {
   uint32_t* offsets;       // inclusive scan of tiles_sorted
   uint32_t* open_counts;   // phase B: open tiles touched per depth rank (0 for the near ranks) ...
   uint32_t* open_offsets;  // ... and their inclusive scan
-  uint32_t* view_meta;     // [NV][4] two-phase binning: {startA, startB, baseA, baseB} instance offsets per view
-  uint32_t* totals;        // [6] {R, R_near, tiles not finished after phase A, -, exact 64-bit instance count (lo, hi)}
+  uint32_t* view_meta;     // [2][NV][2] two-phase binning, per candidate near fraction and view: where its near
+                           // instances start in the global scan and in the compact phase-A buffer
+  BinTotals* totals;
   Camera* cams;
   void* scan_temp;
   size_t scan_bytes;
@@ -87,8 +100,8 @@ struct GeomState {
     s.offsets = c.take<uint32_t>(N);
     s.open_counts = c.take<uint32_t>(N);
     s.open_offsets = c.take<uint32_t>(N);
-    s.view_meta = c.take<uint32_t>((size_t)NV * 8);  // two candidate near fractions (adaptive two-phase binning)
-    s.totals = c.take<uint32_t>(8);
+    s.view_meta = c.take<uint32_t>((size_t)NV * 4);
+    s.totals = c.take<BinTotals>(1);
     s.cams = c.take<Camera>(NV);
     size_t scan_b = 0, sort_b = 0;
     cub::DeviceScan::InclusiveSum(nullptr, scan_b, s.tiles_sorted, s.offsets, (int)N);
@@ -488,7 +501,7 @@ __global__ void __launch_bounds__(256) project_kernel(Problem pb, GeomState gs, 
 }
 
 // tiles touched in depth-rank order (input of the instance-offset scan)
-// Also accumulates the EXACT instance count in 64 bits (totals[4..5]): the 32-bit scan below wraps silently beyond
+// Also accumulates the EXACT instance count in 64 bits (totals->R64): the 32-bit scan below wraps silently beyond
 // 2^32 instances, and the host must be able to tell "too many for one batch" from a small wrapped number.
 __global__ void gather_tiles_kernel(size_t N, int P, GeomState gs) {
   const size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -501,7 +514,62 @@ __global__ void gather_tiles_kernel(size_t N, int P, GeomState gs) {
   unsigned long long sum = t;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-  if ((threadIdx.x & 31) == 0 && sum) atomicAdd(reinterpret_cast<unsigned long long*>(gs.totals + 4), sum);
+  if ((threadIdx.x & 31) == 0 && sum) atomicAdd(&gs.totals->R64, sum);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Walking a Gaussian's tile rect, shared by every binning kernel that visits tiles one by one.
+// walk_rect visits the tiles of [x0,x1) x [y0,y1) in row-major order as visit(tile, rank, payload), tile = y * gx + x.
+// A rect under DUP_COOP_THRESHOLD tiles is walked by its own thread; larger ones (a few big splats would otherwise
+// serialise a thread for hundreds of tiles) lane-parallel by the whole warp, one rect after another, with the owner's
+// payload broadcast.  keep(tile) drops tiles (KeepAll: none); rank is the tile's position among the kept tiles of its
+// rect, counted by the thread or, on the warp path, by a ballot prefix over each 32-tile step, so ranks stay in
+// row-major order.  Every lane of the warp must call it; an empty rect visits nothing.
+// ---------------------------------------------------------------------------------------------
+constexpr int DUP_COOP_THRESHOLD = 32;
+struct KeepAll {};
+
+template <typename Keep, typename Visit>
+__device__ __forceinline__ void walk_rect(int x0, int y0, int x1, int y1, int gx, uint2 payload, Keep keep, Visit visit) {
+  constexpr bool kFilter = !std::is_same<Keep, KeepAll>::value;
+  const int lane = threadIdx.x & 31;
+  const int w = x1 - x0, area = w * (y1 - y0);
+  if (area > 0 && area < DUP_COOP_THRESHOLD) {
+    uint32_t rank = 0;
+    for (int y = y0; y < y1; y++)
+      for (int x = x0; x < x1; x++) {
+        const int t = y * gx + x;
+        if constexpr (kFilter) {
+          if (!keep(t)) continue;
+        }
+        visit(t, rank++, payload);
+      }
+  }
+  unsigned big = __ballot_sync(0xffffffffu, area >= DUP_COOP_THRESHOLD);
+  while (big) {
+    const int src = __ffs(big) - 1;
+    big &= big - 1;
+    const int bx0 = __shfl_sync(0xffffffffu, x0, src), by0 = __shfl_sync(0xffffffffu, y0, src);
+    const int bw = __shfl_sync(0xffffffffu, w, src), barea = __shfl_sync(0xffffffffu, area, src);
+    const uint2 bp = make_uint2(__shfl_sync(0xffffffffu, payload.x, src), __shfl_sync(0xffffffffu, payload.y, src));
+    if constexpr (kFilter) {
+      uint32_t rank = 0;
+      for (int t0 = 0; t0 < barea; t0 += 32) {
+        const int t = t0 + lane;
+        int tile = 0;
+        bool kept = false;
+        if (t < barea) {
+          tile = (by0 + t / bw) * gx + bx0 + t % bw;
+          kept = keep(tile);
+        }
+        const unsigned m = __ballot_sync(0xffffffffu, kept);
+        if (kept) visit(tile, rank + __popc(m & ((1u << lane) - 1u)), bp);
+        rank += __popc(m);
+      }
+    } else {
+      for (uint32_t t = lane; t < (uint32_t)barea; t += 32) visit((by0 + (int)(t / bw)) * gx + bx0 + (int)(t % bw), t, bp);
+    }
+  }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -510,76 +578,63 @@ __global__ void gather_tiles_kernel(size_t N, int P, GeomState gs) {
 // (a sort of P elements), instances are emitted in that order, and the big per-instance sort only has to be a
 // STABLE sort by the 32-bit tile id (2 radix passes over 8-byte pairs instead of 6 over 12-byte pairs).
 // The resulting order -- tile, then depth, ties by Gaussian index -- is identical.
-// A warp handles its lanes' small rects one thread each, then co-operates lane-parallel on every large rect.
 // ---------------------------------------------------------------------------------------------
-constexpr int DUP_COOP_THRESHOLD = 32;
 
-// Two-phase binning bookkeeping: per view, where its near (ranks < Pn) and far instances start in the global scan and
-// in the two compact per-phase buffers; totals[0] = R, totals[1] = R_near.  One block, NV is small.
+// Two-phase binning bookkeeping for one near fraction: per view, where its near instances (ranks < Pn) start in the
+// global scan and in the compact phase-A buffer (near_meta[2v], near_meta[2v + 1]); *r_near = their total, totals->R =
+// every instance.  One thread: NV is small.
 __global__ void chunk_meta_kernel(int NV, int P, int Pn, const uint32_t* __restrict__ offsets,
-                                  uint32_t* __restrict__ view_meta, uint32_t* __restrict__ totals, int near_slot) {
+                                  uint32_t* __restrict__ near_meta, BinTotals* __restrict__ totals,
+                                  uint32_t* __restrict__ r_near) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  uint32_t baseA = 0, baseB = 0;
+  uint32_t base = 0;
   for (int v = 0; v < NV; v++) {
     const size_t k0 = (size_t)v * P;
-    const uint32_t startA = (k0 == 0) ? 0u : offsets[k0 - 1];
-    const uint32_t startB = offsets[k0 + Pn - 1];
-    const uint32_t end = offsets[k0 + P - 1];
-    view_meta[4 * v + 0] = startA; view_meta[4 * v + 1] = startB;
-    view_meta[4 * v + 2] = baseA; view_meta[4 * v + 3] = baseB;
-    baseA += startB - startA;
-    baseB += end - startB;
+    const uint32_t start = (k0 == 0) ? 0u : offsets[k0 - 1];
+    near_meta[2 * v + 0] = start;
+    near_meta[2 * v + 1] = base;
+    base += offsets[k0 + Pn - 1] - start;
   }
-  totals[0] = baseA + baseB;
-  totals[near_slot] = baseA;
-  totals[2] = 0;
+  totals->R = offsets[(size_t)NV * P - 1];
+  *r_near = base;
 }
 
-// phase 0: every rank, global scan offsets; phase 1: ranks [0, Pn) into the compact near buffer; phase 2: ranks
-// [Pn, P) into the compact far buffer
-__global__ void __launch_bounds__(256) emit_keys_kernel(Problem pb, GeomState gs, uint32_t* __restrict__ keys,
-                                                        uint32_t* __restrict__ vals, int phase, int rank_lo,
-                                                        int rank_hi) {
+// Ranks [rank_lo, rank_hi) of every view.  OPEN = false: every tile of the rect, at the rank's exclusive scan position
+// in `offsets`, rebased per view into the compact phase-A buffer when near_meta is given.  OPEN = true (phase B): only
+// the tiles still open after phase A, at the rank's exclusive scan position in `open_offsets`.
+template <bool OPEN>
+__global__ void __launch_bounds__(256) emit_keys_kernel(Problem pb, GeomState gs, const uint32_t* __restrict__ tile_open,
+                                                        const uint32_t* __restrict__ near_meta,
+                                                        uint32_t* __restrict__ keys, uint32_t* __restrict__ vals,
+                                                        int rank_lo, int rank_hi) {
   const int view = blockIdx.y;
   const int r = rank_lo + blockIdx.x * blockDim.x + threadIdx.x;  // depth rank inside the view
-  const int lane = threadIdx.x & 31;
   const bool in_range = r < rank_hi;
   const size_t k = (size_t)view * pb.P + (in_range ? r : rank_lo);
-  uint32_t cnt = in_range ? gs.tiles_sorted[k] : 0;
+  const uint32_t cnt = !in_range ? 0u : OPEN ? gs.open_counts[k] : gs.tiles_sorted[k];
   uint32_t off = 0, id = 0;
   int x0 = 0, y0 = 0, x1 = 0, y1 = 0;
   if (cnt) {
-    off = (k == 0) ? 0u : gs.offsets[k - 1];
-    if (phase == 1) off = off - gs.view_meta[4 * view + 0] + gs.view_meta[4 * view + 2];
-    else if (phase == 2) off = off - gs.view_meta[4 * view + 1] + gs.view_meta[4 * view + 3];
+    if (OPEN) {
+      off = gs.open_offsets[k] - cnt;  // inclusive scan
+    } else {
+      off = (k == 0) ? 0u : gs.offsets[k - 1];
+      if (near_meta) off = off - near_meta[2 * view] + near_meta[2 * view + 1];
+    }
     id = gs.perm[k];
     const float4 g = gs.g0[(size_t)view * pb.P + id];
     tile_rect(g.x, g.y, __float_as_int(g.w), pb.gx, pb.gy, x0, y0, x1, y1);
   }
   const uint32_t tile_base = (uint32_t)(view * pb.tiles);
-  if (cnt && cnt < DUP_COOP_THRESHOLD) {
-    for (int y = y0; y < y1; y++)
-      for (int x = x0; x < x1; x++) {
-        keys[off] = tile_base + (uint32_t)(y * pb.gx + x);
-        vals[off] = id;
-        off++;
-      }
-  }
-  unsigned big = __ballot_sync(0xffffffffu, cnt >= DUP_COOP_THRESHOLD);
-  while (big) {
-    const int src = __ffs(big) - 1;
-    big &= big - 1;
-    const uint32_t c_ = __shfl_sync(0xffffffffu, cnt, src);
-    const uint32_t o_ = __shfl_sync(0xffffffffu, off, src);
-    const int bx0 = __shfl_sync(0xffffffffu, x0, src), by0 = __shfl_sync(0xffffffffu, y0, src);
-    const int bx1 = __shfl_sync(0xffffffffu, x1, src);
-    const uint32_t bid = __shfl_sync(0xffffffffu, id, src);
-    const int w = bx1 - bx0;
-    for (uint32_t t = lane; t < c_; t += 32) {
-      const int y = by0 + (int)(t / w), x = bx0 + (int)(t % w);
-      keys[o_ + t] = tile_base + (uint32_t)(y * pb.gx + x);
-      vals[o_ + t] = bid;
-    }
+  auto emit = [&](int tile, uint32_t rank, uint2 p) {
+    keys[p.x + rank] = tile_base + (uint32_t)tile;
+    vals[p.x + rank] = p.y;
+  };
+  if constexpr (OPEN) {
+    const uint32_t* open = tile_open + (size_t)view * pb.tiles;
+    walk_rect(x0, y0, x1, y1, pb.gx, make_uint2(off, id), [&](int tile) { return open[tile] != 0u; }, emit);
+  } else {
+    walk_rect(x0, y0, x1, y1, pb.gx, make_uint2(off, id), KeepAll(), emit);
   }
 }
 
@@ -603,67 +658,6 @@ __global__ void __launch_bounds__(256) count_open_kernel(Problem pb, GeomState g
   gs.open_counts[k] = cnt;
 }
 
-// phase-B emission: ranks [Pn, P), open tiles only, offsets = scan of count_open_kernel's counts
-__global__ void __launch_bounds__(256) emit_open_keys_kernel(Problem pb, GeomState gs, const uint32_t* __restrict__ tile_open,
-                                                             uint32_t* __restrict__ keys, uint32_t* __restrict__ vals,
-                                                             int Pn) {
-  const int view = blockIdx.y;
-  const int r = Pn + blockIdx.x * blockDim.x + threadIdx.x;
-  const int lane = threadIdx.x & 31;
-  const bool in_range = r < pb.P;
-  const size_t k = (size_t)view * pb.P + (in_range ? r : Pn);
-  const uint32_t cnt = in_range ? gs.open_counts[k] : 0;
-  uint32_t off = 0, id = 0;
-  int x0 = 0, y0 = 0, x1 = 0, y1 = 0;
-  if (cnt) {
-    off = gs.open_offsets[k] - cnt;  // inclusive scan
-    id = gs.perm[k];
-    const float4 g = gs.g0[(size_t)view * pb.P + id];
-    tile_rect(g.x, g.y, __float_as_int(g.w), pb.gx, pb.gy, x0, y0, x1, y1);
-  }
-  const uint32_t tile_base = (uint32_t)(view * pb.tiles);
-  const uint32_t* op = tile_open + (size_t)view * pb.tiles;
-  const int area = (x1 - x0) * (y1 - y0);
-  if (cnt && area < DUP_COOP_THRESHOLD) {
-    for (int y = y0; y < y1; y++)
-      for (int x = x0; x < x1; x++) {
-        const int t = y * pb.gx + x;
-        if (op[t]) {
-          keys[off] = tile_base + (uint32_t)t;
-          vals[off] = id;
-          off++;
-        }
-      }
-  }
-  unsigned big = __ballot_sync(0xffffffffu, cnt && area >= DUP_COOP_THRESHOLD);
-  while (big) {
-    const int src = __ffs(big) - 1;
-    big &= big - 1;
-    uint32_t o_ = __shfl_sync(0xffffffffu, off, src);
-    const int bx0 = __shfl_sync(0xffffffffu, x0, src), by0 = __shfl_sync(0xffffffffu, y0, src);
-    const int bx1 = __shfl_sync(0xffffffffu, x1, src);
-    const int barea = __shfl_sync(0xffffffffu, area, src);
-    const uint32_t bid = __shfl_sync(0xffffffffu, id, src);
-    const int w = bx1 - bx0;
-    for (int t0 = 0; t0 < barea; t0 += 32) {  // rect tiles in row-major order, 32 at a time, compacted by ballot
-      const int t = t0 + lane;
-      int tl = 0;
-      bool open = false;
-      if (t < barea) {
-        tl = (by0 + t / w) * pb.gx + bx0 + t % w;
-        open = op[tl] != 0;
-      }
-      const unsigned m = __ballot_sync(0xffffffffu, open);
-      if (open) {
-        const uint32_t pos = o_ + __popc(m & ((1u << lane) - 1u));
-        keys[pos] = tile_base + (uint32_t)tl;
-        vals[pos] = bid;
-      }
-      o_ += __popc(m);
-    }
-  }
-}
-
 // ---------------------------------------------------------------------------------------------
 // Small-scene binning: when a batch has few view-Gaussians the global machinery above (depth ranking sort, scan,
 // key emission, tile sort: ~12 launches) costs more than the work.  Instead: the projection counts instances per tile,
@@ -676,9 +670,9 @@ constexpr int SMALL_TILE_CAP = 4096;      // longest tile list the shared-memory
 constexpr int SMALL_MAX_N = 1 << 18;      // view-Gaussians
 constexpr int SMALL_MAX_TILES = 1 << 15;  // views * tiles (one block scans them)
 
-// counts[t] -> ranges[t] = [start, end), cursor[t] = start; totals[0] = R, totals[3] = longest list, totals[4..5] = R (64 bit)
+// counts[t] -> ranges[t] = [start, end), cursor[t] = start; totals->R = R, totals->longest = longest list
 __global__ void __launch_bounds__(1024) tile_scan_kernel(int ntiles, const uint32_t* __restrict__ counts, uint2* __restrict__ ranges,
-                                                         uint2* __restrict__ cursor, uint32_t* __restrict__ totals) {
+                                                         uint2* __restrict__ cursor, BinTotals* __restrict__ totals) {
   __shared__ uint32_t s_warp[32];
   __shared__ uint32_t s_carry, s_max;
   if (threadIdx.x == 0) { s_carry = 0; s_max = 0; }
@@ -719,56 +713,39 @@ __global__ void __launch_bounds__(1024) tile_scan_kernel(int ntiles, const uint3
     __syncthreads();
   }
   if (threadIdx.x == 0) {
-    totals[0] = s_carry; totals[1] = 0; totals[2] = 0; totals[3] = s_max; totals[4] = s_carry; totals[5] = 0;
+    totals->R = s_carry;
+    totals->longest = s_max;
   }
 }
 
 // COUNT: every (view, Gaussian) adds 1 to each tile of its rect.  FILL: it drops one (depth bits, id) record into each of
-// those tiles at the tile's cursor.  Rects below 32 tiles are walked by their own thread; larger ones (a few big splats
-// would otherwise serialise a thread for hundreds of atomics) lane-parallel by the whole warp, one after the other.
+// those tiles at the tile's cursor.
 template <bool FILL>
 __global__ void __launch_bounds__(256) tile_count_fill_kernel(Problem pb, GeomState gs, uint32_t* __restrict__ counts,
                                                               uint2* __restrict__ cursor, uint32_t* __restrict__ depth_out,
                                                               uint32_t* __restrict__ id_out) {
   const int view = blockIdx.y;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const int lane = threadIdx.x & 31;
   int x0 = 0, y0 = 0, x1 = 0, y1 = 0;
-  uint32_t cnt = 0, depth = 0;
+  uint32_t depth = 0;
   if (i < pb.P) {
     const size_t n = (size_t)view * pb.P + i;
-    cnt = gs.tiles[n];
-    if (cnt) {
+    if (gs.tiles[n]) {
       const float4 g = gs.g0[n];
       tile_rect(g.x, g.y, __float_as_int(g.w), pb.gx, pb.gy, x0, y0, x1, y1);
       depth = __float_as_uint(g.z);
     }
   }
   const size_t tbase = (size_t)view * pb.tiles;
-  auto visit = [&](int tile, uint32_t d, uint32_t id) {
+  walk_rect(x0, y0, x1, y1, pb.gx, make_uint2(depth, (uint32_t)i), KeepAll(), [&](int tile, uint32_t, uint2 p) {
     if (FILL) {
       const uint32_t pos = atomicAdd(&cursor[tbase + tile].x, 1u);
-      depth_out[pos] = d;
-      id_out[pos] = id;
+      depth_out[pos] = p.x;
+      id_out[pos] = p.y;
     } else {
       atomicAdd(counts + tbase + tile, 1u);
     }
-  };
-  if (cnt && cnt < DUP_COOP_THRESHOLD) {
-    for (int y = y0; y < y1; y++)
-      for (int x = x0; x < x1; x++) visit(y * pb.gx + x, depth, (uint32_t)i);
-  }
-  unsigned big = __ballot_sync(0xffffffffu, cnt >= DUP_COOP_THRESHOLD);
-  while (big) {
-    const int src = __ffs(big) - 1;
-    big &= big - 1;
-    const int bx0 = __shfl_sync(0xffffffffu, x0, src), by0 = __shfl_sync(0xffffffffu, y0, src);
-    const int bx1 = __shfl_sync(0xffffffffu, x1, src), by1 = __shfl_sync(0xffffffffu, y1, src);
-    const uint32_t bd = __shfl_sync(0xffffffffu, depth, src);
-    const uint32_t bid = (uint32_t)__shfl_sync(0xffffffffu, i, src);
-    const int w = bx1 - bx0, area = w * (by1 - by0);
-    for (int t = lane; t < area; t += 32) visit((by0 + t / w) * pb.gx + bx0 + t % w, bd, bid);
-  }
+  });
 }
 
 // one CTA per (view, tile): bitonic sort of the bucket's 64-bit (depth bits << 32 | id) keys in shared memory
@@ -985,7 +962,7 @@ __global__ void __launch_bounds__(TILE_PIX) blend_forward_kernel(Problem pb, Geo
     unfinished = __syncthreads_or(!done);
     if (threadIdx.x == 0) {
       im.tile_open[tile_g] = unfinished ? 1u : 0u;
-      if (unfinished) atomicAdd(gs.totals + 2, 1u);
+      if (unfinished) atomicAdd(&gs.totals->unfinished, 1u);
     }
   }
   if (inside) {
@@ -1507,246 +1484,282 @@ static int bits_for(uint32_t n) {  // smallest b with (n >> b) == 0  (getHigherM
   return b;
 }
 
-struct ForwardPlan {
+struct Allocators {  // the caller's arena callbacks: geometry, binning (once per bin pass) and image state
+  dgs_alloc_fn geom; void* geom_user;
+  dgs_alloc_fn bin; void* bin_user;
+  dgs_alloc_fn img; void* img_user;
+};
+
+// Batched: C2W and fxfycxcy per view (build_cameras_kernel).  Single view (c2w == nullptr): the view and projection
+// matrices, camera position and tan(fov) of GaussianRasterizationSettings (pack_camera_kernel).
+struct CameraInput {
+  const float* c2w = nullptr;
+  const float* fxfycxcy = nullptr;
+  const float* view = nullptr;
+  const float* proj = nullptr;
+  const float* campos = nullptr;
+  float tanx = 0.f, tany = 0.f;
+};
+
+struct Forward {  // one forward's problem, arenas and launch context, shared by its stages
   Problem pb;
   GeomState gs;
   ImgState im;
-  BinState bs;
-  long long R;
+  Allocators al;
+  float* out_color;
+  MseFwd mse;
+  cudaStream_t st;
+  int debug;
+  size_t N, ntiles;  // view-Gaussians, view-tiles
+  dim3 pgrid() const { return dim3(ceil_div(pb.P, 256), pb.NV); }
 };
 
-static int run_forward(Problem pb, bool build_cams, const float* c2w, const float* fxfycxcy, const float* view,
-                       const float* proj, const float* campos, float tanx, float tany, dgs_alloc_fn geom_alloc,
-                       void* geom_user, dgs_alloc_fn bin_alloc, void* bin_user, dgs_alloc_fn img_alloc,
-                       void* img_user, float* out_color, int* radii, long long* R_out, long long chunk_R[2],
-                       cudaStream_t st, int debug, MseFwd mse = MseFwd()) {
-  const size_t N = (size_t)pb.NV * pb.P;
-  DGS_REQUIRE(N < (size_t)INT32_MAX, "n_views * P = %zu does not fit the 32-bit scan", N);
-  size_t gbytes = 0, ibytes = 0;
-  GeomState::carve(nullptr, pb.NV, pb.P, &gbytes);
-  ImgState::carve(nullptr, pb.NV, pb.W, pb.H, &ibytes);
-  void* gbuf = geom_alloc(gbytes, geom_user);
-  void* ibuf = img_alloc(ibytes, img_user);
-  if (!gbuf || !ibuf) { set_error("arena allocator returned NULL"); return DGS_ERR_ALLOC; }
-  GeomState gs = GeomState::carve(gbuf, pb.NV, pb.P, nullptr);
-  ImgState im = ImgState::carve(ibuf, pb.NV, pb.W, pb.H, nullptr);
+static int alloc_binning(const Forward& f, long long R, BinState* bs) {
+  size_t bytes = 0;
+  BinState::carve(nullptr, R, &bytes);
+  void* buf = f.al.bin(bytes, f.al.bin_user);
+  if (!buf) { set_error("binning allocator returned NULL"); return DGS_ERR_ALLOC; }
+  *bs = BinState::carve(buf, R, nullptr);
+  return DGS_OK;
+}
 
-  // small scenes: try the per-tile path first (decided after the one host sync, when the longest tile list is known)
-  const size_t ntiles_all = (size_t)pb.NV * pb.tiles;
-  static int small_on = -1;
-  if (small_on < 0) {
-    const char* e = getenv("DGS_RASTER_SMALL");
-    small_on = (e && e[0] == '0') ? 0 : 1;
-  }
-  const bool small_try = small_on && N <= (size_t)SMALL_MAX_N && ntiles_all <= (size_t)SMALL_MAX_TILES;
-  if (small_try) DGS_CUDA_OK(cudaMemsetAsync(im.tile_open, 0, ntiles_all * sizeof(uint32_t), st));
-  if (build_cams) {
-    build_cameras_kernel<<<ceil_div(pb.NV, 64), 64, 0, st>>>(pb.NV, c2w, fxfycxcy, pb.W, pb.H, gs.cams);
+template <int MODE>
+static int blend_forward(const Forward& f, const uint32_t* point_list) {
+  ProfScope ps(f.st, PROF_RASTER_BLEND_FWD);
+  blend_forward_kernel<MODE><<<(unsigned)f.ntiles, TILE_PIX, 0, f.st>>>(f.pb, f.gs, f.im, point_list, f.out_color, f.mse);
+  DGS_LAUNCH_OK(f.st, f.debug);
+  return DGS_OK;
+}
+
+static int project(const Forward& f, const CameraInput& cam, int* radii) {
+  if (cam.c2w) {
+    build_cameras_kernel<<<ceil_div(f.pb.NV, 64), 64, 0, f.st>>>(f.pb.NV, cam.c2w, cam.fxfycxcy, f.pb.W, f.pb.H, f.gs.cams);
   } else {
-    pack_camera_kernel<<<1, 32, 0, st>>>(view, proj, campos, tanx, tany, pb.W, pb.H, gs.cams);
+    pack_camera_kernel<<<1, 32, 0, f.st>>>(cam.view, cam.proj, cam.campos, cam.tanx, cam.tany, f.pb.W, f.pb.H, f.gs.cams);
   }
-  DGS_LAUNCH_OK(st, debug);
-  dim3 pgrid(ceil_div(pb.P, 256), pb.NV);
+  DGS_LAUNCH_OK(f.st, f.debug);
+  ProfScope ps(f.st, PROF_RASTER_PROJECT);
+  project_kernel<<<f.pgrid(), 256, 0, f.st>>>(f.pb, f.gs, radii);
+  DGS_LAUNCH_OK(f.st, f.debug);
+  return DGS_OK;
+}
+
+// Small-scene binning and blend.  *done = false: a tile list is longer than the shared-memory sort takes, and the
+// caller bins globally instead (the projection's outputs stand).
+static int bin_small(const Forward& f, long long* R_out, bool* done) {
+  // no phase B on this path: its image arrays hold the per-tile instance counts and the fill cursors
+  uint32_t* tile_counts = f.im.tile_open;
+  uint2* fill_cursor = f.im.ranges_b;
+  BinTotals tot;
+  DGS_CUDA_OK(cudaMemsetAsync(tile_counts, 0, f.ntiles * sizeof(uint32_t), f.st));
   {
-    ProfScope ps(st, PROF_RASTER_PROJECT);
-    project_kernel<<<pgrid, 256, 0, st>>>(pb, gs, radii);
-    DGS_LAUNCH_OK(st, debug);
+    ProfScope ps(f.st, PROF_RASTER_SCAN);
+    tile_count_fill_kernel<false><<<f.pgrid(), 256, 0, f.st>>>(f.pb, f.gs, tile_counts, nullptr, nullptr, nullptr);
+    DGS_LAUNCH_OK(f.st, f.debug);
+    tile_scan_kernel<<<1, 1024, 0, f.st>>>((int)f.ntiles, tile_counts, f.im.ranges, fill_cursor, f.gs.totals);
+    DGS_LAUNCH_OK(f.st, f.debug);
+    DGS_CUDA_OK(cudaMemcpyAsync(&tot, f.gs.totals, sizeof(tot), cudaMemcpyDeviceToHost, f.st));
+    DGS_CUDA_OK(cudaStreamSynchronize(f.st));  // the one host sync of the batch
   }
-  if (small_try) {
-    uint32_t tot[6] = {0, 0, 0, 0, 0, 0};
+  *done = tot.longest <= (uint32_t)SMALL_TILE_CAP;
+  if (!*done) return DGS_OK;
+  const long long R = (long long)tot.R;
+  *R_out = R;
+  BinState bs;
+  int rc = alloc_binning(f, R, &bs);
+  if (rc) return rc;
+  if (R > 0) {
     {
-      ProfScope ps(st, PROF_RASTER_SCAN);
-      tile_count_fill_kernel<false><<<pgrid, 256, 0, st>>>(pb, gs, im.tile_open, nullptr, nullptr, nullptr);
-      DGS_LAUNCH_OK(st, debug);
-      tile_scan_kernel<<<1, 1024, 0, st>>>((int)ntiles_all, im.tile_open, im.ranges, im.ranges_b, gs.totals);
-      DGS_LAUNCH_OK(st, debug);
-      DGS_CUDA_OK(cudaMemcpyAsync(tot, gs.totals, 6 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-      DGS_CUDA_OK(cudaStreamSynchronize(st));  // the one host sync of the batch
+      ProfScope ps(f.st, PROF_RASTER_EMIT);
+      tile_count_fill_kernel<true><<<f.pgrid(), 256, 0, f.st>>>(f.pb, f.gs, nullptr, fill_cursor, bs.keys_in, bs.vals_in);
+      DGS_LAUNCH_OK(f.st, f.debug);
     }
-    if (tot[3] <= (uint32_t)SMALL_TILE_CAP) {
-      const long long R = (long long)tot[0];
-      *R_out = R;
-      chunk_R[0] = R;
-      chunk_R[1] = 0;
-      size_t bbytes = 0;
-      BinState::carve(nullptr, R, &bbytes);
-      void* bbuf = bin_alloc(bbytes, bin_user);
-      if (!bbuf) { set_error("binning allocator returned NULL"); return DGS_ERR_ALLOC; }
-      BinState bs = BinState::carve(bbuf, R, nullptr);
-      if (R > 0) {
-        {
-          ProfScope ps(st, PROF_RASTER_EMIT);
-          tile_count_fill_kernel<true><<<pgrid, 256, 0, st>>>(pb, gs, nullptr, im.ranges_b, bs.keys_in, bs.vals_in);
-          DGS_LAUNCH_OK(st, debug);
-        }
-        {
-          ProfScope ps(st, PROF_RASTER_SORT);
-          int cap = 2;
-          while (cap < (int)tot[3]) cap <<= 1;
-          static bool configured = false;
-          if (!configured) {
-            DGS_CUDA_OK(cudaFuncSetAttribute(tile_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMALL_TILE_CAP * 8));
-            configured = true;
-          }
-          tile_sort_kernel<<<(unsigned)ntiles_all, 256, (size_t)cap * 8, st>>>(im.ranges, bs.keys_in, bs.vals_in, bs.point_list);
-          DGS_LAUNCH_OK(st, debug);
-        }
-      }
-      ProfScope ps(st, PROF_RASTER_BLEND_FWD);
-      blend_forward_kernel<0><<<(unsigned)ntiles_all, TILE_PIX, 0, st>>>(pb, gs, im, bs.point_list, out_color, mse);
-      DGS_LAUNCH_OK(st, debug);
-      return DGS_OK;
+    ProfScope ps(f.st, PROF_RASTER_SORT);
+    int cap = 2;
+    while (cap < (int)tot.longest) cap <<= 1;
+    static bool configured = false;
+    if (!configured) {
+      DGS_CUDA_OK(cudaFuncSetAttribute(tile_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMALL_TILE_CAP * 8));
+      configured = true;
     }
-    // a tile list longer than the shared-memory sort takes: continue on the global path (the projection's outputs stand)
+    tile_sort_kernel<<<(unsigned)f.ntiles, 256, (size_t)cap * 8, f.st>>>(f.im.ranges, bs.keys_in, bs.vals_in, bs.point_list);
+    DGS_LAUNCH_OK(f.st, f.debug);
   }
-  {
-    ProfScope ps(st, PROF_RASTER_SCAN);  // per-view depth ranking + instance offsets in rank order
-    const int depth_end_bit = 32 + bits_for((uint32_t)pb.NV);
-    DGS_CUDA_OK(cub::DeviceRadixSort::SortPairs(gs.scan_temp, gs.scan_bytes, gs.dkey_in, gs.dkey, gs.perm_in, gs.perm,
-                                                (int)N, 0, depth_end_bit, st));
-    DGS_CUDA_OK(cudaMemsetAsync(gs.totals, 0, 6 * sizeof(uint32_t), st));
-    gather_tiles_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(N, pb.P, gs);
-    DGS_LAUNCH_OK(st, debug);
-    DGS_CUDA_OK(cub::DeviceScan::InclusiveSum(gs.scan_temp, gs.scan_bytes, gs.tiles_sorted, gs.offsets, (int)N, st));
-  }
-  // two-phase binning candidates need the near/far split of the instance counts; it rides on the same single sync
-  // near_log2 < 0 = adaptive: the splits at 1/8 and 1/16 are both prepared (two 1-thread kernels) and the host picks after
-  // the sync: 1/16 when its near lists are still long enough to saturate the pixels (>= 2048 entries per tile on average:
-  // the dense random-init step), 1/8 otherwise (sparser lists leave the near pass short of work)
+  return blend_forward<0>(f, bs.point_list);
+}
+
+// per-view depth ranking of the Gaussians, and the instance offsets in rank order
+static int rank_and_scan(const Forward& f) {
+  ProfScope ps(f.st, PROF_RASTER_SCAN);
+  GeomState gs = f.gs;  // (cub takes the temp size by reference)
+  const int depth_end_bit = 32 + bits_for((uint32_t)f.pb.NV);
+  DGS_CUDA_OK(cub::DeviceRadixSort::SortPairs(gs.scan_temp, gs.scan_bytes, gs.dkey_in, gs.dkey, gs.perm_in, gs.perm,
+                                              (int)f.N, 0, depth_end_bit, f.st));
+  DGS_CUDA_OK(cudaMemsetAsync(gs.totals, 0, sizeof(BinTotals), f.st));
+  gather_tiles_kernel<<<(unsigned)((f.N + 255) / 256), 256, 0, f.st>>>(f.N, f.pb.P, gs);
+  DGS_LAUNCH_OK(f.st, f.debug);
+  DGS_CUDA_OK(cub::DeviceScan::InclusiveSum(gs.scan_temp, gs.scan_bytes, gs.tiles_sorted, gs.offsets, (int)f.N, f.st));
+  return DGS_OK;
+}
+
+struct Split {                // how the global path bins
+  long long R;                // instances of the batch
+  long long RA;               // instances of the first (or only) bin pass
+  int Pn;                     // two-phase: near ranks per view binned in phase A; 0: one pass over every rank
+  const uint32_t* near_meta;  // two-phase: chunk_meta_kernel's output for Pn
+};
+
+// The split decision, after the one host sync of the global path.  near_log2 > 0: phase A = the nearest P >> near_log2
+// Gaussians of every view; 0: single pass; < 0 adaptive: the splits at 1/8 and 1/16 are both prepared and the host picks
+// 1/16 when its near lists are still long enough to saturate the pixels (>= 2048 entries per tile on average: the dense
+// random-init step), 1/8 otherwise (sparser lists leave the near pass short of work).  Phase A must be a real saving:
+// at most half of the instances, in a batch of at least 2^21.
+static int plan_split(const Forward& f, Split* sp) {
+  const Problem& pb = f.pb;
+  const GeomState& gs = f.gs;
   const bool adaptive = pb.near_log2 < 0;
   const int k_a = adaptive ? 3 : pb.near_log2;
   int Pn = (k_a > 0) ? (pb.P >> k_a) : 0;
   const int Pn_b = adaptive ? (pb.P >> 4) : 0;
   const bool may_split = Pn >= 1024;
   const bool two_cands = adaptive && Pn_b >= 1024;
-  uint32_t tot[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  uint32_t* const meta_b = gs.view_meta + (size_t)pb.NV * 2;
+  BinTotals tot = {};
   if (may_split) {
-    chunk_meta_kernel<<<1, 32, 0, st>>>(pb.NV, pb.P, Pn, gs.offsets, gs.view_meta, gs.totals, 1);
-    if (two_cands) chunk_meta_kernel<<<1, 32, 0, st>>>(pb.NV, pb.P, Pn_b, gs.offsets, gs.view_meta + (size_t)pb.NV * 4, gs.totals, 6);
-    DGS_LAUNCH_OK(st, debug);
-    DGS_CUDA_OK(cudaMemcpyAsync(tot, gs.totals, 8 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    chunk_meta_kernel<<<1, 32, 0, f.st>>>(pb.NV, pb.P, Pn, gs.offsets, gs.view_meta, gs.totals, &gs.totals->R_near);
+    if (two_cands) chunk_meta_kernel<<<1, 32, 0, f.st>>>(pb.NV, pb.P, Pn_b, gs.offsets, meta_b, gs.totals, &gs.totals->R_near_b);
+    DGS_LAUNCH_OK(f.st, f.debug);
+    DGS_CUDA_OK(cudaMemcpyAsync(&tot, gs.totals, sizeof(tot), cudaMemcpyDeviceToHost, f.st));
   } else {
-    DGS_CUDA_OK(cudaMemcpyAsync(tot, gs.offsets + N - 1, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-    DGS_CUDA_OK(cudaMemcpyAsync(tot + 4, gs.totals + 4, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    DGS_CUDA_OK(cudaMemcpyAsync(&tot.R, gs.offsets + f.N - 1, sizeof(tot.R), cudaMemcpyDeviceToHost, f.st));
+    DGS_CUDA_OK(cudaMemcpyAsync(&tot.R64, &gs.totals->R64, sizeof(tot.R64), cudaMemcpyDeviceToHost, f.st));
   }
-  DGS_CUDA_OK(cudaStreamSynchronize(st));  // the one host sync per batch (two-phase: a second, after phase A)
-  const long long R64 = (long long)(((unsigned long long)tot[5] << 32) | tot[4]);  // exact, never wrapped
-  if (R64 >= (long long)INT32_MAX) {
-    set_error("instance count %lld exceeds 2^31-1 (render the views in smaller batches)", R64);
+  DGS_CUDA_OK(cudaStreamSynchronize(f.st));  // the one host sync per batch (two-phase: a second, after phase A)
+  if (tot.R64 >= (unsigned long long)INT32_MAX) {
+    set_error("instance count %lld exceeds 2^31-1 (render the views in smaller batches)", (long long)tot.R64);
     return DGS_ERR_OVERFLOW;
   }
-  const long long R = (long long)tot[0];
-  *R_out = R;
-  if (two_cands && (unsigned long long)tot[6] >= 2048ull * (unsigned long long)pb.NV * pb.tiles) {
-    Pn = Pn_b;          // the 1/16 split: its per-view instance offsets are the second view_meta set
-    tot[1] = tot[6];
-    gs.view_meta += (size_t)pb.NV * 4;
+  const long long R = (long long)tot.R;
+  uint32_t R_near = tot.R_near;
+  const uint32_t* near_meta = gs.view_meta;
+  if (two_cands && (unsigned long long)tot.R_near_b >= 2048ull * (unsigned long long)pb.NV * pb.tiles) {
+    Pn = Pn_b;
+    R_near = tot.R_near_b;
+    near_meta = meta_b;
   }
-  // phase A must be a real saving: at most half of the instances
-  const bool split = may_split && R >= (1ll << 21) && 2ll * tot[1] <= R && tot[1] > 0;
-  const long long RA = split ? (long long)tot[1] : R;
-  (void)0;  // (the far instance count R - RA is an upper bound only: phase B bins the open tiles)
-  chunk_R[0] = RA;
-  chunk_R[1] = 0;
-
-  const size_t ntiles = (size_t)pb.NV * pb.tiles;
-  const int end_bit = bits_for((uint32_t)ntiles);  // tile ids only: depth order is already in the emission order
-  // one binning pass over a rank range into its own arena: emit -> stable tile sort -> tile ranges
-  auto bin_pass = [&](long long Rp, int phase, int rank_lo, int rank_hi, uint2* ranges, BinState* out_bs) -> int {
-    size_t bbytes = 0;
-    BinState::carve(nullptr, Rp, &bbytes);
-    void* bbuf = bin_alloc(bbytes, bin_user);
-    if (!bbuf) { set_error("binning allocator returned NULL"); return DGS_ERR_ALLOC; }
-    BinState bs = BinState::carve(bbuf, Rp, nullptr);
-    *out_bs = bs;
-    DGS_CUDA_OK(cudaMemsetAsync(ranges, 0, ntiles * sizeof(uint2), st));
-    if (Rp > 0) {
-      {
-        ProfScope ps(st, PROF_RASTER_EMIT);
-        dim3 egrid(ceil_div(rank_hi - rank_lo, 256), pb.NV);
-        emit_keys_kernel<<<egrid, 256, 0, st>>>(pb, gs, bs.keys_in, bs.vals_in, phase, rank_lo, rank_hi);
-        DGS_LAUNCH_OK(st, debug);
-      }
-      {
-        ProfScope ps(st, PROF_RASTER_SORT);
-        DGS_CUDA_OK(cub::DeviceRadixSort::SortPairs(bs.sort_temp, bs.sort_bytes, bs.keys_in, bs.keys, bs.vals_in,
-                                                    bs.point_list, (int)Rp, 0, end_bit, st));
-      }
-      {
-        ProfScope ps(st, PROF_RASTER_RANGES);
-        tile_ranges_kernel<<<(unsigned)((Rp + 255) / 256), 256, 0, st>>>(Rp, bs.keys, ranges);
-        DGS_LAUNCH_OK(st, debug);
-      }
-    }
-    return DGS_OK;
-  };
-
-  BinState bsa, bsb;
-  if (!split) {
-    int rc = bin_pass(R, 0, 0, pb.P, im.ranges, &bsa);
-    if (rc) return rc;
-    ProfScope ps(st, PROF_RASTER_BLEND_FWD);
-    blend_forward_kernel<0><<<(unsigned)ntiles, TILE_PIX, 0, st>>>(pb, gs, im, bsa.point_list, out_color, mse);
-    DGS_LAUNCH_OK(st, debug);
-    return DGS_OK;
-  }
-  // ---- phase A: the nearest Pn Gaussians of every view.  In dense scenes every pixel saturates here and the
-  // remaining (1 - 2^-near_log2) of the instances are never emitted, sorted or read.
-  {
-    int rc = bin_pass(RA, 1, 0, Pn, im.ranges, &bsa);
-    if (rc) return rc;
-    ProfScope ps(st, PROF_RASTER_BLEND_FWD);
-    blend_forward_kernel<1><<<(unsigned)ntiles, TILE_PIX, 0, st>>>(pb, gs, im, bsa.point_list, out_color, mse);
-    DGS_LAUNCH_OK(st, debug);
-  }
-  uint32_t unfinished = 0;
-  DGS_CUDA_OK(cudaMemcpyAsync(&unfinished, gs.totals + 2, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-  DGS_CUDA_OK(cudaStreamSynchronize(st));
-  if (unfinished == 0) return DGS_OK;
-  // ---- phase B: everything behind the near ranks, for the OPEN tiles only, continuing from the saved per-pixel state.
-  // A tile that saturated in phase A never looks at its far entries, so they are neither counted, emitted nor sorted;
-  // an open tile gets every far Gaussian of its rect, in the same (depth, index) order as the single-pass list.
-  {
-    uint32_t rb = 0;
-    {
-      ProfScope ps(st, PROF_RASTER_SCAN);
-      count_open_kernel<<<dim3(ceil_div(pb.P, 256), pb.NV), 256, 0, st>>>(pb, gs, im.tile_open, Pn);
-      DGS_LAUNCH_OK(st, debug);
-      DGS_CUDA_OK(cub::DeviceScan::InclusiveSum(gs.scan_temp, gs.scan_bytes, gs.open_counts, gs.open_offsets, (int)N, st));
-      DGS_CUDA_OK(cudaMemcpyAsync(&rb, gs.open_offsets + N - 1, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-      DGS_CUDA_OK(cudaStreamSynchronize(st));
-    }
-    const long long RBo = (long long)rb;
-    size_t bbytes = 0;
-    BinState::carve(nullptr, RBo, &bbytes);
-    void* bbuf = bin_alloc(bbytes, bin_user);
-    if (!bbuf) { set_error("binning allocator returned NULL"); return DGS_ERR_ALLOC; }
-    bsb = BinState::carve(bbuf, RBo, nullptr);
-    DGS_CUDA_OK(cudaMemsetAsync(im.ranges_b, 0, ntiles * sizeof(uint2), st));
-    if (RBo > 0) {
-      {
-        ProfScope ps(st, PROF_RASTER_EMIT);
-        emit_open_keys_kernel<<<dim3(ceil_div(pb.P - Pn, 256), pb.NV), 256, 0, st>>>(pb, gs, im.tile_open, bsb.keys_in,
-                                                                                     bsb.vals_in, Pn);
-        DGS_LAUNCH_OK(st, debug);
-      }
-      {
-        ProfScope ps(st, PROF_RASTER_SORT);
-        DGS_CUDA_OK(cub::DeviceRadixSort::SortPairs(bsb.sort_temp, bsb.sort_bytes, bsb.keys_in, bsb.keys, bsb.vals_in,
-                                                    bsb.point_list, (int)RBo, 0, end_bit, st));
-      }
-      {
-        ProfScope ps(st, PROF_RASTER_RANGES);
-        tile_ranges_kernel<<<(unsigned)((RBo + 255) / 256), 256, 0, st>>>(RBo, bsb.keys, im.ranges_b);
-        DGS_LAUNCH_OK(st, debug);
-      }
-    }
-    chunk_R[1] = RBo;
-    ProfScope ps(st, PROF_RASTER_BLEND_FWD);
-    blend_forward_kernel<2><<<(unsigned)ntiles, TILE_PIX, 0, st>>>(pb, gs, im, bsb.point_list, out_color, mse);
-    DGS_LAUNCH_OK(st, debug);
-  }
+  const bool split = may_split && R >= (1ll << 21) && 2ll * R_near <= R && R_near > 0;
+  sp->R = R;
+  sp->RA = split ? (long long)R_near : R;
+  sp->Pn = split ? Pn : 0;
+  sp->near_meta = split ? near_meta : nullptr;
   return DGS_OK;
+}
+
+struct Emission {             // which instances a bin pass emits
+  int rank_lo, rank_hi;       // depth ranks of every view
+  bool open_only;             // phase B: only the tiles still open after phase A
+  const uint32_t* near_meta;  // phase A: rebase into the compact near buffer (Split::near_meta)
+};
+
+// One binning pass into its own arena: allocate -> zero the ranges -> emit -> stable sort by tile -> tile ranges
+static int bin_pass(const Forward& f, long long R, const Emission& e, uint2* ranges, BinState* bs) {
+  int rc = alloc_binning(f, R, bs);
+  if (rc) return rc;
+  DGS_CUDA_OK(cudaMemsetAsync(ranges, 0, f.ntiles * sizeof(uint2), f.st));
+  if (R == 0) return DGS_OK;
+  {
+    ProfScope ps(f.st, PROF_RASTER_EMIT);
+    const dim3 grid(ceil_div(e.rank_hi - e.rank_lo, 256), f.pb.NV);
+    if (e.open_only)
+      emit_keys_kernel<true><<<grid, 256, 0, f.st>>>(f.pb, f.gs, f.im.tile_open, nullptr, bs->keys_in, bs->vals_in,
+                                                     e.rank_lo, e.rank_hi);
+    else
+      emit_keys_kernel<false><<<grid, 256, 0, f.st>>>(f.pb, f.gs, nullptr, e.near_meta, bs->keys_in, bs->vals_in,
+                                                      e.rank_lo, e.rank_hi);
+    DGS_LAUNCH_OK(f.st, f.debug);
+  }
+  {
+    ProfScope ps(f.st, PROF_RASTER_SORT);  // tile ids only: depth order is already in the emission order
+    DGS_CUDA_OK(cub::DeviceRadixSort::SortPairs(bs->sort_temp, bs->sort_bytes, bs->keys_in, bs->keys, bs->vals_in,
+                                                bs->point_list, (int)R, 0, bits_for((uint32_t)f.ntiles), f.st));
+  }
+  ProfScope ps(f.st, PROF_RASTER_RANGES);
+  tile_ranges_kernel<<<(unsigned)((R + 255) / 256), 256, 0, f.st>>>(R, bs->keys, ranges);
+  DGS_LAUNCH_OK(f.st, f.debug);
+  return DGS_OK;
+}
+
+// Two-phase binning.  Phase A: the nearest Pn Gaussians of every view.  In dense scenes every pixel saturates here and
+// the remaining instances are never emitted, sorted or read.  Phase B: everything behind the near ranks, for the OPEN
+// tiles only, continuing from the saved per-pixel state.  A tile that saturated in phase A never looks at its far
+// entries, so they are neither counted, emitted nor sorted; an open tile gets every far Gaussian of its rect, in the
+// same (depth, index) order as the single-pass list.
+static int bin_two_phase(const Forward& f, const Split& sp, long long* R_far) {
+  BinState bsa, bsb;
+  int rc = bin_pass(f, sp.RA, Emission{0, sp.Pn, false, sp.near_meta}, f.im.ranges, &bsa);
+  if (rc) return rc;
+  rc = blend_forward<1>(f, bsa.point_list);
+  if (rc) return rc;
+  uint32_t unfinished = 0, rb = 0;
+  DGS_CUDA_OK(cudaMemcpyAsync(&unfinished, &f.gs.totals->unfinished, sizeof(uint32_t), cudaMemcpyDeviceToHost, f.st));
+  DGS_CUDA_OK(cudaStreamSynchronize(f.st));
+  if (unfinished == 0) return DGS_OK;
+  {
+    ProfScope ps(f.st, PROF_RASTER_SCAN);
+    count_open_kernel<<<f.pgrid(), 256, 0, f.st>>>(f.pb, f.gs, f.im.tile_open, sp.Pn);
+    DGS_LAUNCH_OK(f.st, f.debug);
+    size_t scan_bytes = f.gs.scan_bytes;
+    DGS_CUDA_OK(cub::DeviceScan::InclusiveSum(f.gs.scan_temp, scan_bytes, f.gs.open_counts, f.gs.open_offsets, (int)f.N,
+                                              f.st));
+    DGS_CUDA_OK(cudaMemcpyAsync(&rb, f.gs.open_offsets + f.N - 1, sizeof(uint32_t), cudaMemcpyDeviceToHost, f.st));
+    DGS_CUDA_OK(cudaStreamSynchronize(f.st));
+  }
+  rc = bin_pass(f, rb, Emission{sp.Pn, f.pb.P, true, nullptr}, f.im.ranges_b, &bsb);
+  if (rc) return rc;
+  *R_far = rb;
+  return blend_forward<2>(f, bsb.point_list);
+}
+
+// projection -> small-scene binning, or depth ranking and scan -> split decision -> bin pass(es) + blend
+static int run_forward(Problem pb, const CameraInput& cam, const Allocators& al, float* out_color, int* radii,
+                       long long* R_out, long long chunk_R[2], cudaStream_t st, int debug, MseFwd mse = MseFwd()) {
+  Forward f;
+  f.pb = pb; f.al = al; f.out_color = out_color; f.mse = mse; f.st = st; f.debug = debug;
+  f.N = (size_t)pb.NV * pb.P;
+  f.ntiles = (size_t)pb.NV * pb.tiles;
+  DGS_REQUIRE(f.N < (size_t)INT32_MAX, "n_views * P = %zu does not fit the 32-bit scan", f.N);
+  size_t gbytes = 0, ibytes = 0;
+  GeomState::carve(nullptr, pb.NV, pb.P, &gbytes);
+  ImgState::carve(nullptr, pb.NV, pb.W, pb.H, &ibytes);
+  void* gbuf = al.geom(gbytes, al.geom_user);
+  void* ibuf = al.img(ibytes, al.img_user);
+  if (!gbuf || !ibuf) { set_error("arena allocator returned NULL"); return DGS_ERR_ALLOC; }
+  f.gs = GeomState::carve(gbuf, pb.NV, pb.P, nullptr);
+  f.im = ImgState::carve(ibuf, pb.NV, pb.W, pb.H, nullptr);
+
+  int rc = project(f, cam, radii);
+  if (rc) return rc;
+  chunk_R[1] = 0;
+  if (f.N <= (size_t)SMALL_MAX_N && f.ntiles <= (size_t)SMALL_MAX_TILES) {
+    bool done = false;
+    rc = bin_small(f, R_out, &done);
+    if (rc || done) {
+      chunk_R[0] = *R_out;
+      return rc;
+    }
+  }
+  rc = rank_and_scan(f);
+  if (rc) return rc;
+  Split sp;
+  rc = plan_split(f, &sp);
+  if (rc) return rc;
+  *R_out = sp.R;
+  chunk_R[0] = sp.RA;
+  if (sp.Pn > 0) return bin_two_phase(f, sp, &chunk_R[1]);
+  BinState bs;
+  rc = bin_pass(f, sp.R, Emission{0, pb.P, false, nullptr}, f.im.ranges, &bs);
+  if (rc) return rc;
+  return blend_forward<0>(f, bs.point_list);
 }
 
 static Problem make_problem(int NV, int V, int P, int D, int M, int W, int H, int raw, float mod) {
@@ -1818,9 +1831,11 @@ int dgs_raster_forward(const dgs_raster_args* a, dgs_alloc_fn geom_alloc, void* 
   DGS_CUDA_OK(cudaStreamSynchronize(st));
   Problem pb = single_problem(a, bg);
   long long R = 0, chunk_R[2] = {0, 0};
-  rc = run_forward(pb, false, nullptr, nullptr, a->viewmatrix, a->projmatrix, a->campos, a->tan_fovx, a->tan_fovy,
-                   geom_alloc, geom_user, bin_alloc, bin_user, img_alloc, img_user, out_color, radii, &R, chunk_R, st,
-                   a->debug);
+  CameraInput cam;
+  cam.view = a->viewmatrix; cam.proj = a->projmatrix; cam.campos = a->campos;
+  cam.tanx = a->tan_fovx; cam.tany = a->tan_fovy;
+  const Allocators al = {geom_alloc, geom_user, bin_alloc, bin_user, img_alloc, img_user};
+  rc = run_forward(pb, cam, al, out_color, radii, &R, chunk_R, st, a->debug);
   *num_rendered = (int)R;
   return rc;
 }
@@ -1907,9 +1922,11 @@ int dgs_render_batch_forward_mse(const dgs_render_batch_args* a, dgs_alloc_fn ge
     mf.target = mse->target; mf.tc = mse->target_channels; mf.loss = mse->loss_sum;
   }
   Problem pb = batch_problem(a);
-  return run_forward(pb, true, a->c2w, a->fxfycxcy, nullptr, nullptr, nullptr, 0.f, 0.f, geom_alloc, geom_user,
-                     bin_alloc, bin_user, img_alloc, img_user, out_images, nullptr, num_rendered, chunk_instances,
-                     (cudaStream_t)stream, a->debug, mf);
+  CameraInput cam;
+  cam.c2w = a->c2w; cam.fxfycxcy = a->fxfycxcy;
+  const Allocators al = {geom_alloc, geom_user, bin_alloc, bin_user, img_alloc, img_user};
+  return run_forward(pb, cam, al, out_images, nullptr, num_rendered, chunk_instances, (cudaStream_t)stream, a->debug,
+                     mf);
 }
 
 int dgs_render_batch_backward(const dgs_render_batch_args* a, long long R, const long long* chunk_instances,

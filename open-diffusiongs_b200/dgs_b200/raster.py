@@ -148,12 +148,6 @@ def mark_visible(means3D, viewmatrix, projmatrix):
 # ------------------------------------------------------------------------------------------------
 # batched renderer
 # ------------------------------------------------------------------------------------------------
-import os as _os
-
-# two-phase binning: phase A = the nearest 1/2^k of every view's Gaussians (0 = single pass); DGS_RASTER_NEAR_LOG2 overrides
-DEFAULT_NEAR_LOG2 = int(_os.environ.get("DGS_RASTER_NEAR_LOG2", "-1"))  # -1 = adaptive: 1/8, or 1/16 for dense scenes
-
-
 def _batch_args(xyz, features, scaling, rotation, opacity, C2W, fxfycxcy, H, W, scale_modifier, debug=False,
                 near_log2=0):
     B, P = xyz.shape[0], xyz.shape[1]
@@ -212,7 +206,8 @@ def _render_batch_forward_one(xyz, features, scaling, rotation, opacity, H, W, C
     with torch.cuda.device(dev):
         out = torch.empty(B, V, 3, int(H), int(W), dtype=torch.float32, device=dev)
         geom, binning, img = (_Arena(dev, arena_cache, k) for k in ("geom", "binning", "img"))
-        near_log2 = DEFAULT_NEAR_LOG2 if near_log2 is None else near_log2
+        # two-phase binning: phase A = the nearest 1/2^k of every view's Gaussians (0 = single pass, -1 = adaptive)
+        near_log2 = -1 if near_log2 is None else near_log2
         a = _batch_args(*tens, H, W, scale_modifier, near_log2=near_log2)
         R = C.c_longlong(0)
         chunks = (C.c_longlong * 2)(0, 0)
