@@ -209,8 +209,7 @@ int block_forward(const dgs_dit_weights* w, const dgs_dit_weights_fp8* w8, int l
   const int B = d.B, N = d.N, M = d.M, D = d.D, U = d.U, ms = d.mod_stride;
   {
     ProfScope ps(st, PROF_DIT_LN);
-    if (w8) DGS_TRY(ln_modulate_fp8(b.x_in, m, m + D, ms, (uint8_t*)b.h1, b.sa_h, B, N, D, 1e-6f, st));
-    else DGS_TRY(ln_modulate(b.x_in, nullptr, m, m + D, ms, b.h1, B, N, 0, N, D, 1e-6f, 0, st));
+    DGS_TRY(ln_forward(w8 ? LN_E4M3 : LN_BF16, b.x_in, nullptr, m, m + D, ms, b.h1, b.sa_h, B, N, 0, N, D, 1e-6f, st));
   }
   {
     ProfScope ps(st, PROF_DIT_GEMM_QKV);
@@ -236,8 +235,8 @@ int block_forward(const dgs_dit_weights* w, const dgs_dit_weights_fp8* w8, int l
   }
   {
     ProfScope ps(st, PROF_DIT_LN);
-    if (w8) DGS_TRY(ln_modulate_fp8(b.x_mid, m + 3 * D, m + 4 * D, ms, (uint8_t*)b.h2, b.sa_h, B, N, D, 1e-6f, st));
-    else DGS_TRY(ln_modulate(b.x_mid, nullptr, m + 3 * D, m + 4 * D, ms, b.h2, B, N, 0, N, D, 1e-6f, 0, st));
+    DGS_TRY(ln_forward(w8 ? LN_E4M3 : LN_BF16, b.x_mid, nullptr, m + 3 * D, m + 4 * D, ms, b.h2, b.sa_h, B, N, 0, N, D,
+                       1e-6f, st));
   }
   {
     ProfScope ps(st, PROF_DIT_GEMM_FC1);
@@ -293,7 +292,8 @@ int dit_forward(const dgs_dit_weights* w, const dgs_dit_weights_fp8* w8, const d
   }
   DGS_TRY(assemble_tokens(ws.tok, w->pos_embed, x0, B, G, T, D, st));
   if (train) DGS_CUDA_OK(cudaMemcpyAsync(ts.x_pre, x0, d.MD * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  DGS_TRY(ln_weight_inplace(x0, w->in_ln_w, d.M, D, 1e-5f, st));  // nn.LayerNorm default eps (denoiser.py:234-236)
+  // in place, nn.LayerNorm's default eps (denoiser.py:234-236)
+  DGS_TRY(ln_forward(LN_F32, x0, w->in_ln_w, nullptr, nullptr, 0, x0, nullptr, 1, d.M, 0, d.M, D, 1e-5f, st));
   if (g_prof_on) { prof_end(st, PROF_DIT_INPUT); prof_begin(st, PROF_DIT_COND); }
 
   // ---- conditioning: timestep MLP, then the adaLN modulation of ALL blocks and both heads in one launch ----
@@ -321,13 +321,13 @@ int dit_forward(const dgs_dit_weights* w, const dgs_dit_weights_fp8* w8, const d
   const float* mu = ws.mod + (size_t)L * 6 * D;  // upsampler: shift | scale
   const float* md = mu + 2 * D;                  // image_token_decoder: shift | scale
   if (G > 0) {
-    DGS_TRY(ln_modulate(x_fin, w->ups_ln_w, mu, mu + D, mod_stride, ws.hg, B, N, 0, G, D, 1e-5f, 1, st));
+    DGS_TRY(ln_forward(LN_SPLIT_BF16, x_fin, w->ups_ln_w, mu, mu + D, mod_stride, ws.hg, nullptr, B, N, 0, G, D, 1e-5f, st));
     DGS_TRY(tiny_linear_bf16(ws.hg, (const __nv_bfloat16*)w->ups_w, ws.gs_tok, B * G, 14, 3 * D, st));
   }
   // the decoder head runs split-bf16 (K = 3*width) so the Gaussian parameters are fp32-accurate functions of the
   // residual stream; its A operand re-uses the (now free) MLP hidden buffer
   __nv_bfloat16* hdec = train ? ts.hdec : ws.u;
-  DGS_TRY(ln_modulate(x_fin, w->dec_ln_w, md, md + D, mod_stride, hdec, B, N, G, T, D, 1e-5f, 1, st));
+  DGS_TRY(ln_forward(LN_SPLIT_BF16, x_fin, w->dec_ln_w, md, md + D, mod_stride, hdec, nullptr, B, N, G, T, D, 1e-5f, st));
   {
     GemmEpilogue ep;
     ep.out = ws.img_gs; ep.ldc = d.Ndec;
@@ -383,11 +383,11 @@ int heads_backward(const dgs_dit_weights* w, const dgs_dit_weights_t* wT, const 
   // image_token_decoder: dh = d_img W, dW = d_img^T h
   DGS_TRY(dgrad(d_img, wT->dec_wT, ts.dh, d.Mt, D, d.Ndec, EPI_BIAS_BF16, nullptr, st));
   DGS_TRY(wgrad_tn(d_img, d.Ndec, ts.hdec, 3 * D, g->dec_w, d.Ndec, D, d.Mt, st));  // hi part of the [hi|lo|hi] operand
-  DGS_TRY(ln_modulate_bwd(x_fin, ts.dh, 0, w->dec_ln_w, md + D, d.mod_stride, B, N, G, T, D, 1e-5f, ts.dx, 0, dmd,
+  DGS_TRY(ln_modulate_bwd(x_fin, ts.dh, w->dec_ln_w, md + D, d.mod_stride, B, N, G, T, D, 1e-5f, ts.dx, 0, dmd,
                           dmd + D, g->dec_ln_w, ts.ln_stats, st));
   if (G > 0) {  // upsampler (the free Gaussian tokens, rows 0..G of every sample)
     DGS_TRY(tiny_linear_bwd(ts.d_gs_tok, wT->ups_w, ws.hg, ts.dyb, g->ups_w, B * G, 14, D, st));
-    DGS_TRY(ln_modulate_bwd(x_fin, ts.dyb, 0, w->ups_ln_w, mu + D, d.mod_stride, B, N, 0, G, D, 1e-5f, ts.dx, 0, dmu,
+    DGS_TRY(ln_modulate_bwd(x_fin, ts.dyb, w->ups_ln_w, mu + D, d.mod_stride, B, N, 0, G, D, 1e-5f, ts.dx, 0, dmu,
                             dmu + D, g->ups_ln_w, ts.ln_stats, st));
   }
   return DGS_OK;
@@ -433,7 +433,7 @@ int block_backward(const dgs_dit_weights* w, const dgs_dit_weights_t* wT, const 
   DGS_TRY(trace_out(tr.dh2, l, ts.dh, MD * b2, st));
   {
     ProfScope ps(st, PROF_DIT_BWD_ELEM);
-    DGS_TRY(ln_modulate_bwd(b.x_mid, ts.dh, 0, nullptr, m + 4 * D, ms, B, N, 0, N, D, 1e-6f, ts.dx, 1, dm + 3 * D,
+    DGS_TRY(ln_modulate_bwd(b.x_mid, ts.dh, nullptr, m + 4 * D, ms, B, N, 0, N, D, 1e-6f, ts.dx, 1, dm + 3 * D,
                             dm + 4 * D, nullptr, ts.ln_stats, st));
     DGS_TRY(trace_out(tr.dx_mid, l, ts.dx, MD * f4, st));
     // -- attention branch: x_mid = x_in + gate_msa * proj(attn(qkv(h1)))
@@ -472,7 +472,7 @@ int block_backward(const dgs_dit_weights* w, const dgs_dit_weights_t* wT, const 
   DGS_TRY(trace_out(tr.dh1, l, ts.dh, MD * b2, st));
   {
     ProfScope ps(st, PROF_DIT_BWD_ELEM);
-    DGS_TRY(ln_modulate_bwd(b.x_in, ts.dh, 0, nullptr, m + D, ms, B, N, 0, N, D, 1e-6f, ts.dx, 1, dm, dm + D, nullptr,
+    DGS_TRY(ln_modulate_bwd(b.x_in, ts.dh, nullptr, m + D, ms, B, N, 0, N, D, 1e-6f, ts.dx, 1, dm, dm + D, nullptr,
                             ts.ln_stats, st));
     DGS_TRY(trace_out(tr.dx, l, ts.dx, MD * f4, st));
     // this block's adaLN linear (6w x w, a third of the block's parameters): d mod_l is complete now, so its weight /
@@ -489,11 +489,11 @@ int block_backward(const dgs_dit_weights* w, const dgs_dit_weights_t* wT, const 
 int input_cond_backward(const dgs_dit_weights* w, const dgs_dit_grads* g, const DitDims& d, const DitWorkspace& ws,
                         const TrainState& ts, cudaStream_t st) {
   const int B = d.B, N = d.N, T = d.T, G = d.G, D = d.D, L = w->layers;
-  DGS_TRY(ln_modulate_bwd(ts.x_pre, ts.dx, 1, w->in_ln_w, nullptr, 0, B, N, 0, N, D, 1e-5f, ts.dx_pre, 0, nullptr, nullptr,
+  DGS_TRY(ln_modulate_bwd(ts.x_pre, ts.dx, w->in_ln_w, nullptr, 0, B, N, 0, N, D, 1e-5f, ts.dx_pre, 0, nullptr, nullptr,
                           g->in_ln_w, ts.ln_stats, st));
   DGS_TRY(pos_embed_bwd(ts.dx_pre, g->pos_embed, B, G, N, D, st));
-  DGS_TRY(transpose_to_bf16(ts.dx_pre, 1, D, B, N, G, T, D, ts.bigT0, nullptr, st));                  // d tok^T [D, Mtp]
-  DGS_TRY(transpose_to_bf16(ws.tokens, 0, 3 * d.Kin, 1, d.Mt, 0, d.Mt, d.Kin, ts.bigT1, nullptr, st));  // hi part of the patches
+  DGS_TRY(transpose_to_bf16(ts.dx_pre, D, B, N, G, T, D, ts.bigT0, nullptr, st));                  // d tok^T [D, Mtp]
+  DGS_TRY(transpose_to_bf16(ws.tokens, 3 * d.Kin, 1, d.Mt, 0, d.Mt, d.Kin, ts.bigT1, nullptr, st));  // hi part of the patches
   {
     GemmEpilogue ep;  // dW[D, Kin] = d tok^T [D, Mtp] x (patches^T [Kin, Mtp])^T   (K = padded row count, pads are zero)
     ep.out = g->tokenizer_w; ep.ldc = d.Kin;
@@ -563,7 +563,8 @@ int dgs_quantize_rows_e4m3(const float* x, int rows, int cols, void* q, float* s
 int dgs_ln_modulate_fp8(const float* x, const float* shift, const float* scale, int mod_stride, void* q, float* q_scale,
                         int B, int rows, int width, float eps, void* stream) {
   DGS_REQUIRE(x && shift && scale && q && q_scale, "NULL pointer");
-  return ln_modulate_fp8(x, shift, scale, mod_stride, (uint8_t*)q, q_scale, B, rows, width, eps, (cudaStream_t)stream);
+  return ln_forward(LN_E4M3, x, nullptr, shift, scale, mod_stride, q, q_scale, B, rows, 0, rows, width, eps,
+                    (cudaStream_t)stream);
 }
 
 int dgs_gemm_fp8(const void* A, const float* sa, const void* W, const float* sw, const float* bias, const float* gate,
@@ -731,7 +732,10 @@ int dgs_stream_wait_event(void* stream, void* ev) {
 
 int dgs_transpose_bf16(const void* in, int in_is_f32, int M, int C, void* out, float* colsum, void* stream) {
   DGS_REQUIRE(in && out && M > 0, "NULL pointer / bad shape");
-  return transpose_to_bf16(in, in_is_f32, C, 1, M, 0, M, C, (__nv_bfloat16*)out, colsum, (cudaStream_t)stream);
+  __nv_bfloat16* o = (__nv_bfloat16*)out;
+  cudaStream_t st = (cudaStream_t)stream;
+  return in_is_f32 ? transpose_to_bf16((const float*)in, C, 1, M, 0, M, C, o, colsum, st)
+                   : transpose_to_bf16((const __nv_bfloat16*)in, C, 1, M, 0, M, C, o, colsum, st);
 }
 
 int dgs_adamw_step(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, size_t n, float lr, float beta1,
@@ -790,8 +794,11 @@ int dgs_ln_modulate_bwd(const float* x, const void* dh, int dh_is_f32, const flo
                         int mod_stride, int B, int rows, int width, float eps, float* dx, int accumulate, float* dshift,
                         float* dscale, float* dln_w, float* stats, void* stream) {
   DGS_REQUIRE(x && dh && dx && stats, "NULL pointer");
-  return ln_modulate_bwd(x, dh, dh_is_f32, ln_w, scale, mod_stride, B, rows, 0, rows, width, eps, dx, accumulate, dshift,
-                         dscale, dln_w, stats, (cudaStream_t)stream);
+  cudaStream_t st = (cudaStream_t)stream;
+  return dh_is_f32 ? ln_modulate_bwd(x, (const float*)dh, ln_w, scale, mod_stride, B, rows, 0, rows, width, eps, dx,
+                                     accumulate, dshift, dscale, dln_w, stats, st)
+                   : ln_modulate_bwd(x, (const __nv_bfloat16*)dh, ln_w, scale, mod_stride, B, rows, 0, rows, width, eps,
+                                     dx, accumulate, dshift, dscale, dln_w, stats, st);
 }
 
 int dgs_gate_bwd(const float* dx, const void* y, const float* gate, int gate_stride, int rows_per_sample, int M, int C,
@@ -815,8 +822,8 @@ int dgs_attention_fwd(const void* qkv, void* out, int B, int N, int heads, void*
 int dgs_ln_modulate(const float* x, const float* ln_w, const float* shift, const float* scale, int mod_stride, void* h,
                     int B, int rows, int width, float eps, void* stream) {
   DGS_REQUIRE(x && shift && scale && h, "NULL pointer");
-  return ln_modulate(x, ln_w, shift, scale, mod_stride, (__nv_bfloat16*)h, B, rows, 0, rows, width, eps, 0,
-                     (cudaStream_t)stream);
+  return ln_forward(LN_BF16, x, ln_w, shift, scale, mod_stride, h, nullptr, B, rows, 0, rows, width, eps,
+                    (cudaStream_t)stream);
 }
 
 }  // extern "C"

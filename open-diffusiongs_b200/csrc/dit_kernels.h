@@ -49,21 +49,21 @@ inline int attention_lse_stride(int N) { return (N + 127) / 128 * 128; }
 int attention_bwd(const void* qkv, const void* out, const void* dout, float* lse2, float* dsum, void* dqkv, int B, int N,
                   int H, cudaStream_t st);
 
-// ---- dit_misc.cu -------------------------------------------------------------------------------
-// h[r,:] = (LN(x[r,:]; eps) [* w]) * (1 + scale[b,:]) + shift[b,:]   -> bf16
-// rows are gathered: output row r (0..B*rows_out) reads x row  b*rows_in + row_off + (r % rows_out)
-// split != 0: the output row is [hi | lo | hi] (3*D bf16) with value = hi + lo (split-bf16 operand)
-int ln_modulate(const float* x, const float* ln_weight, const float* shift, const float* scale, int mod_stride,
-                __nv_bfloat16* h, int B, int rows_in, int row_off, int rows_out, int D, float eps, int split,
-                cudaStream_t st);
-// the same LayerNorm + modulate (no LN weight, no gather) -> e4m3 q [B*rows, D] with one power-of-two scale per row
-// and 128-column group, q_scale [D/128][fp8_scale_stride(B*rows)]
-int ln_modulate_fp8(const float* x, const float* shift, const float* scale, int mod_stride, uint8_t* q, float* q_scale,
-                    int B, int rows, int D, float eps, cudaStream_t st);
+// ---- dit_glue.cu: forward ----------------------------------------------------------------------
+// LayerNorm [* w] + adaLN modulate: output row r (0..B*rows_out) normalises x row  b*rows_in + row_off + (r % rows_out),
+// b = r / rows_out, to y = LN(x; eps) [* w] and stores  y * (1 + scale[b,:]) + shift[b,:]  as
+enum LnOut {
+  LN_BF16,        // bf16 [B*rows_out, D]
+  LN_SPLIT_BF16,  // bf16 [B*rows_out, 3*D] = [hi | lo | hi] with value = hi + lo (split-bf16 operand)
+  LN_E4M3,        // e4m3 [B*rows_out, D] with one power-of-two scale per row and 128-column group,
+                  // out_scale [D/128][fp8_scale_stride(B*rows_out)]; no LN weight (ln_weight ignored)
+  LN_F32,         // fp32, out = y (no modulate: shift / scale unused); in place (out == x); needs ln_weight
+};
+int ln_forward(LnOut kind, const float* x, const float* ln_weight, const float* shift, const float* scale,
+               int mod_stride, void* out, float* out_scale, int B, int rows_in, int row_off, int rows_out, int D,
+               float eps, cudaStream_t st);
 // q [rows, cols] e4m3 = x / scale[r] with one power-of-two scale per row (the FP8 weight format)
 int quantize_rows_e4m3(const float* x, int rows, int cols, uint8_t* q, float* scale, cudaStream_t st);
-// plain LayerNorm with weight (no bias), fp32 -> fp32, in place over [rows, D]
-int ln_weight_inplace(float* x, const float* w, int rows, int D, float eps, cudaStream_t st);
 // out[b, n] = act_in(in[b,:]) . W[n,:] + bias[n], W fp32 [N,K]; act_in: 0 none, 1 SiLU
 int skinny_linear(const float* in, const float* W, const float* bias, float* out, int B, int N, int K,
                   int act_in, int act_out_silu, cudaStream_t st);
@@ -83,17 +83,20 @@ struct GsOut { float* xyz; float* features; float* scaling; float* rotation; flo
 int gaussians_epilogue(const float* gs_tokens /*[B,G,14]*/, const float* img_gs /*[B*V*hh*ww, p*p*14]*/,
                        const float* ray_o, const float* ray_d, GsOut out, int B, int G, int V, int H, int W, int patch,
                        int scene_mode, float near_, float far_, cudaStream_t st);
-int f32_to_bf16(const float* in, __nv_bfloat16* out, size_t n, cudaStream_t st);
 
-// ---- dit_bwd_misc.cu (backward glue) -------------------------------------------------------------
+// ---- dit_glue.cu: backward ---------------------------------------------------------------------
 // out[c, m] = bf16(in[row(m), c]); m = b*rows_out + j -> input row b*rows_in + row_off + j; out [C, round_up(M,64)]
-int transpose_to_bf16(const void* in, int in_is_f32, int ldi, int B, int rows_in, int row_off, int rows_out, int C,
-                      __nv_bfloat16* out, float* colsum, cudaStream_t st);
+// TI: float or __nv_bfloat16
+template <typename TI>
+int transpose_to_bf16(const TI* in, int ldi, int B, int rows_in, int row_off, int rows_out, int C, __nv_bfloat16* out,
+                      float* colsum, cudaStream_t st);
 int gate_bwd(const float* dx, const __nv_bfloat16* y, const float* gate, int gate_stride, int rows_per_sample, int M,
              int C, __nv_bfloat16* dy, __nv_bfloat16* dyT, float* dgate, float* dbias, cudaStream_t st);
-int ln_modulate_bwd(const float* x, const void* dh, int dh_is_f32, const float* lnw, const float* scale, int mod_stride,
-                    int B, int rows_in, int row_off, int rows_out, int D, float eps, float* dx, int accumulate,
-                    float* dshift, float* dscale, float* dlnw, float* stats /* scratch [B*rows_out*2] */, cudaStream_t st);
+// backward of ln_forward (TG, the type of dh: float or __nv_bfloat16)
+template <typename TG>
+int ln_modulate_bwd(const float* x, const TG* dh, const float* lnw, const float* scale, int mod_stride, int B,
+                    int rows_in, int row_off, int rows_out, int D, float eps, float* dx, int accumulate, float* dshift,
+                    float* dscale, float* dlnw, float* stats /* scratch [B*rows_out*2] */, cudaStream_t st);
 // Where the weight/bias gradient rows of a (stacked) skinny linear go: n_seg regular segments of seg_rows rows each
 // (segment i at dW0 + i*seg_stride floats, its bias gradient at db0 + i*seg_stride), then two tail segments.
 struct SkinnySegs {

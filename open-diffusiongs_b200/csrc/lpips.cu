@@ -36,12 +36,6 @@ constexpr ConvSpec kConv[NCONV] = {
     {512, 512, 4, -1, true},  {512, 512, 4, -1, false}, {512, 512, 4, 4, false}};
 constexpr int kTapConv[NTAP] = {1, 3, 6, 9, 12};
 
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 __device__ __forceinline__ void unpack8(const uint4& u, float (&f)[8]) {
   const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
 #pragma unroll

@@ -21,6 +21,7 @@
 #include <type_traits>
 
 #include "dgs_internal.h"
+#include "sm90_ptx.cuh"
 
 namespace dgs {
 
@@ -1007,11 +1008,7 @@ __global__ void __launch_bounds__(TILE_PIX) blend_forward_kernel(Problem pb, Geo
 // shuffles, then across the CTA's 8 warps in shared memory, and only ONE atomic per gradient component
 // per (tile, Gaussian) instance reaches L2 (the reference issues 9 atomics per contributing pair).
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
+using ptx::warp_sum;
 
 constexpr int BWD_CHUNK = 64;  // Gaussians staged per round in the backward
 

@@ -133,6 +133,12 @@ __device__ __forceinline__ uint32_t pack2_bf16(float a, float b) {
   __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&v);
 }
+// sum over the 32 lanes of a warp (butterfly: every lane gets the total)
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
 
 // ---- e4m3 (FP8) quantization with power-of-two scales ----------------------------------------------
 // A group with absolute maximum amax gets the scale s = 2^e, e = ceil(log2(amax / 448)) (the smallest e with

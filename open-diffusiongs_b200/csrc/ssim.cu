@@ -20,6 +20,7 @@
 //   dx(p) = s [(W^T alpha)(p) + 2 x(p) (W^T beta)(p) + y(p) (W^T gamma)(p)],   s = dout / (3 (H-10)(W-10)).
 // No atomics: every result is independent of n and of whether a training state is written, bit for bit.
 #include "dgs_internal.h"
+#include "sm90_ptx.cuh"
 
 namespace dgs {
 namespace {
@@ -29,11 +30,7 @@ constexpr int TH = 32, TW = 32, LH = TH + HALO, LW = TW + HALO, NT = 256;
 
 struct Win { float g[WIN]; };
 
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
+using ptx::warp_sum;
 
 // partial[(img * tiles + tile) * 2 + {0, 1}] = sum of S over the tile's valid pixels and 3 channels, and (want_psnr)
 // the sum of (clamp(x) - clamp(y))^2 over the image pixels the tile owns.  maps (training): [n, 3 ch, 3, Hv, Wv].
