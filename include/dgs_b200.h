@@ -176,6 +176,31 @@ int dgs_render_batch_backward_mse(const dgs_render_batch_args* args, long long R
                                   float* d_xyz, float* d_features, float* d_scaling, float* d_rotation, float* d_opacity,
                                   dgs_alloc_fn scratch_alloc, void* scratch_user, void* stream);
 
+/* The same pair with per-pixel depth and alpha maps, from the blend the colour uses (same order, alpha >= 1/255 test, 0.99
+ * clamp and T < 1e-4 stop; w_i = alpha_i T_i the colour's weight):
+ *   depth[b,v,0,y,x] = sum_i w_i z_i   (z_i the Gaussian's view-space depth; background 0: the ACCUMULATED depth,
+ *                                       expected depth is depth / alpha)
+ *   alpha[b,v,0,y,x] = 1 - final T     (accumulated opacity)
+ * aux == NULL: exactly the _mse pair (mse may be NULL too; a fused MSE combines with aux).  The backward takes the upstream
+ * gradients of either map (either may be NULL); with neither it runs the plain kernels, otherwise its scratch records grow
+ * to 48 B per (view, Gaussian).  Images, final_T, n_contrib and loss_sum do not depend on aux. */
+typedef struct {
+  float* depth;             /* forward out [B,V,1,H,W], required when aux != NULL */
+  float* alpha;             /* forward out [B,V,1,H,W], required when aux != NULL */
+  const float* dL_ddepth;   /* backward in [B,V,1,H,W], or NULL */
+  const float* dL_dalpha;   /* backward in [B,V,1,H,W], or NULL */
+} dgs_render_aux;
+int dgs_render_batch_forward_aux(const dgs_render_batch_args* args, dgs_alloc_fn geom_alloc, void* geom_user,
+                                 dgs_alloc_fn binning_alloc, void* binning_user, dgs_alloc_fn image_alloc,
+                                 void* image_user, float* out_images, long long* num_rendered, long long* chunk_instances,
+                                 const dgs_render_mse* mse, const dgs_render_aux* aux, void* stream);
+int dgs_render_batch_backward_aux(const dgs_render_batch_args* args, long long R, const long long* chunk_instances,
+                                  const void* geom_buffer, const void* binning_buffer, const void* binning_buffer_b,
+                                  const void* image_buffer, const float* dL_dimages, const dgs_render_mse* mse,
+                                  const dgs_render_aux* aux, float* d_xyz, float* d_features, float* d_scaling,
+                                  float* d_rotation, float* d_opacity, dgs_alloc_fn scratch_alloc, void* scratch_user,
+                                  void* stream);
+
 /* Introspection used by the parity tests: copies of per-(view, Gaussian) / per-pixel forward state
  * out of the opaque arenas into caller DEVICE buffers (any may be NULL):
  * xy [N,2], depth [N], conic_opacity [N,4], rgb [N,3], tiles_touched [N] (N = n_views*P),

@@ -844,15 +844,29 @@ struct MseBwd {
   const float* coef = nullptr;    // [samples] device
 };
 
+// Depth and alpha maps (the blend kernels' AUX instantiations).  depth = sum_i w_i z_i with w_i = alpha_i T_i the colour's
+// blend weight and z_i the view-space depth in g0.z (background 0); alpha = 1 - final T.  Both are linear in the same
+// weights as the colour, so the backward adds one accumulator, folds dL/dalpha into the background term and reduces one
+// more per-Gaussian component, dL/dz, which the geometry backward pushes through W2C's third row.
+struct AuxFwd {
+  float* depth = nullptr;  // [NV,1,H,W]; two-phase: phase A leaves its partial sum here for phase B
+  float* alpha = nullptr;  // [NV,1,H,W]
+};
+struct AuxBwd {
+  const float* ddepth = nullptr;  // [NV,1,H,W] or null
+  const float* dalpha = nullptr;  // [NV,1,H,W] or null
+  float* dz = nullptr;            // [N] out: dL/dz per (view, Gaussian)
+};
 // ---------------------------------------------------------------------------------------------
 // K6: per-tile front-to-back alpha blend (forward.cu:261-374), one CTA per (view, tile)
 // ---------------------------------------------------------------------------------------------
 // MODE 0: the whole list in one pass.  MODE 1: phase A of two (the nearest Gaussians); saves the per-pixel blend state
 // and counts the tiles that still have unfinished pixels.  MODE 2: phase B, continues from that state.
-template <int MODE>
+// AUX: also the depth and alpha maps; z rides in the .w of s_rgb (the clamped bits the blend does not read).
+template <int MODE, bool AUX = false>
 __global__ void __launch_bounds__(TILE_PIX) blend_forward_kernel(Problem pb, GeomState gs, ImgState im,
                                                                  const uint32_t* __restrict__ point_list,
-                                                                 float* __restrict__ out_color, MseFwd mse) {
+                                                                 float* __restrict__ out_color, MseFwd mse, AuxFwd aux) {
   const int tile_g = blockIdx.x;
   const int view = tile_g / pb.tiles, tile = tile_g - view * pb.tiles;
   const int tx = tile % pb.gx, ty = tile / pb.gx;
@@ -872,7 +886,7 @@ __global__ void __launch_bounds__(TILE_PIX) blend_forward_kernel(Problem pb, Geo
   const float tx0 = (float)(tx * TILE);
 
   bool done = !inside;
-  float T = 1.0f, C0 = 0.f, C1 = 0.f, C2 = 0.f;
+  float T = 1.0f, C0 = 0.f, C1 = 0.f, C2 = 0.f, D = 0.f;
   uint32_t contributor = 0, last = 0;
   if (MODE == 2 && inside) {
     const float4 a = im.acc[pix_g];
@@ -881,6 +895,7 @@ __global__ void __launch_bounds__(TILE_PIX) blend_forward_kernel(Problem pb, Geo
     contributor = cb & 0x7fffffffu;
     done = (cb >> 31) != 0;
     last = im.n_contrib[pix_g];
+    if constexpr (AUX) D = aux.depth[pix_g];
   }
   // visits before this kernel's list: 0, or (phase B) the phase-A list length, which every unfinished pixel has visited fully
   const uint32_t contrib0 = (MODE == 2) ? (im.ranges[tile_g].y - im.ranges[tile_g].x) : 0u;
@@ -896,7 +911,12 @@ __global__ void __launch_bounds__(TILE_PIX) blend_forward_kernel(Problem pb, Geo
       const float2 ext = alpha_extent(q);
       s_xy[threadIdx.x] = make_float4(a0.x, a0.y, ext.x, ext.y);
       s_co[threadIdx.x] = conic_log2(q);
-      s_rgb[threadIdx.x] = gs.g2[g];
+      if constexpr (AUX) {
+        const float4 c = gs.g2[g];
+        s_rgb[threadIdx.x] = make_float4(c.x, c.y, c.z, a0.z);
+      } else {
+        s_rgb[threadIdx.x] = gs.g2[g];
+      }
       small = ext.y < SKIP_WORTH;
     }
     const int use_skip = __syncthreads_or(small);  // dense chunks (every footprint covers the tile) keep the plain loop
@@ -948,6 +968,7 @@ __global__ void __launch_bounds__(TILE_PIX) blend_forward_kernel(Problem pb, Geo
       ok = ok && !sat;
       const float w = ok ? alpha * T : 0.f;
       C0 = fmaf(col.x, w, C0); C1 = fmaf(col.y, w, C1); C2 = fmaf(col.z, w, C2);
+      if constexpr (AUX) D = fmaf(col.w, w, D);
       T = ok ? test_T : T;
       last = ok ? visit : last;
     }
@@ -976,6 +997,10 @@ __global__ void __launch_bounds__(TILE_PIX) blend_forward_kernel(Problem pb, Geo
     oc[pid] = C0 + T * pb.bg[0];
     oc[plane + pid] = C1 + T * pb.bg[1];
     oc[2 * plane + pid] = C2 + T * pb.bg[2];
+    if constexpr (AUX) {
+      aux.depth[ibase + pid] = D;
+      aux.alpha[ibase + pid] = 1.0f - T;
+    }
   }
   if (mse.target) {
     // every pixel's FINAL colour is counted exactly once: phase A counts the tiles it finished, phase B the open ones
@@ -1012,6 +1037,8 @@ using ptx::warp_sum;
 
 constexpr int BWD_CHUNK = 64;  // Gaussians staged per round in the backward
 
+// AUX: the depth / alpha gradients as well (see AuxFwd): a tenth reduced component, dL/dz, into aux.dz.
+template <bool AUX = false>
 __global__ void __launch_bounds__(TILE_PIX) blend_backward_kernel(Problem pb, GeomState gs, ImgState im,
                                                                   const uint32_t* __restrict__ point_list,
                                                                   const uint32_t* __restrict__ point_list_b,
@@ -1019,7 +1046,8 @@ __global__ void __launch_bounds__(TILE_PIX) blend_backward_kernel(Problem pb, Ge
                                                                   float* __restrict__ dmean2D /*[N,3]*/,
                                                                   float* __restrict__ dconic /*[N,4]*/,
                                                                   float* __restrict__ dopac /*[N]*/,
-                                                                  float* __restrict__ dcolor /*[N,3]*/) {
+                                                                  float* __restrict__ dcolor /*[N,3]*/, AuxBwd aux) {
+  constexpr int NC = AUX ? 10 : 9;  // reduced components per staged Gaussian
   const int tile_g = blockIdx.x;
   const int view = tile_g / pb.tiles, tile = tile_g - view * pb.tiles;
   const int tx = tile % pb.gx, ty = tile / pb.gx;
@@ -1040,7 +1068,7 @@ __global__ void __launch_bounds__(TILE_PIX) blend_backward_kernel(Problem pb, Ge
   __shared__ float4 s_xy[BWD_CHUNK];  // x, y, x half-extent, y half-extent (alpha_extent)
   __shared__ float4 s_co[BWD_CHUNK];
   __shared__ float4 s_rgb[BWD_CHUNK];
-  __shared__ float s_acc[BWD_CHUNK][9];  // CTA-level partial sums, 9 components per staged Gaussian
+  __shared__ float s_acc[BWD_CHUNK][NC];  // CTA-level partial sums per staged Gaussian
   __shared__ uint8_t s_list[TILE_PIX / 32][BWD_CHUNK];  // per-warp compacted slot indices
   __shared__ uint32_t s_max;
 
@@ -1059,6 +1087,11 @@ __global__ void __launch_bounds__(TILE_PIX) blend_backward_kernel(Problem pb, Ge
       dp0 = fmaf(k, c[0] - t[0], dp0); dp1 = fmaf(k, c[plane] - t[plane], dp1); dp2 = fmaf(k, c[2 * plane] - t[2 * plane], dp2);
     }
   }
+  float dD = 0.f, dA = 0.f;
+  if constexpr (AUX) {
+    if (inside && aux.ddepth) dD = aux.ddepth[ibase + pid];
+    if (inside && aux.dalpha) dA = aux.dalpha[ibase + pid];
+  }
   if (threadIdx.x == 0) s_max = 0;
   __syncthreads();
   {
@@ -1075,7 +1108,10 @@ __global__ void __launch_bounds__(TILE_PIX) blend_backward_kernel(Problem pb, Ge
 
   float T = T_final;
   float acc0 = 0.f, acc1 = 0.f, acc2 = 0.f, lc0 = 0.f, lc1 = 0.f, lc2 = 0.f, last_alpha = 0.f;
-  const float bg_dot = pb.bg[0] * dp0 + pb.bg[1] * dp1 + pb.bg[2] * dp2;
+  float accD = 0.f, lz = 0.f;
+  float bg_dot = pb.bg[0] * dp0 + pb.bg[1] * dp1 + pb.bg[2] * dp2;
+  // alpha = 1 - T_final has d/dalpha_i = T_final / (1 - alpha_i): the background term's factor with the opposite sign
+  if constexpr (AUX) bg_dot -= dA;
   const float ddelx_dx = 0.5f * pb.W, ddely_dy = 0.5f * pb.H;
 
   // walk positions deepest-1 ... 0 in chunks; within a chunk slot j holds position (top - j)
@@ -1093,9 +1129,14 @@ __global__ void __launch_bounds__(TILE_PIX) blend_backward_kernel(Problem pb, Ge
       const float2 ext = alpha_extent(q);
       s_xy[threadIdx.x] = make_float4(a0.x, a0.y, ext.x, ext.y);
       s_co[threadIdx.x] = q;
-      s_rgb[threadIdx.x] = gs.g2[g];
+      if constexpr (AUX) {
+        const float4 c = gs.g2[g];
+        s_rgb[threadIdx.x] = make_float4(c.x, c.y, c.z, a0.z);
+      } else {
+        s_rgb[threadIdx.x] = gs.g2[g];
+      }
     }
-    for (int t = threadIdx.x; t < nb * 9; t += TILE_PIX) (&s_acc[0][0])[t] = 0.f;
+    for (int t = threadIdx.x; t < nb * NC; t += TILE_PIX) (&s_acc[0][0])[t] = 0.f;
     __syncthreads();
     // per-warp compaction of the staged slots whose footprint can reach this warp's pixels (see alpha_extent and the
     // forward kernel); 2 tests per lane, order preserved
@@ -1120,6 +1161,7 @@ __global__ void __launch_bounds__(TILE_PIX) blend_backward_kernel(Problem pb, Ge
       const int j = (int)s_list[warp][k];
       const uint32_t pos = (uint32_t)(top - j);  // 0-based position in the tile list
       float g_c0 = 0.f, g_c1 = 0.f, g_c2 = 0.f, g_mx = 0.f, g_my = 0.f, g_ca = 0.f, g_cb = 0.f, g_cc = 0.f, g_op = 0.f;
+      float g_z = 0.f;
       bool active = false;
       const float4 xy = s_xy[j];
       if (pos < last) {
@@ -1138,6 +1180,11 @@ __global__ void __launch_bounds__(TILE_PIX) blend_backward_kernel(Problem pb, Ge
             acc1 = last_alpha * lc1 + (1.f - last_alpha) * acc1; lc1 = col.y;
             acc2 = last_alpha * lc2 + (1.f - last_alpha) * acc2; lc2 = col.z;
             float dL_dalpha = (col.x - acc0) * dp0 + (col.y - acc1) * dp1 + (col.z - acc2) * dp2;
+            if constexpr (AUX) {
+              accD = last_alpha * lz + (1.f - last_alpha) * accD; lz = col.w;
+              dL_dalpha += (col.w - accD) * dD;
+              g_z = dch * dD;
+            }
             g_c0 = dch * dp0; g_c1 = dch * dp1; g_c2 = dch * dp2;
             dL_dalpha *= T;
             last_alpha = alpha;
@@ -1186,12 +1233,16 @@ __global__ void __launch_bounds__(TILE_PIX) blend_backward_kernel(Problem pb, Ge
         // {mean.x, mean.y, conic.a, conic.b, conic.c, opacity, colour.r, colour.g}
         if ((lane & 3) == 0) atomicAdd(&s_acc[j][((lane >> 4) & 1) * 4 + ((lane >> 3) & 1) * 2 + ((lane >> 2) & 1)], a0);
         if (lane == 1) atomicAdd(&s_acc[j][8], g_c2);
+        if constexpr (AUX) {
+          g_z = warp_sum(g_z);
+          if (lane == 2) atomicAdd(&s_acc[j][9], g_z);
+        }
       }
     }
     __syncthreads();
     // flush: one global atomic per component per staged Gaussian
-    for (int t = threadIdx.x; t < nb * 9; t += TILE_PIX) {
-      const int j = t / 9, c = t - 9 * j;
+    for (int t = threadIdx.x; t < nb * NC; t += TILE_PIX) {
+      const int j = t / NC, c = t - NC * j;
       const float v = s_acc[j][c];
       if (v != 0.f) {
         const size_t g = gbase + s_id[j];
@@ -1204,6 +1255,9 @@ __global__ void __launch_bounds__(TILE_PIX) blend_backward_kernel(Problem pb, Ge
           case 4: dst = dconic + 4 * g + 3; break;
           case 5: dst = dopac + g; break;
           default: dst = dcolor + 3 * g + (c - 6); break;
+        }
+        if constexpr (AUX) {
+          if (c == 9) dst = aux.dz + g;
         }
         atomicAdd(dst, v);
       }
@@ -1225,11 +1279,14 @@ struct GeomGradOut {
   float* dopac_raw;  // [S*P] raw-opacity gradient (batched mode) or null
 };
 
+// AUX: plus dL/dz (blend_backward_kernel<true>'s tenth component) through z = W2C[2] . (mean, 1)
+template <bool AUX = false>
 __global__ void __launch_bounds__(256) geometry_backward_kernel(Problem pb, GeomState gs, const int* __restrict__ radii_in,
                                                                 const float* __restrict__ dmean2D,
                                                                 const float* __restrict__ dconic,
                                                                 const float* __restrict__ dopac,
-                                                                const float* __restrict__ dcolor, GeomGradOut out) {
+                                                                const float* __restrict__ dcolor, GeomGradOut out,
+                                                                const float* __restrict__ dz) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const int s = blockIdx.y;
   if (i >= pb.P) return;
@@ -1360,6 +1417,10 @@ __global__ void __launch_bounds__(256) geometry_backward_kernel(Problem pb, Geom
     dmv[0] += (pm[0] * mw - pm[3] * mul1) * gx2 + (pm[1] * mw - pm[3] * mul2) * gy2;
     dmv[1] += (pm[4] * mw - pm[7] * mul1) * gx2 + (pm[5] * mw - pm[7] * mul2) * gy2;
     dmv[2] += (pm[8] * mw - pm[11] * mul1) * gx2 + (pm[9] * mw - pm[11] * mul2) * gy2;
+    if constexpr (AUX) {
+      const float gz = dz[n];
+      dmv[0] += vm[2] * gz; dmv[1] += vm[6] * gz; dmv[2] += vm[10] * gz;
+    }
     // ---- colour -> SH (backward.cu:20-139) ----
     if (pb.shs) {
       const int clamped = __float_as_int(gs.g2[n].w);
@@ -1505,6 +1566,7 @@ struct Forward {  // one forward's problem, arenas and launch context, shared by
   Allocators al;
   float* out_color;
   MseFwd mse;
+  AuxFwd aux;
   cudaStream_t st;
   int debug;
   size_t N, ntiles;  // view-Gaussians, view-tiles
@@ -1523,7 +1585,12 @@ static int alloc_binning(const Forward& f, long long R, BinState* bs) {
 template <int MODE>
 static int blend_forward(const Forward& f, const uint32_t* point_list) {
   ProfScope ps(f.st, PROF_RASTER_BLEND_FWD);
-  blend_forward_kernel<MODE><<<(unsigned)f.ntiles, TILE_PIX, 0, f.st>>>(f.pb, f.gs, f.im, point_list, f.out_color, f.mse);
+  if (!f.aux.depth)
+    blend_forward_kernel<MODE><<<(unsigned)f.ntiles, TILE_PIX, 0, f.st>>>(f.pb, f.gs, f.im, point_list, f.out_color, f.mse,
+                                                                          f.aux);
+  else
+    blend_forward_kernel<MODE, true><<<(unsigned)f.ntiles, TILE_PIX, 0, f.st>>>(f.pb, f.gs, f.im, point_list, f.out_color,
+                                                                                f.mse, f.aux);
   DGS_LAUNCH_OK(f.st, f.debug);
   return DGS_OK;
 }
@@ -1719,9 +1786,10 @@ static int bin_two_phase(const Forward& f, const Split& sp, long long* R_far) {
 
 // projection -> small-scene binning, or depth ranking and scan -> split decision -> bin pass(es) + blend
 static int run_forward(Problem pb, const CameraInput& cam, const Allocators& al, float* out_color, int* radii,
-                       long long* R_out, long long chunk_R[2], cudaStream_t st, int debug, MseFwd mse = MseFwd()) {
+                       long long* R_out, long long chunk_R[2], cudaStream_t st, int debug, MseFwd mse = MseFwd(),
+                       AuxFwd aux = AuxFwd()) {
   Forward f;
-  f.pb = pb; f.al = al; f.out_color = out_color; f.mse = mse; f.st = st; f.debug = debug;
+  f.pb = pb; f.al = al; f.out_color = out_color; f.mse = mse; f.aux = aux; f.st = st; f.debug = debug;
   f.N = (size_t)pb.NV * pb.P;
   f.ntiles = (size_t)pb.NV * pb.tiles;
   DGS_REQUIRE(f.N < (size_t)INT32_MAX, "n_views * P = %zu does not fit the 32-bit scan", f.N);
@@ -1856,15 +1924,15 @@ int dgs_raster_backward(const dgs_raster_args* a, int R, const int* radii, const
   ImgState im = ImgState::carve(const_cast<void*>(image_buffer), 1, a->W, a->H, nullptr);
   BinState bs = BinState::carve(const_cast<void*>(binning_buffer), R, nullptr);
   if (R > 0) {
-    blend_backward_kernel<<<pb.tiles, TILE_PIX, 0, st>>>(pb, gs, im, bs.point_list, nullptr, dL_dpix, MseBwd(), dL_dmean2D,
-                                                          dL_dconic, dL_dopacity, dL_dcolor);
+    blend_backward_kernel<false><<<pb.tiles, TILE_PIX, 0, st>>>(pb, gs, im, bs.point_list, nullptr, dL_dpix, MseBwd(),
+                                                                 dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolor, AuxBwd());
     DGS_LAUNCH_OK(st, a->debug);
   }
   GeomGradOut out;
   out.dmeans = dL_dmean3D; out.dcov3d = dL_dcov3D; out.dsh = dL_dsh; out.dscale = dL_dscale; out.drot = dL_drot;
   out.dopac_raw = nullptr;
-  geometry_backward_kernel<<<dim3(ceil_div(a->P, 256), 1), 256, 0, st>>>(pb, gs, radii, dL_dmean2D, dL_dconic,
-                                                                          dL_dopacity, dL_dcolor, out);
+  geometry_backward_kernel<false><<<dim3(ceil_div(a->P, 256), 1), 256, 0, st>>>(pb, gs, radii, dL_dmean2D, dL_dconic,
+                                                                                 dL_dopacity, dL_dcolor, out, nullptr);
   DGS_LAUNCH_OK(st, a->debug);
   return DGS_OK;
 }
@@ -1908,6 +1976,14 @@ int dgs_render_batch_forward_mse(const dgs_render_batch_args* a, dgs_alloc_fn ge
                                  dgs_alloc_fn bin_alloc, void* bin_user, dgs_alloc_fn img_alloc, void* img_user,
                                  float* out_images, long long* num_rendered, long long* chunk_instances,
                                  const dgs_render_mse* mse, void* stream) {
+  return dgs_render_batch_forward_aux(a, geom_alloc, geom_user, bin_alloc, bin_user, img_alloc, img_user, out_images,
+                                      num_rendered, chunk_instances, mse, nullptr, stream);
+}
+
+int dgs_render_batch_forward_aux(const dgs_render_batch_args* a, dgs_alloc_fn geom_alloc, void* geom_user,
+                                 dgs_alloc_fn bin_alloc, void* bin_user, dgs_alloc_fn img_alloc, void* img_user,
+                                 float* out_images, long long* num_rendered, long long* chunk_instances,
+                                 const dgs_render_mse* mse, const dgs_render_aux* aux, void* stream) {
   int rc = check_batch_args(a);
   if (rc) return rc;
   DGS_REQUIRE(geom_alloc && bin_alloc && img_alloc && out_images && num_rendered && chunk_instances,
@@ -1918,12 +1994,17 @@ int dgs_render_batch_forward_mse(const dgs_render_batch_args* a, dgs_alloc_fn ge
                 "mse: target / loss_sum NULL or target_channels not 3|4");
     mf.target = mse->target; mf.tc = mse->target_channels; mf.loss = mse->loss_sum;
   }
+  AuxFwd af;
+  if (aux) {
+    DGS_REQUIRE(aux->depth && aux->alpha, "aux: depth / alpha output NULL");
+    af.depth = aux->depth; af.alpha = aux->alpha;
+  }
   Problem pb = batch_problem(a);
   CameraInput cam;
   cam.c2w = a->c2w; cam.fxfycxcy = a->fxfycxcy;
   const Allocators al = {geom_alloc, geom_user, bin_alloc, bin_user, img_alloc, img_user};
   return run_forward(pb, cam, al, out_images, nullptr, num_rendered, chunk_instances, (cudaStream_t)stream, a->debug,
-                     mf);
+                     mf, af);
 }
 
 int dgs_render_batch_backward(const dgs_render_batch_args* a, long long R, const long long* chunk_instances,
@@ -1942,9 +2023,22 @@ int dgs_render_batch_backward_mse(const dgs_render_batch_args* a, long long R, c
                                   const void* image_buffer, const float* dL_dimages, const dgs_render_mse* mse,
                                   float* d_xyz, float* d_features, float* d_scaling, float* d_rotation,
                                   float* d_opacity, dgs_alloc_fn scratch_alloc, void* scratch_user, void* stream) {
+  return dgs_render_batch_backward_aux(a, R, chunk_instances, geom_buffer, binning_buffer, binning_buffer_b, image_buffer,
+                                       dL_dimages, mse, nullptr, d_xyz, d_features, d_scaling, d_rotation, d_opacity,
+                                       scratch_alloc, scratch_user, stream);
+}
+
+int dgs_render_batch_backward_aux(const dgs_render_batch_args* a, long long R, const long long* chunk_instances,
+                                  const void* geom_buffer, const void* binning_buffer, const void* binning_buffer_b,
+                                  const void* image_buffer, const float* dL_dimages, const dgs_render_mse* mse,
+                                  const dgs_render_aux* aux, float* d_xyz, float* d_features, float* d_scaling,
+                                  float* d_rotation, float* d_opacity, dgs_alloc_fn scratch_alloc, void* scratch_user,
+                                  void* stream) {
   int rc = check_batch_args(a);
   if (rc) return rc;
-  DGS_REQUIRE(geom_buffer && binning_buffer && image_buffer && (dL_dimages || mse) && scratch_alloc && chunk_instances,
+  const bool has_aux = aux && (aux->dL_ddepth || aux->dL_dalpha);  // no aux gradient: the plain kernels
+  DGS_REQUIRE(geom_buffer && binning_buffer && image_buffer && (dL_dimages || mse || has_aux) && scratch_alloc &&
+                  chunk_instances,
               "NULL state buffer");
   MseBwd mb;
   if (mse) {
@@ -1962,10 +2056,11 @@ int dgs_render_batch_backward_mse(const dgs_render_batch_args* a, long long R, c
   const uint32_t* list_b = nullptr;
   if (chunk_instances[1] > 0)
     list_b = BinState::carve(const_cast<void*>(binning_buffer_b), chunk_instances[1], nullptr).point_list;
-  // per-(view, Gaussian) screen-space gradient records: mean2D[3] conic[4] opacity[1] colour[3]
+  // per-(view, Gaussian) screen-space gradient records: mean2D[3] conic[4] opacity[1] colour[3], and with aux gradients z[1]
   const size_t N = (size_t)pb.NV * pb.P;
   Carver c(nullptr);
   c.take<float>(N * 3); c.take<float>(N * 4); c.take<float>(N); c.take<float>(N * 3);
+  if (has_aux) c.take<float>(N);
   const size_t sbytes = c.bytes();
   void* sbuf = scratch_alloc(sbytes, scratch_user);
   if (!sbuf) { set_error("scratch allocator returned NULL"); return DGS_ERR_ALLOC; }
@@ -1974,11 +2069,21 @@ int dgs_render_batch_backward_mse(const dgs_render_batch_args* a, long long R, c
   float* dconic = cc.take<float>(N * 4);
   float* dopac = cc.take<float>(N);
   float* dcolor = cc.take<float>(N * 3);
+  AuxBwd ab;
+  if (has_aux) {
+    ab.ddepth = aux->dL_ddepth; ab.dalpha = aux->dL_dalpha;
+    ab.dz = cc.take<float>(N);
+  }
   DGS_CUDA_OK(cudaMemsetAsync(sbuf, 0, sbytes, st));
   if (R > 0) {
     ProfScope ps(st, PROF_RASTER_BLEND_BWD);
-    blend_backward_kernel<<<(unsigned)((size_t)pb.NV * pb.tiles), TILE_PIX, 0, st>>>(
-        pb, gs, im, bs.point_list, list_b, dL_dimages, mb, dmean2D, dconic, dopac, dcolor);
+    const unsigned grid = (unsigned)((size_t)pb.NV * pb.tiles);
+    if (has_aux)
+      blend_backward_kernel<true><<<grid, TILE_PIX, 0, st>>>(pb, gs, im, bs.point_list, list_b, dL_dimages, mb, dmean2D,
+                                                             dconic, dopac, dcolor, ab);
+    else
+      blend_backward_kernel<false><<<grid, TILE_PIX, 0, st>>>(pb, gs, im, bs.point_list, list_b, dL_dimages, mb, dmean2D,
+                                                              dconic, dopac, dcolor, ab);
     DGS_LAUNCH_OK(st, a->debug);
   }
   GeomGradOut out;
@@ -1986,8 +2091,11 @@ int dgs_render_batch_backward_mse(const dgs_render_batch_args* a, long long R, c
   out.dopac_raw = d_opacity;
   {
     ProfScope ps(st, PROF_RASTER_GEOM_BWD);
-    geometry_backward_kernel<<<dim3(ceil_div(a->P, 256), a->B), 256, 0, st>>>(pb, gs, nullptr, dmean2D, dconic, dopac,
-                                                                               dcolor, out);
+    const dim3 grid(ceil_div(a->P, 256), a->B);
+    if (has_aux)
+      geometry_backward_kernel<true><<<grid, 256, 0, st>>>(pb, gs, nullptr, dmean2D, dconic, dopac, dcolor, out, ab.dz);
+    else
+      geometry_backward_kernel<false><<<grid, 256, 0, st>>>(pb, gs, nullptr, dmean2D, dconic, dopac, dcolor, out, nullptr);
     DGS_LAUNCH_OK(st, a->debug);
   }
   return DGS_OK;

@@ -68,6 +68,10 @@ class RenderMse(C.Structure):  # dgs_render_mse
                 ("images", C.c_void_p)]
 
 
+class RenderAux(C.Structure):  # dgs_render_aux
+    _fields_ = [("depth", C.c_void_p), ("alpha", C.c_void_p), ("dL_ddepth", C.c_void_p), ("dL_dalpha", C.c_void_p)]
+
+
 class LpipsWeights(C.Structure):  # dgs_lpips_weights
     _fields_ = [("conv_w", C.c_void_p * 13), ("conv_wt", C.c_void_p * 13), ("conv_b", C.c_void_p * 13),
                 ("lin", C.c_void_p * 5), ("shift", C.c_void_p), ("scale", C.c_void_p)]
@@ -153,6 +157,11 @@ def lib():
                                                    C.POINTER(RenderMse), vp]
         L.dgs_render_batch_backward_mse.argtypes = [C.POINTER(RenderBatchArgs), C.c_longlong, C.POINTER(C.c_longlong)] + \
             [vp] * 5 + [C.POINTER(RenderMse)] + [vp] * 5 + [ALLOC_FN, vp, vp]
+        L.dgs_render_batch_forward_aux.argtypes = [C.POINTER(RenderBatchArgs), ALLOC_FN, vp, ALLOC_FN, vp, ALLOC_FN, vp, vp,
+                                                   C.POINTER(C.c_longlong), C.POINTER(C.c_longlong),
+                                                   C.POINTER(RenderMse), C.POINTER(RenderAux), vp]
+        L.dgs_render_batch_backward_aux.argtypes = [C.POINTER(RenderBatchArgs), C.c_longlong, C.POINTER(C.c_longlong)] + \
+            [vp] * 5 + [C.POINTER(RenderMse), C.POINTER(RenderAux)] + [vp] * 5 + [ALLOC_FN, vp, vp]
         L.dgs_transpose_bf16.argtypes = [vp, C.c_int, C.c_int, C.c_int, vp, vp, vp]
         L.dgs_adamw_step.argtypes = [vp, vp, vp, vp, C.c_size_t] + [C.c_float] * 5 + [C.c_int, C.c_float, vp, vp]
         L.dgs_cast_transpose_f32.argtypes = [vp, C.c_longlong, C.c_int, C.c_int, C.c_int, vp, vp, vp]
@@ -229,5 +238,5 @@ EXPORTED = [  # every symbol include/dgs_b200.h declares (checked by tests/test_
     "dgs_dit_export_ends", "dgs_lpips_workspace_bytes", "dgs_lpips_state_bytes", "dgs_lpips_forward", "dgs_lpips_backward",
     "dgs_ssim_workspace_bytes", "dgs_ssim_state_bytes", "dgs_ssim_forward", "dgs_ssim_backward",
     "dgs_dit_workspace_bytes_fp8", "dgs_dit_forward_fp8", "dgs_quantize_rows_e4m3", "dgs_ln_modulate_fp8", "dgs_gemm_fp8",
-    "dgs_mesh_field", "dgs_marching_cubes",
+    "dgs_mesh_field", "dgs_marching_cubes", "dgs_render_batch_forward_aux", "dgs_render_batch_backward_aux",
 ]

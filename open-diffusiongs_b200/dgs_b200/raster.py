@@ -9,7 +9,7 @@ import ctypes as C
 import torch
 
 from . import _lib
-from ._lib import ALLOC_FN, DgsError, RasterArgs, RenderBatchArgs, RenderMse, check
+from ._lib import ALLOC_FN, DgsError, RasterArgs, RenderAux, RenderBatchArgs, RenderMse, check
 
 
 LAST_NUM_RENDERED = None  # instance count R of the most recent batched forward (bench/roofline bookkeeping)
@@ -164,16 +164,20 @@ def _batch_args(xyz, features, scaling, rotation, opacity, C2W, fxfycxcy, H, W, 
 
 
 def render_batch_forward(xyz, features, scaling, rotation, opacity, H, W, C2W, fxfycxcy, scale_modifier=None,
-                         arena_cache=None, near_log2=None, mse_target=None, mse_loss_sum=None):
+                         arena_cache=None, near_log2=None, mse_target=None, mse_loss_sum=None, aux=False):
     """All (sample, view) pairs in one launch set -> (images [B,V,3,H,W] fp32, state).
     mse_target [B,V,3|4,H,W] + mse_loss_sum (fp64 [B], zeroed by the caller): the blend kernel also adds
-    sum (render - target)^2 of every sample into mse_loss_sum (dgs_render_batch_forward_mse).  When the batch holds more than
+    sum (render - target)^2 of every sample into mse_loss_sum (dgs_render_batch_forward_mse).
+    aux=True: also the depth and alpha maps of the same blend -> (images, depth [B,V,1,H,W], alpha [B,V,1,H,W], state),
+    depth = sum_i w_i z_i (accumulated view-space depth; expected depth = depth / alpha), alpha = 1 - final T
+    (dgs_render_batch_forward_aux).  When the batch holds more than
     2^31-1 instances (e.g. a random-init denoiser at 512x512: ~6e8 per view) the views are rendered in halves,
     recursively -- the reference renders one view per call anyway (gs_core.py:990-1001); `state` then carries one
     sub-state per chunk and render_batch_backward sums the chunks' gradients."""
+    maps = dict(aux=True) if aux else {}  # a plain render passes the plain render's arguments only
     try:
         return _render_batch_forward_one(xyz, features, scaling, rotation, opacity, H, W, C2W, fxfycxcy, scale_modifier,
-                                         arena_cache, near_log2, mse_target, mse_loss_sum)
+                                         arena_cache, near_log2, mse_target, mse_loss_sum, **maps)
     except DgsError as e:
         V = C2W.shape[1]
         if "exceeds 2^31-1" not in str(e) or V < 2:
@@ -184,18 +188,19 @@ def render_batch_forward(xyz, features, scaling, rotation, opacity, H, W, C2W, f
         sub_cache = None if arena_cache is None else arena_cache.setdefault(("views", ci), {})
         if mse_loss_sum is not None and ci == 0:
             mse_loss_sum.zero_()  # the failed whole-batch attempt may have counted some tiles already
-        o, st = render_batch_forward(xyz, features, scaling, rotation, opacity, H, W, C2W[:, v0:v1].contiguous(),
-                                     fxfycxcy[:, v0:v1].contiguous(), scale_modifier, sub_cache, near_log2,
-                                     None if mse_target is None else mse_target[:, v0:v1].contiguous(), mse_loss_sum)
+        *o, st = render_batch_forward(xyz, features, scaling, rotation, opacity, H, W, C2W[:, v0:v1].contiguous(),
+                                      fxfycxcy[:, v0:v1].contiguous(), scale_modifier, sub_cache, near_log2,
+                                      None if mse_target is None else mse_target[:, v0:v1].contiguous(), mse_loss_sum,
+                                      **maps)
         outs.append(o)
         subs.append((v0, v1, st))
         total += st["R"]
     LAST_NUM_RENDERED = total
-    return torch.cat(outs, dim=1), dict(sub=subs, R=total, tensors=subs[0][2]["tensors"])
+    return (*(torch.cat(maps, dim=1) for maps in zip(*outs)), dict(sub=subs, R=total, tensors=subs[0][2]["tensors"]))
 
 
 def _render_batch_forward_one(xyz, features, scaling, rotation, opacity, H, W, C2W, fxfycxcy, scale_modifier=None,
-                              arena_cache=None, near_log2=None, mse_target=None, mse_loss_sum=None):
+                              arena_cache=None, near_log2=None, mse_target=None, mse_loss_sum=None, aux=False):
     """One launch set over every (sample, view) pair.  `arena_cache` (a dict): re-use grow-only arenas across calls; the caller must not hand the same dict to another
     forward while this call's state is still needed (renderer.py keeps one dict for inference and a pool of dicts for
     differentiated forwards); stream order makes the re-use safe."""
@@ -220,34 +225,57 @@ def _render_batch_forward_one(xyz, features, scaling, rotation, opacity, H, W, C
                 raise ValueError("mse_loss_sum must be a float64 tensor with one entry per sample")
             mse = RenderMse(target=mse_target.data_ptr(), target_channels=mse_target.shape[2],
                             loss_sum=mse_loss_sum.data_ptr(), coef=None, images=None)
-        check(_lib.lib().dgs_render_batch_forward_mse(C.byref(a), geom.cb, None, binning.cb, None, img.cb, None,
-                                                      out.data_ptr(), C.byref(R), chunks,
-                                                      None if mse is None else C.byref(mse), _stream(dev)))
+        maps, aux_args = (), None
+        if aux:
+            maps = tuple(torch.empty(B, V, 1, int(H), int(W), dtype=torch.float32, device=dev) for _ in range(2))
+            aux_args = RenderAux(depth=maps[0].data_ptr(), alpha=maps[1].data_ptr(), dL_ddepth=None, dL_dalpha=None)
+        L = _lib.lib()
+        fn, extra = (L.dgs_render_batch_forward_mse, ()) if aux_args is None else \
+            (L.dgs_render_batch_forward_aux, (C.byref(aux_args),))
+        check(fn(C.byref(a), geom.cb, None, binning.cb, None, img.cb, None, out.data_ptr(), C.byref(R), chunks,
+                 None if mse is None else C.byref(mse), *extra, _stream(dev)))
     global LAST_NUM_RENDERED
     LAST_NUM_RENDERED = R.value
     state = dict(mse_target=mse_target, images=out if mse_target is not None else None, tensors=tens, geom=geom.tensor, binning=binning.tensors[0],
                  binning_b=binning.tensors[1] if len(binning.tensors) > 1 else None, img=img.tensor, R=R.value,
                  chunks=(int(chunks[0]), int(chunks[1])), H=int(H), W=int(W), scale_modifier=scale_modifier,
                  near_log2=near_log2)
-    return out, state
+    return (out, *maps, state)
 
 
-def render_batch_backward(state, grad_images, arena_cache=None, mse_coef=None):
+def _view_slice(t, v0, v1):
+    return None if t is None else t[:, v0:v1]
+
+
+def render_batch_backward(state, grad_images, arena_cache=None, mse_coef=None, grad_depth=None, grad_alpha=None):
     """-> (d_xyz, d_features, d_scaling, d_rotation, d_opacity), re-using the forward's sorted lists.
     mse_coef (fp32 [B], device): dL/dpix += mse_coef[b] * (render - target) is formed inside the blend-backward kernel
-    (the forward must have been given mse_target); grad_images may then be None."""
+    (the forward must have been given mse_target); grad_images may then be None.
+    grad_depth / grad_alpha ([B,V,1,H,W], either may be None): upstream gradients of the aux=True forward's depth and alpha
+    maps (dgs_render_batch_backward_aux); without them the plain kernels run."""
     if "sub" in state:  # view-chunked forward: the per-Gaussian gradients are sums over views
         total = None
         for ci, (v0, v1, st) in enumerate(state["sub"]):
             sub_cache = None if arena_cache is None else arena_cache.setdefault(("views", ci), {})
-            g = render_batch_backward(st, None if grad_images is None else grad_images[:, v0:v1], sub_cache, mse_coef)
+            maps = {}  # a plain backward passes the plain backward's arguments only
+            if grad_depth is not None or grad_alpha is not None:
+                maps = dict(grad_depth=_view_slice(grad_depth, v0, v1), grad_alpha=_view_slice(grad_alpha, v0, v1))
+            g = render_batch_backward(st, _view_slice(grad_images, v0, v1), sub_cache, mse_coef, **maps)
             total = g if total is None else tuple(a + b for a, b in zip(total, g))
         return total
     tens = state["tensors"]
     dev = tens[0].device
     g = _f32c(grad_images)
-    if g is None and mse_coef is None:
-        raise ValueError("render_batch_backward needs grad_images or mse_coef")
+    gd, ga = _f32c(grad_depth), _f32c(grad_alpha)
+    if g is None and mse_coef is None and gd is None and ga is None:
+        raise ValueError("render_batch_backward needs grad_images, mse_coef, grad_depth or grad_alpha")
+    aux = None
+    if gd is not None or ga is not None:
+        shape = (tens[0].shape[0], tens[5].shape[1], 1, state["H"], state["W"])
+        for name, t in (("grad_depth", gd), ("grad_alpha", ga)):
+            if t is not None and tuple(t.shape) != shape:
+                raise ValueError(f"{name} shape {tuple(t.shape)} != {list(shape)}")
+        aux = RenderAux(depth=None, alpha=None, dL_ddepth=_ptr(gd), dL_dalpha=_ptr(ga))
     mse = None
     if mse_coef is not None:
         if state.get("mse_target") is None:
@@ -260,10 +288,13 @@ def render_batch_backward(state, grad_images, arena_cache=None, mse_coef=None):
         scratch = _Arena(dev, arena_cache, "bwd_scratch")
         a = _batch_args(*tens, state["H"], state["W"], state["scale_modifier"], near_log2=state["near_log2"])
         chunks = (C.c_longlong * 2)(*state["chunks"])
-        check(_lib.lib().dgs_render_batch_backward_mse(
+        L = _lib.lib()
+        fn, extra = (L.dgs_render_batch_backward_mse, ()) if aux is None else \
+            (L.dgs_render_batch_backward_aux, (C.byref(aux),))
+        check(fn(
             C.byref(a), state["R"], chunks, _ptr(state["geom"]), _ptr(state["binning"]), _ptr(state["binning_b"]),
             _ptr(state["img"]), None if g is None else g.data_ptr(), None if mse is None else C.byref(mse),
-            outs[0].data_ptr(), outs[1].data_ptr(), outs[2].data_ptr(), outs[3].data_ptr(), outs[4].data_ptr(),
+            *extra, outs[0].data_ptr(), outs[1].data_ptr(), outs[2].data_ptr(), outs[3].data_ptr(), outs[4].data_ptr(),
             scratch.cb, None, _stream(dev)))
     return tuple(outs)
 

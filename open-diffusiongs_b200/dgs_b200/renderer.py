@@ -100,6 +100,47 @@ class BatchedGaussianRenderMSE(torch.autograd.Function):
         return (*grads, None, None, None, None, None, None, None)
 
 
+class BatchedGaussianRenderBuffers(torch.autograd.Function):
+    """BatchedGaussianRender plus the depth and alpha maps of the same blend -> (images [b,v,3,H,W],
+    depth [b,v,1,H,W] = sum_i w_i z_i (accumulated view-space depth), alpha [b,v,1,H,W] = 1 - final T).  An output that
+    receives no gradient costs nothing in the backward; with none of depth and alpha it is the plain backward."""
+
+    @staticmethod
+    def forward(ctx, xyz, features, scaling, rotation, opacity, height, width, C2W, fxfycxcy, scaling_modifier=None,
+                arena_cache=None):
+        ctx.set_materialize_grads(False)
+        needs_bwd = any(ctx.needs_input_grad[:5])
+        cache = None
+        if arena_cache is not None:
+            if needs_bwd:
+                pool = arena_cache.setdefault("pool", [])
+                cache = pool.pop() if pool else {}
+            else:
+                cache = arena_cache.setdefault("infer", {})
+        with torch.no_grad():
+            images, depth, alpha, state = _raster.render_batch_forward(xyz, features, scaling, rotation, opacity, height,
+                                                                       width, C2W, fxfycxcy, scaling_modifier,
+                                                                       arena_cache=cache, aux=True)
+        ctx.state = state
+        ctx.pool = (arena_cache, cache) if needs_bwd and arena_cache is not None else None
+        ctx.in_dtypes = (xyz.dtype, features.dtype, scaling.dtype, rotation.dtype, opacity.dtype)
+        return images, depth, alpha
+
+    @staticmethod
+    def backward(ctx, g_images, g_depth, g_alpha):
+        cache = ctx.pool[1] if ctx.pool else None
+        grads = (None,) * 5
+        if g_images is not None or g_depth is not None or g_alpha is not None:
+            grads = _raster.render_batch_backward(ctx.state, g_images, arena_cache=cache, grad_depth=g_depth,
+                                                  grad_alpha=g_alpha)
+            grads = tuple(g.to(dt) for g, dt in zip(grads, ctx.in_dtypes))
+        ctx.state = None
+        if ctx.pool:
+            ctx.pool[0]["pool"].append(cache)
+            ctx.pool = None
+        return (*grads, None, None, None, None, None, None)
+
+
 batched_gaussian_render = BatchedGaussianRender.apply
 deferred_gaussian_render = batched_gaussian_render  # reference name (gs_core.py:1064)
 
@@ -389,6 +430,18 @@ class Renderer(nn.Module):
                                              self.scaling_modifier, self._arena_cache)
         self.last_num_rendered = _raster.LAST_NUM_RENDERED
         return out
+
+    @torch.amp.custom_fwd(device_type="cuda", cast_inputs=torch.float32)
+    def forward_buffers(self, xyz, features, scaling, rotation, opacity, height, width, C2W, fxfycxcy):
+        """forward() plus per-pixel depth and alpha from the same blend, in the same launch set ->
+        dict(render [b,v,3,H,W], depth [b,v,1,H,W], alpha [b,v,1,H,W]), the keys of the reference's planned
+        edict(render=..., depth=..., alpha=...).  depth = sum_i w_i z_i with w_i the colour's blend weight and z_i the
+        Gaussian's view-space depth (background 0), the ACCUMULATED depth: expected depth is depth / alpha.
+        alpha = 1 - final transmittance.  render equals forward()'s output bit for bit; all three are differentiable."""
+        render, depth, alpha = BatchedGaussianRenderBuffers.apply(xyz, features, scaling, rotation, opacity, height, width,
+                                                                  C2W, fxfycxcy, self.scaling_modifier, self._arena_cache)
+        self.last_num_rendered = _raster.LAST_NUM_RENDERED
+        return dict(render=render, depth=depth, alpha=alpha)
 
     def new_gaussians_model(self):
         return copy.deepcopy(self.gaussians_model)
