@@ -281,8 +281,8 @@ int dgs_dit_forward(const dgs_dit_weights* w, const dgs_dit_io* io, void* worksp
  * one fp32 scale per row and 128-column group, stored transposed as [K/128][round_up(M, 4)].  Every scale is a power
  * of two, 2^ceil(log2(amax / 448)) (1 for an all-zero group), so quantizing is an exact scaling and one
  * round-to-nearest-even: q = e4m3(x / s).  A GEMM computes sw[n] * sum over k-blocks of sa[kb][m] * (qa qw^T)_kb, then
- * the bf16 path's epilogue.  Everything else (input stage, conditioning, attention, attn.proj, heads) is the bf16 path;
- * there is no FP8 training. */
+ * the bf16 path's epilogue.  Everything else (input stage, conditioning, attention unless DGS_FP8_ATTENTION, attn.proj,
+ * heads) is the bf16 path; there is no FP8 training. */
 typedef struct {
   const void* qkv_w; const float* qkv_s;  /* e4m3 [L, 3w, w], fp32 [L, 3w] */
   const void* fc1_w; const float* fc1_s;  /* e4m3 [L, 4w, w], fp32 [L, 4w] */
@@ -307,6 +307,32 @@ int dgs_ln_modulate_fp8(const float* x, const float* shift, const float* scale, 
 int dgs_gemm_fp8(const void* A, const float* sa, const void* W, const float* sw, const float* bias, const float* gate,
                  void* out, float* out_scale, int M, int N, int K, int epi, int ldc, int gate_stride,
                  int rows_per_sample, void* stream);
+
+/* ---- opt-in FP8 attention: flags of the _ex FP8 forward ----
+ * DGS_FP8_ATTENTION: besides the three GEMMs, the attention forward of every block runs both of its products (Q K^T and
+ * P V) on e4m3 operands.  A quantize pass turns the bf16 qkv GEMM output [B, N, 3, H, 64] into (Nk = round_up(N, 128)):
+ *   q8, k8  e4m3 [B, N, H, 64];
+ *   vt8     e4m3 [B, H, 64, Nk]: V transposed (keys contiguous, one 128-key block = one 128-byte row).  Within every 16
+ *           keys, slot a holds key 2 (a / 4) + (a % 2) + 8 ((a / 2) % 2) (the order that maps the fp32 score
+ *           accumulator's columns onto the e4m3 A fragment of P V); the pad keys past N are zeros;
+ *   sq      fp32 [B, H, N]:       one scale per (token, head);
+ *   sk, sv  fp32 [B, H, Nk/128]: one scale per (128-key block, head), over the valid keys.
+ * Every scale follows the FP8 rule above.  The kernel computes, per 128-key block j, the probabilities
+ * P = 2^(s sq sk_j log2(e) / 8 - m + 8) (m: the running row max, log2 units) rounded to e4m3, accumulates O in units of
+ * the block's V scale (rescaled by alpha sv_{j-1} / sv_j from block to block) and divides by the fp32 row sums at the end.
+ * Inference only: no log-sum-exp is stored. */
+#define DGS_FP8_ATTENTION 1
+/* dgs_dit_workspace_bytes_fp8 for the given flags (0: the same); 0 for unknown flags */
+size_t dgs_dit_workspace_bytes_fp8_ex(const dgs_dit_weights* w, int B, int V, int H, int W, int flags);
+/* dgs_dit_forward_fp8 with flags (0 == dgs_dit_forward_fp8); the workspace is dgs_dit_workspace_bytes_fp8_ex's */
+int dgs_dit_forward_fp8_ex(const dgs_dit_weights* w, const dgs_dit_weights_fp8* w8, const dgs_dit_io* io, int flags,
+                           void* workspace, size_t workspace_bytes, void* stream);
+/* The two steps of the FP8 attention (the kernels the forward launches): the quantize pass, then the attention on its
+ * output -> out [B, N, heads*64] bf16.  head_dim 64. */
+int dgs_attention_quantize_e4m3(const void* qkv, void* q8, void* k8, void* vt8, float* sq, float* sk, float* sv,
+                                int B, int N, int heads, void* stream);
+int dgs_attention_fwd_fp8(const void* q8, const void* k8, const void* vt8, const float* sq, const float* sk,
+                          const float* sv, void* out, int B, int N, int heads, void* stream);
 
 /* ---- training: backward of dgs_dit_forward (what torch autograd derives for denoiser.py:306-416 in the reference) ----
  * dgrad GEMMs read TRANSPOSED bf16 copies of the block weights (W^T, [in, out] row-major) so that every GEMM of the

@@ -13,6 +13,7 @@ namespace {
 struct DitDims {
   int B, T, G, N, M, Mp, Mt, Mtp;
   int D, U;          // width, mlp_hidden
+  int heads;
   int Kin, Ndec;     // patch*patch*9 tokenizer inputs, patch*patch*14 decoder outputs per token
   int mod_stride;    // L*6w + 4w: the adaLN modulation of every block and of both heads, per sample
   size_t MD, MU;     // elements of an [M, w] and an [M, mlp_hidden] tensor
@@ -20,7 +21,7 @@ struct DitDims {
   DitDims(const dgs_dit_weights* w, int B_, int V, int H, int W)
       : B(B_), T(V * (H / w->patch) * (W / w->patch)), G(w->n_gaussians), N(T + G), M(B * N), Mp((M + 63) / 64 * 64),
         Mt(B * T), Mtp((Mt + 63) / 64 * 64), D(w->width), U(w->mlp_hidden), Kin(w->patch * w->patch * 9),
-        Ndec(w->patch * w->patch * 14), mod_stride(w->layers * 6 * D + 4 * D), MD((size_t)M * D), MU((size_t)M * U),
+        Ndec(w->patch * w->patch * 14), heads(w->heads), mod_stride(w->layers * 6 * D + 4 * D), MD((size_t)M * D), MU((size_t)M * U),
         lse_n((size_t)B * w->heads * attention_lse_stride(N)) {}
 };
 
@@ -43,8 +44,12 @@ struct DitWorkspace {
   // [w/128][Ms]) and u (GELU output, [4w/128][Ms]); the e4m3 activations themselves live in h / u.
   float* sa_h;
   float* sa_u;
-  size_t bytes;      // without the FP8 scales
-  size_t bytes_fp8;  // with them
+  // DGS_FP8_ATTENTION only, carved after those: the e4m3 attention operands of one block and their scales
+  uint8_t *q8, *k8, *vt8;
+  float *sq, *sk, *sv;
+  size_t bytes;          // without the FP8 scales
+  size_t bytes_fp8;      // with them
+  size_t bytes_fp8_att;  // with the FP8 attention operands as well
   DitWorkspace(void* base, const DitDims& d) {
     Carver c_(base);
     tokens = c_.take<__nv_bfloat16>((size_t)d.Mt * 3 * d.Kin);
@@ -66,6 +71,14 @@ struct DitWorkspace {
     sa_h = c_.take<float>((size_t)(d.D / 128) * Ms);
     sa_u = c_.take<float>((size_t)(d.U / 128) * Ms);
     bytes_fp8 = c_.bytes();
+    const size_t Nk = attention_lse_stride(d.N), BH = (size_t)d.B * d.heads;
+    q8 = c_.take<uint8_t>(d.MD);
+    k8 = c_.take<uint8_t>(d.MD);
+    vt8 = c_.take<uint8_t>(BH * 64 * Nk);
+    sq = c_.take<float>(BH * d.N);
+    sk = c_.take<float>(BH * Nk / 128);
+    sv = c_.take<float>(BH * Nk / 128);
+    bytes_fp8_att = c_.bytes();
   }
 };
 
@@ -169,6 +182,8 @@ struct BlockBufs {
   __nv_bfloat16 *proj_out, *fc2_out, *u_pre;  // training only (NULL: not stored)
   float* lse;                                  // training only
   float *sa_h, *sa_u;                          // FP8 only: the activation scales of h1 / h2 and of u
+  uint8_t *q8, *k8, *vt8;                      // DGS_FP8_ATTENTION only: the e4m3 attention operands ...
+  float *sq, *sk, *sv;                         // ... and their scales
 };
 
 enum BlockPlan { PLAN_INFER, PLAN_STORE, PLAN_RECOMPUTE, PLAN_REFILL };
@@ -188,6 +203,7 @@ BlockBufs block_bufs(BlockPlan plan, int l, const DitDims& d, const DitWorkspace
     b.x_in = b.x_mid = b.x_out = ws.x;
     b.h1 = b.h2 = ws.h; b.qkv = ws.qkv; b.attn = ws.attn; b.u = ws.u;
     b.sa_h = ws.sa_h; b.sa_u = ws.sa_u;
+    b.q8 = ws.q8; b.k8 = ws.k8; b.vt8 = ws.vt8; b.sq = ws.sq; b.sk = ws.sk; b.sv = ws.sv;
     if (plan == PLAN_RECOMPUTE) b.x_save = ts.x_all + (size_t)l * d.MD;
     return b;
   }
@@ -203,9 +219,10 @@ BlockBufs block_bufs(BlockPlan plan, int l, const DitDims& d, const DitWorkspace
 }
 
 // One DiTBlock forward.  w8 != NULL: the LayerNorms emit e4m3 and qkv, fc1 and fc2 run on the FP8 weights (inference
-// only); attention and attn.proj are the bf16 path's either way.
-int block_forward(const dgs_dit_weights* w, const dgs_dit_weights_fp8* w8, int l, const float* m, const DitDims& d,
-                  const BlockBufs& b, cudaStream_t st) {
+// only); attn.proj is the bf16 path's either way, attention too unless fp8_flags has DGS_FP8_ATTENTION (then the qkv
+// output is quantized to e4m3 and attention runs on it).
+int block_forward(const dgs_dit_weights* w, const dgs_dit_weights_fp8* w8, int fp8_flags, int l, const float* m,
+                  const DitDims& d, const BlockBufs& b, cudaStream_t st) {
   const int B = d.B, N = d.N, M = d.M, D = d.D, U = d.U, ms = d.mod_stride;
   {
     ProfScope ps(st, PROF_DIT_LN);
@@ -223,7 +240,12 @@ int block_forward(const dgs_dit_weights* w, const dgs_dit_weights_fp8* w8, int l
   }
   {
     ProfScope ps(st, PROF_DIT_ATTN);
-    DGS_TRY(attention_fwd(b.qkv, b.attn, b.lse, B, N, w->heads, st));
+    if (fp8_flags & DGS_FP8_ATTENTION) {
+      DGS_TRY(attention_quantize_e4m3(b.qkv, b.q8, b.k8, b.vt8, b.sq, b.sk, b.sv, B, N, w->heads, st));
+      DGS_TRY(attention_fwd_e4m3(b.q8, b.k8, b.vt8, b.sq, b.sk, b.sv, b.attn, B, N, w->heads, st));
+    } else {
+      DGS_TRY(attention_fwd(b.qkv, b.attn, b.lse, B, N, w->heads, st));
+    }
   }
   {
     ProfScope ps(st, PROF_DIT_GEMM_PROJ);
@@ -264,9 +286,10 @@ int block_forward(const dgs_dit_weights* w, const dgs_dit_weights_fp8* w8, int l
   return DGS_OK;
 }
 
-// dgs_dit_forward (w8 == NULL) and dgs_dit_forward_fp8 (w8 != NULL: inference with the FP8 block GEMMs)
-int dit_forward(const dgs_dit_weights* w, const dgs_dit_weights_fp8* w8, const dgs_dit_io* io, void* workspace,
-                size_t workspace_bytes, cudaStream_t st) {
+// dgs_dit_forward (w8 == NULL) and dgs_dit_forward_fp8_ex (w8 != NULL: inference with the FP8 block GEMMs, plus the
+// FP8 attention with fp8_flags = DGS_FP8_ATTENTION)
+int dit_forward(const dgs_dit_weights* w, const dgs_dit_weights_fp8* w8, int fp8_flags, const dgs_dit_io* io,
+                void* workspace, size_t workspace_bytes, cudaStream_t st) {
   DGS_REQUIRE(io != nullptr, "io is NULL");
   DGS_TRY(check_dit(w, io->B, io->V, io->H, io->W));
   DGS_REQUIRE(io->images && io->ray_o && io->ray_d && io->t, "NULL input");
@@ -274,7 +297,7 @@ int dit_forward(const dgs_dit_weights* w, const dgs_dit_weights_fp8* w8, const d
   const DitDims d(w, io->B, io->V, io->H, io->W);
   const int B = d.B, T = d.T, N = d.N, G = d.G, D = d.D, L = w->layers, p = w->patch, mod_stride = d.mod_stride;
   DitWorkspace ws(workspace, d);
-  const size_t need = w8 ? ws.bytes_fp8 : ws.bytes;
+  const size_t need = !w8 ? ws.bytes : (fp8_flags & DGS_FP8_ATTENTION) ? ws.bytes_fp8_att : ws.bytes_fp8;
   DGS_REQUIRE(workspace && workspace_bytes >= need, "workspace too small: %zu < %zu", workspace_bytes, need);
   const bool train = io->train_state != nullptr;
   DGS_TRY(check_train_mode(io->train_mode));
@@ -308,7 +331,7 @@ int dit_forward(const dgs_dit_weights* w, const dgs_dit_weights_fp8* w8, const d
     const float* m = ws.mod + (size_t)l * 6 * D;  // shift_msa | scale_msa | gate_msa | shift_mlp | scale_mlp | gate_mlp
     const BlockBufs bb = block_bufs(plan, l, d, ws, ts);
     if (bb.x_save) DGS_CUDA_OK(cudaMemcpyAsync(bb.x_save, bb.x_in, d.MD * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    DGS_TRY(block_forward(w, w8, l, m, d, bb, st));
+    DGS_TRY(block_forward(w, w8, fp8_flags, l, m, d, bb, st));
   }
   const BlockBufs fin = block_bufs(plan, L, d, ws, ts);  // the stream leaving the last block
   if (fin.x_save) DGS_CUDA_OK(cudaMemcpyAsync(fin.x_save, fin.x_in, d.MD * sizeof(float), cudaMemcpyDeviceToDevice, st));
@@ -539,20 +562,49 @@ size_t dgs_dit_workspace_bytes(const dgs_dit_weights* w, int B, int V, int H, in
 
 int dgs_dit_forward(const dgs_dit_weights* w, const dgs_dit_io* io, void* workspace, size_t workspace_bytes,
                     void* stream) {
-  return dit_forward(w, nullptr, io, workspace, workspace_bytes, (cudaStream_t)stream);
+  return dit_forward(w, nullptr, 0, io, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 size_t dgs_dit_workspace_bytes_fp8(const dgs_dit_weights* w, int B, int V, int H, int W) {
+  return dgs_dit_workspace_bytes_fp8_ex(w, B, V, H, W, 0);
+}
+
+size_t dgs_dit_workspace_bytes_fp8_ex(const dgs_dit_weights* w, int B, int V, int H, int W, int flags) {
   if (check_dit(w, B, V, H, W)) return 0;
-  return DitWorkspace(nullptr, DitDims(w, B, V, H, W)).bytes_fp8;
+  if (flags & ~DGS_FP8_ATTENTION) {
+    set_error("unknown FP8 flags 0x%x", flags);
+    return 0;
+  }
+  const DitWorkspace ws(nullptr, DitDims(w, B, V, H, W));
+  return (flags & DGS_FP8_ATTENTION) ? ws.bytes_fp8_att : ws.bytes_fp8;
 }
 
 int dgs_dit_forward_fp8(const dgs_dit_weights* w, const dgs_dit_weights_fp8* w8, const dgs_dit_io* io, void* workspace,
                         size_t workspace_bytes, void* stream) {
+  return dgs_dit_forward_fp8_ex(w, w8, io, 0, workspace, workspace_bytes, stream);
+}
+
+int dgs_dit_forward_fp8_ex(const dgs_dit_weights* w, const dgs_dit_weights_fp8* w8, const dgs_dit_io* io, int flags,
+                           void* workspace, size_t workspace_bytes, void* stream) {
   DGS_REQUIRE(w8 && w8->qkv_w && w8->qkv_s && w8->fc1_w && w8->fc1_s && w8->fc2_w && w8->fc2_s, "NULL FP8 weight or scale");
   DGS_REQUIRE(io == nullptr || io->train_state == nullptr,
               "dgs_dit_forward_fp8 is inference only (io->train_state must be NULL; training runs bf16)");
-  return dit_forward(w, w8, io, workspace, workspace_bytes, (cudaStream_t)stream);
+  DGS_REQUIRE((flags & ~DGS_FP8_ATTENTION) == 0, "unknown FP8 flags 0x%x", flags);
+  return dit_forward(w, w8, flags, io, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int dgs_attention_quantize_e4m3(const void* qkv, void* q8, void* k8, void* vt8, float* sq, float* sk, float* sv, int B,
+                                int N, int heads, void* stream) {
+  DGS_REQUIRE(qkv && q8 && k8 && vt8 && sq && sk && sv, "NULL pointer");
+  return attention_quantize_e4m3(qkv, (uint8_t*)q8, (uint8_t*)k8, (uint8_t*)vt8, sq, sk, sv, B, N, heads,
+                                 (cudaStream_t)stream);
+}
+
+int dgs_attention_fwd_fp8(const void* q8, const void* k8, const void* vt8, const float* sq, const float* sk,
+                          const float* sv, void* out, int B, int N, int heads, void* stream) {
+  DGS_REQUIRE(q8 && k8 && vt8 && sq && sk && sv && out, "NULL pointer");
+  return attention_fwd_e4m3((const uint8_t*)q8, (const uint8_t*)k8, (const uint8_t*)vt8, sq, sk, sv, out, B, N, heads,
+                            (cudaStream_t)stream);
 }
 
 int dgs_quantize_rows_e4m3(const float* x, int rows, int cols, void* q, float* scale, void* stream) {
@@ -701,7 +753,7 @@ int dgs_dit_backward_ex(const dgs_dit_weights* w, const dgs_dit_weights_t* wT, c
     const float* m = ws.mod + (size_t)l * 6 * D;
     float* dm = ts.dmod + (size_t)l * 6 * D;
     const BlockBufs b = block_bufs(plan, l, d, ws, ts);
-    if (recompute) DGS_TRY(block_forward(w, nullptr, l, m, d, b, st));  // refill the slot (denoiser.py:348-354)
+    if (recompute) DGS_TRY(block_forward(w, nullptr, 0, l, m, d, b, st));  // refill the slot (denoiser.py:348-354)
     DGS_TRY(block_backward(w, wT, g, tr, l, ws.c, m, dm, d, b, ts, st));
     if (done_ev && done_ev[l]) DGS_CUDA_OK(cudaEventRecord((cudaEvent_t)done_ev[l], st));
   }

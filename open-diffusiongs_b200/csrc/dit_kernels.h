@@ -44,6 +44,13 @@ int gemm_fp8(const void* A, const float* sa, const void* W, const float* sw, int
 // lse2 (optional, training): [B, H, attention_lse_stride(N)] fp32, log2-domain log-sum-exp of the scaled scores
 int attention_fwd(const void* qkv, void* out, float* lse2, int B, int N, int H, cudaStream_t st);
 inline int attention_lse_stride(int N) { return (N + 127) / 128 * 128; }
+// FP8 inference attention (attention_sm90.cu; layouts in include/dgs_b200.h): the quantize pass qkv -> q8 / k8 [B, N, H,
+// 64], vt8 [B, H, 64, Nk] (Nk = attention_lse_stride(N)) with scales sq [B, H, N], sk / sv [B, H, Nk/128]; then the
+// attention forward on those operands -> out [B, N, H*64] (bf16)
+int attention_quantize_e4m3(const void* qkv, uint8_t* q8, uint8_t* k8, uint8_t* vt8, float* sq, float* sk, float* sv,
+                            int B, int N, int H, cudaStream_t st);
+int attention_fwd_e4m3(const uint8_t* q8, const uint8_t* k8, const uint8_t* vt8, const float* sq, const float* sk,
+                       const float* sv, void* out, int B, int N, int H, cudaStream_t st);
 // backward (attention_bwd_sm90.cu): dqkv [B, N, 3, H, 64] (bf16) from qkv, out (= O), lse2 and dout [B, N, H*64] (bf16);
 // dsum = scratch [B, H, attention_lse_stride(N)] fp32.  Fills the pad entries of lse2 (+inf) as a side effect.
 int attention_bwd(const void* qkv, const void* out, const void* dout, float* lse2, float* dsum, void* dqkv, int B, int N,

@@ -59,7 +59,7 @@ static EncodeTiledFn get_encode_fn() {
 }
 
 int make_tmap(CUtensorMap* out, CUtensorMapDataType dtype, const void* base, int rank, const uint64_t* dims,
-              const uint64_t* strides_bytes, const uint32_t* box) {
+              const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapSwizzle swizzle) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) { set_error("cuTensorMapEncodeTiled not available (no CUDA driver?)"); return DGS_ERR_CUDA; }
   cuuint64_t gdim[5], gstr[5];
@@ -67,7 +67,7 @@ int make_tmap(CUtensorMap* out, CUtensorMapDataType dtype, const void* base, int
   for (int i = 0; i < rank; i++) { gdim[i] = dims[i]; bx[i] = box[i]; es[i] = 1; }
   for (int i = 0; i + 1 < rank; i++) gstr[i] = strides_bytes[i];
   CUresult r = fn(out, dtype, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx, es,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed with CUresult %d", (int)r); return DGS_ERR_CUDA; }
   return DGS_OK;

@@ -173,6 +173,16 @@ __device__ __forceinline__ uint64_t wg_desc_sw128(uint32_t smem_addr, uint32_t l
   d |= (uint64_t)1 << 62;
   return d;
 }
+// The same with a 64-byte swizzle: K-major tile rows of exactly 64 bytes (64 e4m3), tile base 512-byte aligned, 8-row
+// groups SBO = 512 B apart.  One k32 step of an e4m3 operand advances the start address by 32 B inside the row.
+__device__ __forceinline__ uint64_t wg_desc_sw64(uint32_t smem_addr, uint32_t sbo_bytes) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
+  d |= (uint64_t)2 << 62;
+  return d;
+}
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
@@ -238,13 +248,24 @@ __device__ __forceinline__ void wgmma_m64n64_rs(float (&d)[32], const uint32_t (
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "n"(TB));
 }
+// e4m3 x e4m3 -> fp32, A from registers, B K-major from shared memory.  A fragment of a k32 slice (thread t = 4 g + u of
+// warp w, rows 16 w + g + {0, 8}): a[0] = row +0, k 4u..4u+3; a[1] = row +8, same k; a[2] / a[3] = the same rows at
+// k 16+4u..16+4u+3; byte i of a register is element k + i.
+__device__ __forceinline__ void wgmma_m64n64k32_e4m3_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t db) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n64k32.f32.e4m3.e4m3 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, 1, 1, 1;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
+}
 
 }  // namespace ptx
 
 // host: cuTensorMapEncodeTiled through the runtime's driver entry point (no link-time libcuda dependency),
-// 128-byte swizzle
+// 128-byte swizzle unless told otherwise
 int make_tmap(CUtensorMap* out, CUtensorMapDataType dtype, const void* base, int rank, const uint64_t* dims,
-              const uint64_t* strides_bytes, const uint32_t* box);
+              const uint64_t* strides_bytes, const uint32_t* box,
+              CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B);
 inline int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                           const uint32_t* box) {
   return make_tmap(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, base, rank, dims, strides_bytes, box);

@@ -50,6 +50,7 @@ class DitWeightsFp8(C.Structure):  # dgs_dit_weights_fp8
 
 
 FP8_EPI_BIAS_BF16, FP8_EPI_GATE_RESID_F32, FP8_EPI_F32, FP8_EPI_BIAS_GELU_E4M3 = 0, 2, 3, 6  # dgs_gemm_fp8 epi
+FP8_ATTENTION = 1  # DGS_FP8_ATTENTION, a flag of dgs_dit_forward_fp8_ex
 
 
 BWD_TRACE_FIELDS = ("dx", "dx_mid", "d_fc2_out", "du_pre", "dh2", "d_proj_out", "d_attn", "dsum", "dqkv", "dh1")
@@ -196,6 +197,12 @@ def lib():
         L.dgs_quantize_rows_e4m3.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp]
         L.dgs_ln_modulate_fp8.argtypes = [vp, vp, vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_float, vp]
         L.dgs_gemm_fp8.argtypes = [vp] * 8 + [C.c_int] * 7 + [vp]
+        L.dgs_dit_workspace_bytes_fp8_ex.restype = C.c_size_t
+        L.dgs_dit_workspace_bytes_fp8_ex.argtypes = [C.POINTER(DitWeights)] + [C.c_int] * 5
+        L.dgs_dit_forward_fp8_ex.argtypes = [C.POINTER(DitWeights), C.POINTER(DitWeightsFp8), C.POINTER(DitIO), C.c_int, vp,
+                                             C.c_size_t, vp]
+        L.dgs_attention_quantize_e4m3.argtypes = [vp] * 7 + [C.c_int] * 3 + [vp]
+        L.dgs_attention_fwd_fp8.argtypes = [vp] * 7 + [C.c_int] * 3 + [vp]
         L.dgs_mesh_field.argtypes = [C.c_int, vp, vp, vp, vp, C.c_float, vp, C.c_float, C.c_int, C.c_int, C.c_double,
                                      vp, vp, vp, C.POINTER(C.c_longlong), ALLOC_FN, vp, vp]
         L.dgs_marching_cubes.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_float, ALLOC_FN, vp, C.POINTER(C.c_void_p),
@@ -239,4 +246,5 @@ EXPORTED = [  # every symbol include/dgs_b200.h declares (checked by tests/test_
     "dgs_ssim_workspace_bytes", "dgs_ssim_state_bytes", "dgs_ssim_forward", "dgs_ssim_backward",
     "dgs_dit_workspace_bytes_fp8", "dgs_dit_forward_fp8", "dgs_quantize_rows_e4m3", "dgs_ln_modulate_fp8", "dgs_gemm_fp8",
     "dgs_mesh_field", "dgs_marching_cubes", "dgs_render_batch_forward_aux", "dgs_render_batch_backward_aux",
+    "dgs_dit_workspace_bytes_fp8_ex", "dgs_dit_forward_fp8_ex", "dgs_attention_quantize_e4m3", "dgs_attention_fwd_fp8",
 ]

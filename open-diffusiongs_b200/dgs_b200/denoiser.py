@@ -224,9 +224,11 @@ class DGSDenoiser(nn.Module):
     # ---- inference precision ----
     def set_inference_precision(self, precision):
         """"bf16" (default): every GEMM on bf16 operands.  "fp8": inference runs the qkv, mlp.fc1 and mlp.fc2 GEMMs of
-        every block on e4m3 operands with power-of-two scales (dgs_dit_forward_fp8); training refuses to run."""
-        if precision not in ("bf16", "fp8"):
-            raise ValueError(f"inference precision {precision!r} (expected 'bf16' or 'fp8')")
+        every block on e4m3 operands with power-of-two scales (dgs_dit_forward_fp8).  "fp8_attention": "fp8" plus both
+        products of every block's attention on e4m3 operands (DGS_FP8_ATTENTION).  Training refuses to run in either FP8
+        mode."""
+        if precision not in ("bf16", "fp8", "fp8_attention"):
+            raise ValueError(f"inference precision {precision!r} (expected 'bf16', 'fp8' or 'fp8_attention')")
         self._precision = precision
         return self
 
@@ -248,7 +250,7 @@ class DGSDenoiser(nn.Module):
         in train() mode that has a DitTrainer attached (dgs_b200/train.py), the call is recorded as ONE autograd node
         whose backward is dgs_dit_backward (activations stored, not recomputed)."""
         if torch.is_grad_enabled() and self.training and getattr(self, "_trainer", None) is not None:
-            if self._precision == "fp8":
+            if self._precision != "bf16":
                 raise RuntimeError("DGSDenoiser: FP8 is an inference precision; training runs bf16 "
                                    "(set_inference_precision('bf16') before a training forward)")
             from .train import dit_train_forward
@@ -285,8 +287,12 @@ class DGSDenoiser(nn.Module):
             n_tok = c.n_gaussians + V * (H // c.patch_size) * (W // c.patch_size)
             tokens = new(B, n_tok, c.width) if return_tokens else None
             L = _lib.lib()
-            fp8 = self._precision == "fp8" and train_state is None
-            nbytes = (L.dgs_dit_workspace_bytes_fp8 if fp8 else L.dgs_dit_workspace_bytes)(C.byref(w), B, V, H, W)
+            fp8 = self._precision != "bf16" and train_state is None
+            flags = _lib.FP8_ATTENTION if self._precision == "fp8_attention" else 0
+            if fp8:
+                nbytes = L.dgs_dit_workspace_bytes_fp8_ex(C.byref(w), B, V, H, W, flags)
+            else:
+                nbytes = L.dgs_dit_workspace_bytes(C.byref(w), B, V, H, W)
             if nbytes == 0:
                 raise _lib.DgsError(L.dgs_last_error().decode())
             ws = getattr(self, "_workspace", None)  # grow-only, re-used step after step
@@ -303,7 +309,7 @@ class DGSDenoiser(nn.Module):
             stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
             if fp8:
                 w8, _keep8 = self.packed_weights_fp8()
-                check(L.dgs_dit_forward_fp8(C.byref(w), C.byref(w8), C.byref(io), ws.data_ptr(), nbytes, stream))
+                check(L.dgs_dit_forward_fp8_ex(C.byref(w), C.byref(w8), C.byref(io), flags, ws.data_ptr(), nbytes, stream))
             else:
                 check(L.dgs_dit_forward(C.byref(w), C.byref(io), ws.data_ptr(), nbytes, stream))
         keep = (io, ws, nbytes, images, ray_o, ray_d, tf, w, _keep)  # what a later dgs_dit_backward needs alive
