@@ -589,6 +589,33 @@ int dgs_mesh_field(int P, const float* xyz, const float* scaling, const float* r
 int dgs_marching_cubes(const float* field, int nx, int ny, int nz, float iso, dgs_alloc_fn alloc, void* alloc_user,
                        float** vertices, int** triangles, long long* num_vertices, long long* num_triangles,
                        void* stream);
+/* Quadric edge-collapse decimation (the reference's decimate_mesh, utils/mesh_utils.py:44-85: pymeshlab's
+ * meshing_decimation_quadric_edge_collapse(targetfacenum, optimalplacement=True)) of a welded triangle mesh such as
+ * dgs_marching_cubes emits: vertices (device fp32 [V, 3]) and faces (device int32 [F, 3], every index in [0, V), none
+ * repeated within a face; checked on the device, a bad face is DGS_ERR_INVALID_ARGUMENT naming it).
+ * Garland-Heckbert quadrics in fp64: each face's area-weighted plane quadric, summed per vertex in face order; a
+ * collapse of (a, b) adds Q_a + Q_b.  Placement: the minimiser of v^T (Q_a + Q_b) v; when that 3 x 3 system is singular
+ * or ill-conditioned, its solution not finite, or farther than |a - b| from the midpoint, the best of a, b and the
+ * midpoint instead.  An edge is never collapsed when:
+ *   - an endpoint is locked: both ends of every input edge with a face count other than 2 (boundary, non-manifold), so
+ *     boundary loops come back unchanged (pymeshlab's preserve_border behaviour, not its default);
+ *   - the link condition fails: a and b have a common neighbour besides the apexes c != d of their two faces, or the
+ *     faces (a, c, d) and (b, c, d) both exist;
+ *   - a face around a or b not containing both would flip or become degenerate (new normal . old normal <= 0); faces
+ *     that already had zero area are exempt.
+ * Collapses run in rounds of independent edges (each taken edge has the smallest cost within two hops of its
+ * endpoints); each removes exactly two faces.  The last round takes only the cheapest edges, so the result has
+ * target_faces or target_faces - 1 faces, unless no edge can be collapsed first (then whatever is left: not an error).
+ * The lower index survives at the new position; winding is kept.  The output keeps the surviving vertices in index order
+ * and the surviving faces in face order, and is the same bits on every run; with F <= target_faces it is the input, bit
+ * for bit (unreferenced vertices included).  *rounds (NULL or host) receives the number of rounds that collapsed edges.
+ * alloc is called once for scratch (about 330 B per face plus 140 B per vertex, sized once, free after the call), then,
+ * after the last host sync, for *out_vertices (fp32 [V', 3]) and *out_faces (int32 [F', 3]) when they are not empty;
+ * empty outputs are NULL.  The stream is synchronised once to check the indices and once per round. */
+int dgs_mesh_decimate(const float* vertices, long long num_vertices, const int* faces, long long num_faces,
+                      long long target_faces, dgs_alloc_fn alloc, void* alloc_user, float** out_vertices,
+                      int** out_faces, long long* out_num_vertices, long long* out_num_faces, int* rounds,
+                      void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * B3. The elementwise callers either side of the path.

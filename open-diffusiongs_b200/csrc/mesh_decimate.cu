@@ -1,0 +1,614 @@
+// mesh_decimate.cu -- quadric edge-collapse decimation of a welded triangle mesh to a target face count: the reference's
+// decimate_mesh (utils/mesh_utils.py:44-85, pymeshlab's meshing_decimation_quadric_edge_collapse with
+// optimalplacement=True), as deterministic rounds of parallel Garland-Heckbert collapses.
+//
+// Setup: every index is checked on the device (one flag, read at the first host sync).  Each face's plane quadric
+// K_f = A_f p p^T (p = (n, -n.x0), unit normal n, area A_f) is formed in fp64; each vertex's quadric Q_v is the sum of
+// its faces' K_f in face order, over a stable radix sort of the (vertex, face) incidences.  No floating-point atomics
+// anywhere, so the output is the same bits on every run.
+//
+// Round: unique undirected edges come from a radix sort of the live faces' half-edges by (min, max) and a run-length
+// pass, with each edge's two apex vertices when it has exactly two faces; the vertex -> face lists come from a stable
+// sort of the incidences (a vertex's neighbours are read through its faces).  Both endpoints of an edge whose face
+// count is not 2 (boundary or non-manifold) are locked for the rest of the call, so open surfaces keep their boundary
+// loops exactly (pymeshlab's preserve_border behaviour, not its default).  A collapse never creates such an edge, so
+// the locks are those of the input.  Per edge (a, b), in fp64: Q = Q_a + Q_b, the optimal position solves the 3 x 3
+// system; it falls back to the best of a, b and their midpoint when the system is singular or ill-conditioned, when
+// the solution is not finite, or when it lies farther than |a - b| from the midpoint (the spikes the reference warns
+// about); cost = v^T Q v.  An edge is not collapsible when an endpoint is locked, when the link condition fails (the
+// common neighbours of a and b are not exactly its apexes c != d, or faces (a,c,d) and (b,c,d) both exist), or when
+// the move flips a face around a or b (new normal . old normal <= 0, which also rejects a face the move makes
+// degenerate; faces that already had zero area are exempt, so coincident marching-cubes vertices collapse cleanly).
+// Selection: key = (fp32 bits of cost) << 32 | edge, m1[v] = min key over v's edges, m2[v] = min m1 over v and its
+// neighbours, and an edge is taken iff key == m2[a] == m2[b] (see select_kernel for why the taken edges are
+// independent).  One read-back per round gives the count; if taking all would pass the target, only the smallest keys
+// are kept.  Apply: the lower index survives at the new position with Q_a += Q_b, b becomes a in every face (winding
+// kept), the two faces with both die and the faces are compacted in order.  Rounds stop at F <= target or when no
+// edge can be taken.  Finish: referenced vertices are compacted in index order and the faces remapped.
+#include <cub/cub.cuh>
+
+#include <algorithm>
+
+#include "dgs_internal.h"
+
+namespace dgs {
+namespace {
+
+constexpr int kThreads = 256;
+constexpr unsigned long long kNoKey = ~0ull;
+constexpr double kMaxCondition = 1e7;  // Frobenius condition number above which the 3 x 3 system is not solved
+
+struct Quadric {
+  double q[10];  // xx xy xz xw yy yz yw zz zw ww of the symmetric 4 x 4 form
+};
+
+struct Edge {
+  int a, b;  // a < b
+  int c, d;  // the apexes of its two faces; -1 unless it has exactly two
+};
+
+struct Counters {
+  unsigned long long bad_face;  // smallest face with an index out of range or repeated; kNoKey if none
+  int num_edges, num_selected, num_faces;
+};
+
+__device__ __forceinline__ double3 sub(double3 u, double3 v) { return make_double3(u.x - v.x, u.y - v.y, u.z - v.z); }
+__device__ __forceinline__ double dot(double3 u, double3 v) { return u.x * v.x + u.y * v.y + u.z * v.z; }
+__device__ __forceinline__ double3 cross(double3 u, double3 v) {
+  return make_double3(u.y * v.z - u.z * v.y, u.z * v.x - u.x * v.z, u.x * v.y - u.y * v.x);
+}
+__device__ __forceinline__ double3 load(const float* __restrict__ pos, int v) {
+  return make_double3(pos[3 * v], pos[3 * v + 1], pos[3 * v + 2]);
+}
+__device__ __forceinline__ double3 round_f32(double3 v) {
+  return make_double3((double)(float)v.x, (double)(float)v.y, (double)(float)v.z);
+}
+__device__ __forceinline__ bool has(int3 f, int x) { return f.x == x || f.y == x || f.z == x; }
+__device__ __forceinline__ int corner(int3 f, int k) { return k == 0 ? f.x : k == 1 ? f.y : f.z; }
+
+__device__ Quadric face_quadric(const float* __restrict__ pos, int3 f) {
+  const double3 p0 = load(pos, f.x);
+  const double3 n = cross(sub(load(pos, f.y), p0), sub(load(pos, f.z), p0));
+  const double len = sqrt(dot(n, n));
+  Quadric K;
+  if (!(len > 0.0) || !isfinite(len)) {
+    for (int i = 0; i < 10; i++) K.q[i] = 0.0;
+    return K;
+  }
+  const double w = 0.5 * len;
+  const double p[4] = {n.x / len, n.y / len, n.z / len, -(n.x * p0.x + n.y * p0.y + n.z * p0.z) / len};
+  int k = 0;
+  for (int i = 0; i < 4; i++)
+    for (int j = i; j < 4; j++) K.q[k++] = w * p[i] * p[j];
+  return K;
+}
+
+__device__ __forceinline__ double quadric_cost(const double* q, double3 v) {
+  return v.x * (q[0] * v.x + 2.0 * (q[1] * v.y + q[2] * v.z + q[3])) + v.y * (q[4] * v.y + 2.0 * (q[5] * v.z + q[6])) +
+         v.z * (q[7] * v.z + 2.0 * q[8]) + q[9];
+}
+
+// The fp32 position the collapse of (pa, pb) moves to under quadric q, and its cost there.
+__device__ double3 placement(const double* q, double3 pa, double3 pb, double& cost) {
+  const double3 mid = round_f32(make_double3(0.5 * (pa.x + pb.x), 0.5 * (pa.y + pb.y), 0.5 * (pa.z + pb.z)));
+  const double a00 = q[0], a01 = q[1], a02 = q[2], a11 = q[4], a12 = q[5], a22 = q[7];
+  const double c00 = a11 * a22 - a12 * a12, c01 = a02 * a12 - a01 * a22, c02 = a01 * a12 - a02 * a11;
+  const double c11 = a00 * a22 - a02 * a02, c12 = a01 * a02 - a00 * a12, c22 = a00 * a11 - a01 * a01;
+  const double det = a00 * c00 + a01 * c01 + a02 * c02;
+  const double nA = sqrt(a00 * a00 + a11 * a11 + a22 * a22 + 2.0 * (a01 * a01 + a02 * a02 + a12 * a12));
+  const double nC = sqrt(c00 * c00 + c11 * c11 + c22 * c22 + 2.0 * (c01 * c01 + c02 * c02 + c12 * c12));
+  if (det != 0.0 && nA * nC <= kMaxCondition * fabs(det)) {  // A v = -b by the adjugate (A symmetric)
+    const double b0 = q[3], b1 = q[6], b2 = q[8];
+    const double3 v = round_f32(make_double3(-(c00 * b0 + c01 * b1 + c02 * b2) / det,
+                                             -(c01 * b0 + c11 * b1 + c12 * b2) / det,
+                                             -(c02 * b0 + c12 * b1 + c22 * b2) / det));
+    const double3 dm = sub(v, mid), ab = sub(pa, pb);
+    if (isfinite(v.x) && isfinite(v.y) && isfinite(v.z) && dot(dm, dm) <= dot(ab, ab)) {
+      cost = quadric_cost(q, v);
+      return v;
+    }
+  }
+  double3 best = mid;
+  cost = quadric_cost(q, mid);
+  const double ca = quadric_cost(q, pa), cb = quadric_cost(q, pb);
+  if (ca < cost) { best = pa; cost = ca; }
+  if (cb < cost) { best = pb; cost = cb; }
+  return best;
+}
+
+// Moving v to p keeps the orientation of every face around v that does not contain `other` (those die): its normal
+// after the move has a positive dot product with its normal before.  Faces with zero area before are exempt.
+__device__ bool keeps_orientation(int v, int other, double3 p, const float* __restrict__ pos,
+                                  const int3* __restrict__ faces, const uint2* __restrict__ vrange,
+                                  const uint32_t* __restrict__ vfaces) {
+  const uint2 r = vrange[v];
+  for (uint32_t i = r.x; i < r.y; i++) {
+    const int3 f = faces[vfaces[i]];
+    if (has(f, other)) continue;
+    double3 p0 = load(pos, f.x), p1 = load(pos, f.y), p2 = load(pos, f.z);
+    const double3 n0 = cross(sub(p1, p0), sub(p2, p0));
+    if (n0.x == 0.0 && n0.y == 0.0 && n0.z == 0.0) continue;
+    if (f.x == v) p0 = p; else if (f.y == v) p1 = p; else p2 = p;
+    if (!(dot(n0, cross(sub(p1, p0), sub(p2, p0))) > 0.0)) return false;
+  }
+  return true;
+}
+
+// The link condition of edge (a, b) with apexes c, d: no common neighbour besides c and d, and not both of the faces
+// (a, c, d) and (b, c, d) (the tetrahedron, which the collapse would fold onto itself).
+__device__ bool link_ok(Edge e, const int3* __restrict__ faces, const uint2* __restrict__ vrange,
+                        const uint32_t* __restrict__ vfaces) {
+  if (e.c == e.d) return false;
+  const uint2 ra = vrange[e.a], rb = vrange[e.b];
+  bool acd = false, bcd = false;
+  for (uint32_t i = ra.x; i < ra.y; i++) {
+    const int3 f = faces[vfaces[i]];
+    if (has(f, e.c) && has(f, e.d) && !has(f, e.b)) acd = true;
+    for (int k = 0; k < 3; k++) {
+      const int x = corner(f, k);
+      if (x == e.a || x == e.b || x == e.c || x == e.d) continue;
+      for (uint32_t j = rb.x; j < rb.y; j++)
+        if (has(faces[vfaces[j]], x)) return false;
+    }
+  }
+  for (uint32_t j = rb.x; j < rb.y; j++) {
+    const int3 g = faces[vfaces[j]];
+    if (has(g, e.c) && has(g, e.d) && !has(g, e.a)) bcd = true;
+  }
+  return !(acd && bcd);
+}
+
+// ---------------------------------------------------------------------------------------------------------- setup
+__global__ void validate_kernel(int F, int V, const int3* __restrict__ faces, Counters* __restrict__ ctr) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= F) return;
+  const int3 t = faces[f];
+  const bool ok = t.x >= 0 && t.x < V && t.y >= 0 && t.y < V && t.z >= 0 && t.z < V && t.x != t.y && t.y != t.z &&
+                  t.x != t.z;
+  if (!ok) atomicMin(&ctr->bad_face, (unsigned long long)f);
+}
+
+// (vertex, face) incidences in face order; a stable sort by vertex makes each vertex's faces one run in face order
+__global__ void incidence_kernel(int n, const int3* __restrict__ faces, uint32_t* __restrict__ keys,
+                                 uint32_t* __restrict__ vals) {
+  const int h = blockIdx.x * blockDim.x + threadIdx.x;
+  if (h >= n) return;
+  keys[h] = (uint32_t)corner(faces[h / 3], h % 3);
+  vals[h] = (uint32_t)(h / 3);
+}
+
+__global__ void ranges_kernel(int n, const uint32_t* __restrict__ keys, uint2* __restrict__ ranges) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t k = keys[i];
+  if (i == 0 || keys[i - 1] != k) ranges[k].x = i;
+  if (i == n - 1 || keys[i + 1] != k) ranges[k].y = i + 1;
+}
+
+__global__ void vertex_quadric_kernel(int V, const float* __restrict__ pos, const int3* __restrict__ faces,
+                                      const uint2* __restrict__ vrange, const uint32_t* __restrict__ vfaces,
+                                      Quadric* __restrict__ Q) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= V) return;
+  Quadric s;
+  for (int i = 0; i < 10; i++) s.q[i] = 0.0;
+  const uint2 r = vrange[v];
+  for (uint32_t i = r.x; i < r.y; i++) {
+    const Quadric K = face_quadric(pos, faces[vfaces[i]]);
+    for (int k = 0; k < 10; k++) s.q[k] += K.q[k];
+  }
+  Q[v] = s;
+}
+
+// ---------------------------------------------------------------------------------------------------------- edges
+__global__ void halfedge_kernel(int n, const int3* __restrict__ faces, int vbits, unsigned long long* __restrict__ keys,
+                                uint32_t* __restrict__ vals) {
+  const int h = blockIdx.x * blockDim.x + threadIdx.x;
+  if (h >= n) return;
+  const int3 f = faces[h / 3];
+  const int u = corner(f, h % 3), w = corner(f, (h % 3 + 1) % 3);
+  keys[h] = ((unsigned long long)min(u, w) << vbits) | (unsigned long long)max(u, w);
+  vals[h] = (uint32_t)h;
+}
+
+__global__ void edge_heads_kernel(int n, const unsigned long long* __restrict__ keys, uint32_t* __restrict__ heads) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  heads[i] = i == 0 || keys[i] != keys[i - 1];
+}
+
+// One thread per sorted half-edge: its edge id; the run's first thread writes the edge, its apexes and the locks.
+__global__ void edge_build_kernel(int n, const unsigned long long* __restrict__ keys, const uint32_t* __restrict__ vals,
+                                  const uint32_t* __restrict__ scan, const int3* __restrict__ faces, int vbits,
+                                  Edge* __restrict__ edges, uint32_t* __restrict__ edge_of, uint8_t* __restrict__ lock,
+                                  Counters* __restrict__ ctr) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t eid = scan[i] - 1;
+  edge_of[vals[i]] = eid;
+  if (i == n - 1) ctr->num_edges = (int)scan[i];
+  const unsigned long long key = keys[i];
+  if (i > 0 && keys[i - 1] == key) return;
+  int j = i + 1;
+  while (j < n && keys[j] == key) j++;
+  Edge e;
+  e.a = (int)(key >> vbits);
+  e.b = (int)(key & ((1ull << vbits) - 1));
+  e.c = e.d = -1;
+  if (j - i == 2) {
+    const uint32_t h0 = vals[i], h1 = vals[i + 1];
+    e.c = corner(faces[h0 / 3], (h0 % 3 + 2) % 3);
+    e.d = corner(faces[h1 / 3], (h1 % 3 + 2) % 3);
+  } else {
+    lock[e.a] = 1;
+    lock[e.b] = 1;
+  }
+  edges[eid] = e;
+}
+
+__global__ void cost_kernel(const Counters* __restrict__ ctr, const Edge* __restrict__ edges,
+                            const float* __restrict__ pos, const Quadric* __restrict__ Q, const uint8_t* __restrict__ lock,
+                            const int3* __restrict__ faces, const uint2* __restrict__ vrange,
+                            const uint32_t* __restrict__ vfaces, unsigned long long* __restrict__ ekey,
+                            float3* __restrict__ eplace) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= ctr->num_edges) return;
+  const Edge e = edges[i];
+  ekey[i] = kNoKey;
+  if (e.c < 0 || lock[e.a] || lock[e.b] || !link_ok(e, faces, vrange, vfaces)) return;
+  double q[10];
+  for (int k = 0; k < 10; k++) q[k] = Q[e.a].q[k] + Q[e.b].q[k];
+  double cost;
+  const double3 v = placement(q, load(pos, e.a), load(pos, e.b), cost);
+  if (!isfinite(cost)) return;
+  if (!keeps_orientation(e.a, e.b, v, pos, faces, vrange, vfaces) ||
+      !keeps_orientation(e.b, e.a, v, pos, faces, vrange, vfaces))
+    return;
+  const float c = cost > 0.0 ? (float)cost : 0.f;
+  ekey[i] = ((unsigned long long)__float_as_uint(c) << 32) | (unsigned)i;
+  eplace[i] = make_float3((float)v.x, (float)v.y, (float)v.z);
+}
+
+// m1[v] = the smallest key of v's edges (the two edges of each of v's faces that contain v)
+__global__ void m1_kernel(int V, const int3* __restrict__ faces, const uint2* __restrict__ vrange,
+                          const uint32_t* __restrict__ vfaces, const uint32_t* __restrict__ edge_of,
+                          const unsigned long long* __restrict__ ekey, unsigned long long* __restrict__ m1) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= V) return;
+  unsigned long long m = kNoKey;
+  const uint2 r = vrange[v];
+  for (uint32_t i = r.x; i < r.y; i++) {
+    const uint32_t f = vfaces[i];
+    const int3 t = faces[f];
+    const int k = t.x == v ? 0 : t.y == v ? 1 : 2;
+    m = min(m, min(ekey[edge_of[3 * f + k]], ekey[edge_of[3 * f + (k + 2) % 3]]));
+  }
+  m1[v] = m;
+}
+
+// m2[v] = the smallest m1 over v and its neighbours (the vertices of its faces)
+__global__ void m2_kernel(int V, const int3* __restrict__ faces, const uint2* __restrict__ vrange,
+                          const uint32_t* __restrict__ vfaces, const unsigned long long* __restrict__ m1,
+                          unsigned long long* __restrict__ m2) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= V) return;
+  unsigned long long m = m1[v];
+  const uint2 r = vrange[v];
+  for (uint32_t i = r.x; i < r.y; i++) {
+    const int3 t = faces[vfaces[i]];
+    m = min(m, min(m1[t.x], min(m1[t.y], m1[t.z])));
+  }
+  m2[v] = m;
+}
+
+// Edge (a, b) is taken iff key == m2[a] == m2[b]: its key is the smallest over every edge touching the closed
+// neighbourhoods of a and b.  If another taken edge (a', b') had an endpoint, say a', in N[a] (a or a neighbour), then
+// key' = m2[a'] <= m1[a] <= key and key = m2[a] <= m1[a'] <= key', so key == key' and, keys holding the edge index, the
+// edges are the same.  So the endpoints of two taken edges are at least two hops apart: no face contains endpoints of
+// both, and no vertex whose position or faces one collapse reads (the link and fold-over tests read a, b, their faces
+// and those faces' vertices) is moved or renamed by the other.  The collapses of a round are independent, and each
+// one's tests hold after all of them are applied.
+__global__ void select_kernel(Counters* __restrict__ ctr, const Edge* __restrict__ edges,
+                              const unsigned long long* __restrict__ ekey, const unsigned long long* __restrict__ m2,
+                              unsigned long long* __restrict__ skey) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= ctr->num_edges) return;
+  const unsigned long long key = ekey[i];
+  const Edge e = edges[i];
+  const bool take = key != kNoKey && m2[e.a] == key && m2[e.b] == key;
+  skey[i] = take ? key : kNoKey;
+  if (take) atomicAdd(&ctr->num_selected, 1);
+}
+
+// The taken edges with key <= *thr (every taken edge when thr is NULL): b retires into a.
+__global__ void apply_kernel(const Counters* __restrict__ ctr, const Edge* __restrict__ edges,
+                             const unsigned long long* __restrict__ skey, const unsigned long long* __restrict__ thr,
+                             const float3* __restrict__ eplace, float* __restrict__ pos, Quadric* __restrict__ Q,
+                             int* __restrict__ to) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= ctr->num_edges) return;
+  const unsigned long long key = skey[i];
+  if (key == kNoKey || (thr && key > *thr)) return;
+  const Edge e = edges[i];
+  const float3 p = eplace[i];
+  pos[3 * e.a] = p.x;
+  pos[3 * e.a + 1] = p.y;
+  pos[3 * e.a + 2] = p.z;
+  for (int k = 0; k < 10; k++) Q[e.a].q[k] += Q[e.b].q[k];
+  to[e.b] = e.a;
+}
+
+__global__ void remap_kernel(int F, int3* __restrict__ faces, const int* __restrict__ to, uint8_t* __restrict__ alive) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= F) return;
+  int3 t = faces[f];
+  if (to[t.x] >= 0) t.x = to[t.x];
+  if (to[t.y] >= 0) t.y = to[t.y];
+  if (to[t.z] >= 0) t.z = to[t.z];
+  faces[f] = t;
+  alive[f] = t.x != t.y && t.y != t.z && t.x != t.z;
+}
+
+// ---------------------------------------------------------------------------------------------------------- finish
+__global__ void used_kernel(int n, const int3* __restrict__ faces, uint32_t* __restrict__ used) {
+  const int h = blockIdx.x * blockDim.x + threadIdx.x;
+  if (h >= n) return;
+  used[corner(faces[h / 3], h % 3)] = 1;
+}
+
+__global__ void emit_kernel(int V, int F, const float* __restrict__ pos, const int3* __restrict__ faces,
+                            const uint32_t* __restrict__ used, const uint32_t* __restrict__ vscan,
+                            float* __restrict__ out_v, int3* __restrict__ out_f) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < V && used[i]) {
+    const uint32_t o = vscan[i] - 1;
+    out_v[3 * o] = pos[3 * i];
+    out_v[3 * o + 1] = pos[3 * i + 1];
+    out_v[3 * o + 2] = pos[3 * i + 2];
+  }
+  if (i < F) {
+    const int3 t = faces[i];
+    out_f[i] = make_int3((int)vscan[t.x] - 1, (int)vscan[t.y] - 1, (int)vscan[t.z] - 1);
+  }
+}
+
+// All scratch, sized once from V and F (n = 3F half-edges, at most n edges).
+struct Scratch {
+  Counters* ctr;
+  float* pos;
+  Quadric* Q;
+  uint8_t* lock;
+  int* to;
+  unsigned long long *m1, *m2;
+  uint32_t *used, *vscan;
+  uint2* vrange;
+  int3 *faces, *faces_alt;
+  uint8_t* alive;
+  unsigned long long *hkey_in, *hkey, *skey, *skey_sorted, *ekey;
+  uint32_t *hval_in, *hval, *ikey_in, *ikey, *ival_in, *vfaces, *heads, *edge_of;
+  Edge* edges;
+  float3* eplace;
+  void* temp;
+  size_t temp_bytes;
+
+  size_t carve(void* base, int V, int F, int vbits) {
+    const int n = 3 * F;
+    Carver cv(base);
+    ctr = cv.take<Counters>(1);
+    pos = cv.take<float>(3 * (size_t)V);
+    Q = cv.take<Quadric>(V);
+    lock = cv.take<uint8_t>(V);
+    to = cv.take<int>(V);
+    m1 = cv.take<unsigned long long>(V);
+    m2 = cv.take<unsigned long long>(V);
+    used = cv.take<uint32_t>(V);
+    vscan = cv.take<uint32_t>(V);
+    vrange = cv.take<uint2>(V);
+    faces = cv.take<int3>(F);
+    faces_alt = cv.take<int3>(F);
+    alive = cv.take<uint8_t>(F);
+    hkey_in = cv.take<unsigned long long>(n);
+    hkey = cv.take<unsigned long long>(n);
+    skey = cv.take<unsigned long long>(n);
+    skey_sorted = cv.take<unsigned long long>(n);
+    ekey = cv.take<unsigned long long>(n);
+    hval_in = cv.take<uint32_t>(n);
+    hval = cv.take<uint32_t>(n);
+    ikey_in = cv.take<uint32_t>(n);
+    ikey = cv.take<uint32_t>(n);
+    ival_in = cv.take<uint32_t>(n);
+    vfaces = cv.take<uint32_t>(n);
+    heads = cv.take<uint32_t>(n);
+    edge_of = cv.take<uint32_t>(n);
+    edges = cv.take<Edge>(n);
+    eplace = cv.take<float3>(n);
+    size_t t = 0;
+    temp_bytes = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, t, hkey_in, hkey, hval_in, hval, n, 0, 2 * vbits);
+    temp_bytes = std::max(temp_bytes, t);
+    cub::DeviceRadixSort::SortPairs(nullptr, t, ikey_in, ikey, ival_in, vfaces, n, 0, vbits);
+    temp_bytes = std::max(temp_bytes, t);
+    cub::DeviceRadixSort::SortKeys(nullptr, t, skey, skey_sorted, n);
+    temp_bytes = std::max(temp_bytes, t);
+    cub::DeviceScan::InclusiveSum(nullptr, t, heads, heads, std::max(n, V));
+    temp_bytes = std::max(temp_bytes, t);
+    cub::DeviceSelect::Flagged(nullptr, t, faces, alive, faces_alt, static_cast<int*>(nullptr), F);
+    temp_bytes = std::max(temp_bytes, t);
+    temp = cv.take<char>(temp_bytes);
+    return cv.bytes();
+  }
+};
+
+// The vertex -> face lists of the first F faces: vfaces[vrange[v].x, vrange[v].y) in face order.
+cudaError_t vertex_faces(Scratch& s, int F, int V, int vbits, cudaStream_t st) {
+  const int n = 3 * F;
+  incidence_kernel<<<ceil_div(n, kThreads), kThreads, 0, st>>>(n, s.faces, s.ikey_in, s.ival_in);
+  g_kernel_launches++;
+  cudaError_t e = cub::DeviceRadixSort::SortPairs(s.temp, s.temp_bytes, s.ikey_in, s.ikey, s.ival_in, s.vfaces, n, 0,
+                                                  vbits, st);
+  if (e != cudaSuccess) return e;
+  if ((e = cudaMemsetAsync(s.vrange, 0, (size_t)V * sizeof(uint2), st)) != cudaSuccess) return e;
+  ranges_kernel<<<ceil_div(n, kThreads), kThreads, 0, st>>>(n, s.ikey, s.vrange);
+  g_kernel_launches++;
+  return cudaGetLastError();
+}
+
+}  // namespace
+}  // namespace dgs
+
+using namespace dgs;
+
+extern "C" {
+
+int dgs_mesh_decimate(const float* vertices, long long num_vertices, const int* faces, long long num_faces,
+                      long long target_faces, dgs_alloc_fn alloc, void* alloc_user, float** out_vertices,
+                      int** out_faces, long long* out_num_vertices, long long* out_num_faces, int* rounds,
+                      void* stream) {
+  DGS_REQUIRE(alloc && out_vertices && out_faces && out_num_vertices && out_num_faces,
+              "mesh decimate: alloc and the four outputs must not be NULL");
+  DGS_REQUIRE(num_vertices >= 0 && num_faces >= 0, "mesh decimate: negative size (%lld vertices, %lld faces)",
+              num_vertices, num_faces);
+  DGS_REQUIRE(target_faces >= 0, "mesh decimate: target_faces must be >= 0 (got %lld)", target_faces);
+  DGS_REQUIRE(num_vertices <= 0x7fffffffLL && 3 * num_faces <= 0x7fffffffLL,
+              "mesh decimate: %lld vertices / %lld faces is too many (at most 2^31 - 1 vertices and half-edges)",
+              num_vertices, num_faces);
+  DGS_REQUIRE((num_vertices == 0 || vertices) && (num_faces == 0 || faces),
+              "mesh decimate: vertices and faces must not be NULL");
+  *out_vertices = nullptr;
+  *out_faces = nullptr;
+  *out_num_vertices = *out_num_faces = 0;
+  if (rounds) *rounds = 0;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int V = (int)num_vertices, F = (int)num_faces;
+  int vbits = 1;
+  while (vbits < 31 && (1LL << vbits) < num_vertices) vbits++;
+  const bool decimate = num_faces > target_faces;
+  Scratch s;
+  // the input is returned as it is when it is within the target: only the counters are needed to check it
+  const size_t bytes = decimate ? s.carve(nullptr, V, F, vbits) : sizeof(Counters);
+  void* buf = alloc(bytes, alloc_user);
+  if (!buf) { set_error("mesh decimate: scratch allocation failed (%zu bytes)", bytes); return DGS_ERR_ALLOC; }
+  if (decimate) s.carve(buf, V, F, vbits);
+  else s.ctr = reinterpret_cast<Counters*>(buf);
+  const int3* in_faces = reinterpret_cast<const int3*>(faces);
+  Counters h;
+  DGS_CUDA_OK(cudaMemsetAsync(s.ctr, 0xff, sizeof(Counters), st));
+  if (F > 0) {
+    validate_kernel<<<ceil_div(F, kThreads), kThreads, 0, st>>>(F, V, in_faces, s.ctr);
+    DGS_POST_LAUNCH();
+  }
+  if (decimate) {
+    DGS_CUDA_OK(cudaMemcpyAsync(s.pos, vertices, 3 * (size_t)V * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    DGS_CUDA_OK(cudaMemcpyAsync(s.faces, in_faces, (size_t)F * sizeof(int3), cudaMemcpyDeviceToDevice, st));
+  }
+  DGS_CUDA_OK(cudaMemcpyAsync(&h, s.ctr, sizeof(h), cudaMemcpyDeviceToHost, st));
+  DGS_CUDA_OK(cudaStreamSynchronize(st));  // indices must be valid before any kernel follows them
+  if (h.bad_face != kNoKey) {
+    const int3* bad = in_faces + h.bad_face;
+    int t[3] = {0, 0, 0};
+    DGS_CUDA_OK(cudaMemcpyAsync(t, bad, sizeof(t), cudaMemcpyDeviceToHost, st));
+    DGS_CUDA_OK(cudaStreamSynchronize(st));
+    set_error("mesh decimate: face %llu = (%d, %d, %d) has an index outside [0, %d) or a repeated index", h.bad_face,
+              t[0], t[1], t[2], V);
+    return DGS_ERR_INVALID_ARGUMENT;
+  }
+  if (!decimate) {
+    float* v = V ? reinterpret_cast<float*>(alloc(3 * (size_t)V * sizeof(float), alloc_user)) : nullptr;
+    int* f = F ? reinterpret_cast<int*>(alloc(3 * (size_t)F * sizeof(int), alloc_user)) : nullptr;
+    if ((V && !v) || (F && !f)) { set_error("mesh decimate: output allocation failed"); return DGS_ERR_ALLOC; }
+    if (V) DGS_CUDA_OK(cudaMemcpyAsync(v, vertices, 3 * (size_t)V * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    if (F) DGS_CUDA_OK(cudaMemcpyAsync(f, faces, 3 * (size_t)F * sizeof(int), cudaMemcpyDeviceToDevice, st));
+    *out_vertices = v;
+    *out_faces = f;
+    *out_num_vertices = V;
+    *out_num_faces = F;
+    return DGS_OK;
+  }
+
+  // setup: vertex quadrics over the vertex -> face lists (face order), no locks yet
+  DGS_CUDA_OK(vertex_faces(s, F, V, vbits, st));
+  vertex_quadric_kernel<<<ceil_div(V, kThreads), kThreads, 0, st>>>(V, s.pos, s.faces, s.vrange, s.vfaces, s.Q);
+  DGS_POST_LAUNCH();
+  DGS_CUDA_OK(cudaMemsetAsync(s.lock, 0, (size_t)V, st));
+
+  int live = F, applied_rounds = 0;
+  while (live > (long long)target_faces) {
+    const int n = 3 * live, gn = ceil_div(n, kThreads), gv = ceil_div(V, kThreads);
+    halfedge_kernel<<<gn, kThreads, 0, st>>>(n, s.faces, vbits, s.hkey_in, s.hval_in);
+    DGS_POST_LAUNCH();
+    DGS_CUDA_OK(cub::DeviceRadixSort::SortPairs(s.temp, s.temp_bytes, s.hkey_in, s.hkey, s.hval_in, s.hval, n, 0,
+                                                2 * vbits, st));
+    edge_heads_kernel<<<gn, kThreads, 0, st>>>(n, s.hkey, s.heads);
+    DGS_POST_LAUNCH();
+    DGS_CUDA_OK(cub::DeviceScan::InclusiveSum(s.temp, s.temp_bytes, s.heads, s.heads, n, st));
+    edge_build_kernel<<<gn, kThreads, 0, st>>>(n, s.hkey, s.hval, s.heads, s.faces, vbits, s.edges, s.edge_of, s.lock,
+                                               s.ctr);
+    DGS_POST_LAUNCH();
+    if (applied_rounds > 0) DGS_CUDA_OK(vertex_faces(s, live, V, vbits, st));  // setup built the first round's
+    cost_kernel<<<gn, kThreads, 0, st>>>(s.ctr, s.edges, s.pos, s.Q, s.lock, s.faces, s.vrange, s.vfaces, s.ekey,
+                                         s.eplace);
+    DGS_POST_LAUNCH();
+    m1_kernel<<<gv, kThreads, 0, st>>>(V, s.faces, s.vrange, s.vfaces, s.edge_of, s.ekey, s.m1);
+    DGS_POST_LAUNCH();
+    m2_kernel<<<gv, kThreads, 0, st>>>(V, s.faces, s.vrange, s.vfaces, s.m1, s.m2);
+    DGS_POST_LAUNCH();
+    DGS_CUDA_OK(cudaMemsetAsync(&s.ctr->num_selected, 0, sizeof(int), st));
+    select_kernel<<<gn, kThreads, 0, st>>>(s.ctr, s.edges, s.ekey, s.m2, s.skey);
+    DGS_POST_LAUNCH();
+    DGS_CUDA_OK(cudaMemcpyAsync(&h, s.ctr, sizeof(h), cudaMemcpyDeviceToHost, st));
+    DGS_CUDA_OK(cudaStreamSynchronize(st));  // the one read-back of the round: how many edges were taken
+    if (applied_rounds > 0 && h.num_faces != live) {
+      set_error("mesh decimate: internal error, %d live faces where %d were expected", h.num_faces, live);
+      return DGS_ERR_CUDA;
+    }
+    if (h.num_selected == 0) break;
+    // every collapse removes exactly the two faces of its edge; round up so that the result is target or target - 1
+    const int want = (int)((live - target_faces + 1) / 2), take = std::min(h.num_selected, want);
+    const unsigned long long* thr = nullptr;
+    if (take < h.num_selected) {
+      DGS_CUDA_OK(cub::DeviceRadixSort::SortKeys(s.temp, s.temp_bytes, s.skey, s.skey_sorted, h.num_edges, 0, 64, st));
+      thr = s.skey_sorted + (take - 1);
+    }
+    DGS_CUDA_OK(cudaMemsetAsync(s.to, 0xff, (size_t)V * sizeof(int), st));
+    apply_kernel<<<gn, kThreads, 0, st>>>(s.ctr, s.edges, s.skey, thr, s.eplace, s.pos, s.Q, s.to);
+    DGS_POST_LAUNCH();
+    remap_kernel<<<ceil_div(live, kThreads), kThreads, 0, st>>>(live, s.faces, s.to, s.alive);
+    DGS_POST_LAUNCH();
+    DGS_CUDA_OK(cub::DeviceSelect::Flagged(s.temp, s.temp_bytes, s.faces, s.alive, s.faces_alt, &s.ctr->num_faces, live,
+                                           st));
+    std::swap(s.faces, s.faces_alt);
+    live -= 2 * take;
+    applied_rounds++;
+  }
+
+  // finish: referenced vertices in index order, faces remapped
+  DGS_CUDA_OK(cudaMemsetAsync(s.used, 0, (size_t)V * sizeof(uint32_t), st));
+  if (live > 0) {
+    used_kernel<<<ceil_div(3 * live, kThreads), kThreads, 0, st>>>(3 * live, s.faces, s.used);
+    DGS_POST_LAUNCH();
+  }
+  DGS_CUDA_OK(cub::DeviceScan::InclusiveSum(s.temp, s.temp_bytes, s.used, s.vscan, V, st));
+  uint32_t nv = 0;
+  DGS_CUDA_OK(cudaMemcpyAsync(&nv, s.vscan + V - 1, sizeof(nv), cudaMemcpyDeviceToHost, st));
+  DGS_CUDA_OK(cudaMemcpyAsync(&h, s.ctr, sizeof(h), cudaMemcpyDeviceToHost, st));
+  DGS_CUDA_OK(cudaStreamSynchronize(st));  // the vertex count sizes the output
+  if (applied_rounds > 0 && h.num_faces != live) {
+    set_error("mesh decimate: internal error, %d live faces where %d were expected", h.num_faces, live);
+    return DGS_ERR_CUDA;
+  }
+  if (rounds) *rounds = applied_rounds;
+  if (nv == 0) return DGS_OK;
+  float* v = reinterpret_cast<float*>(alloc((size_t)nv * 3 * sizeof(float), alloc_user));
+  int* f = live ? reinterpret_cast<int*>(alloc((size_t)live * 3 * sizeof(int), alloc_user)) : nullptr;
+  if (!v || (live && !f)) { set_error("mesh decimate: output allocation failed"); return DGS_ERR_ALLOC; }
+  emit_kernel<<<ceil_div(std::max(V, live), kThreads), kThreads, 0, st>>>(V, live, s.pos, s.faces, s.used, s.vscan, v,
+                                                                           reinterpret_cast<int3*>(f));
+  DGS_POST_LAUNCH();
+  *out_vertices = v;
+  *out_faces = f;
+  *out_num_vertices = nv;
+  *out_num_faces = live;
+  return DGS_OK;
+}
+
+}  // extern "C"

@@ -207,6 +207,9 @@ def lib():
                                      vp, vp, vp, C.POINTER(C.c_longlong), ALLOC_FN, vp, vp]
         L.dgs_marching_cubes.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_float, ALLOC_FN, vp, C.POINTER(C.c_void_p),
                                          C.POINTER(C.c_void_p), C.POINTER(C.c_longlong), C.POINTER(C.c_longlong), vp]
+        L.dgs_mesh_decimate.argtypes = [vp, C.c_longlong, vp, C.c_longlong, C.c_longlong, ALLOC_FN, vp,
+                                        C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_longlong),
+                                        C.POINTER(C.c_longlong), C.POINTER(C.c_int), vp]
         _lib = L
     return _lib
 
@@ -247,4 +250,5 @@ EXPORTED = [  # every symbol include/dgs_b200.h declares (checked by tests/test_
     "dgs_dit_workspace_bytes_fp8", "dgs_dit_forward_fp8", "dgs_quantize_rows_e4m3", "dgs_ln_modulate_fp8", "dgs_gemm_fp8",
     "dgs_mesh_field", "dgs_marching_cubes", "dgs_render_batch_forward_aux", "dgs_render_batch_backward_aux",
     "dgs_dit_workspace_bytes_fp8_ex", "dgs_dit_forward_fp8_ex", "dgs_attention_quantize_e4m3", "dgs_attention_fwd_fp8",
+    "dgs_mesh_decimate",
 ]

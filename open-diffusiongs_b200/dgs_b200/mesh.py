@@ -1,10 +1,11 @@
-"""Mesh extraction on libdgs_b200.so (dgs_mesh_field / dgs_marching_cubes): the layer under
+"""Mesh extraction on libdgs_b200.so (dgs_mesh_field / dgs_marching_cubes / dgs_mesh_decimate): the layer under
 `GaussianModel.extract_fields` / `extract_mesh`, and a command line that meshes a saved Gaussian PLY.
 
-    python -m dgs_b200.mesh in.ply out.obj [--resolution 256] [--density-thresh 0.005]
+    python -m dgs_b200.mesh in.ply out.obj [--resolution 256] [--density-thresh 0.005] [--decimate-target N]
 
 reads a PLY written by `GaussianModel.save_ply` (or the reference's), extracts the mesh exactly as
-`extract_mesh(density_thresh, resolution)` does and writes it as OBJ or binary PLY, chosen by the suffix.
+`extract_mesh(density_thresh, resolution)` does and writes it as OBJ or binary PLY, chosen by the suffix; with
+`--decimate-target N` the mesh is first decimated to at most N faces (`decimate`, dgs_mesh_decimate).
 
 Marching cubes produces the same vertex set as PyMCubes (one vertex per sign-changing grid edge, at the linear
 interpolation of the iso value); on the ambiguous cases the triangulation may differ (a face with two diagonally
@@ -120,6 +121,57 @@ def marching_cubes(field, iso):
     return verts, faces
 
 
+def decimate(vertices, faces, target_faces):
+    """Quadric edge-collapse decimation to at most `target_faces` faces (dgs_mesh_decimate; the reference's
+    decimate_mesh with optimalplacement=True, boundary loops kept) -> (vertices, faces).  The signature of
+    extract_mesh's `postprocess`, so `extract_mesh(postprocess=decimate)` returns the reference's <= decimate_target
+    (1e5) face mesh.  numpy input (vertices float [V, 3], faces integer [F, 3]) runs on the current CUDA device and returns
+    numpy float32 [V', 3] / int64 [F', 3]; CUDA tensors return CUDA tensors of those dtypes on their device.  The
+    result has target_faces or target_faces - 1 faces unless no further edge can be collapsed; a mesh within the target
+    comes back unchanged."""
+    is_numpy = isinstance(vertices, np.ndarray) and isinstance(faces, np.ndarray)
+    if not is_numpy and not (isinstance(vertices, torch.Tensor) and isinstance(faces, torch.Tensor)
+                             and vertices.is_cuda and faces.is_cuda and vertices.device == faces.device):
+        raise TypeError("decimate: vertices and faces must both be numpy arrays or CUDA tensors on one device")
+    if vertices.ndim != 2 or vertices.shape[1] != 3 or faces.ndim != 2 or faces.shape[1] != 3:
+        raise ValueError(f"decimate: expected vertices [V, 3] and faces [F, 3], got {tuple(vertices.shape)} and "
+                         f"{tuple(faces.shape)}")
+    float_v = vertices.dtype.kind == "f" if is_numpy else vertices.dtype.is_floating_point
+    int_f = faces.dtype.kind in "iu" if is_numpy else not (faces.dtype.is_floating_point or faces.dtype.is_complex
+                                                             or faces.dtype == torch.bool)
+    if not float_v or not int_f:
+        raise TypeError(f"decimate: vertices must be floating point and faces integer (got {vertices.dtype}, "
+                        f"{faces.dtype})")
+    target = float(target_faces)
+    if not np.isfinite(target) or target < 0:
+        raise ValueError(f"decimate: target_faces must be a finite number >= 0 (got {target_faces!r})")
+    i32 = np.iinfo(np.int32)
+    if len(faces) and (int(faces.min()) < i32.min or int(faces.max()) > i32.max):
+        raise ValueError("decimate: face indices do not fit int32")
+    if is_numpy:
+        dev = torch.device("cuda", torch.cuda.current_device())
+        v = torch.from_numpy(np.ascontiguousarray(vertices, np.float32)).to(dev)
+        f = torch.from_numpy(np.ascontiguousarray(faces, np.int32)).to(dev)
+    else:
+        dev = vertices.device
+        v = vertices.detach().to(torch.float32).contiguous()
+        f = faces.detach().to(torch.int32).contiguous()
+    alloc = _Alloc(dev, "decimate", 1)
+    vp, fp = C.c_void_p(), C.c_void_p()
+    nv, nf, rounds = C.c_longlong(0), C.c_longlong(0), C.c_int(0)
+    with torch.cuda.device(dev):
+        check(_lib.lib().dgs_mesh_decimate(v.data_ptr(), len(v), f.data_ptr(), len(f), int(target), alloc.cb, None,
+                                           C.byref(vp), C.byref(fp), C.byref(nv), C.byref(nf), C.byref(rounds),
+                                           _stream(dev)))
+    V, F = nv.value, nf.value
+    ov = alloc.tensors[1][:V * 12].view(torch.float32).view(V, 3) if V else torch.zeros(0, 3, device=dev)
+    of = alloc.tensors[2][:F * 12].view(torch.int32).view(F, 3).long() if F else torch.zeros(0, 3, dtype=torch.int64,
+                                                                                              device=dev)
+    if is_numpy:
+        return ov.cpu().numpy(), of.cpu().numpy()
+    return ov, of
+
+
 class Mesh:
     """The triangle mesh extract_mesh returns: `vertices` float32 [V, 3] and `faces` int64 [F, 3] numpy arrays (the
     attribute names of trimesh.Trimesh)."""
@@ -163,17 +215,24 @@ def extract_mesh(field, density_thresh, resolution, postprocess=None, decimate_t
     return Mesh(vertices, faces)
 
 
-def main(argv=None):
+def parser():
     ap = argparse.ArgumentParser(description="Extract a mesh from a Gaussian PLY (GaussianModel.extract_mesh)")
     ap.add_argument("ply", help="Gaussians, as written by GaussianModel.save_ply")
     ap.add_argument("out", help="output mesh, .obj or .ply")
     ap.add_argument("--resolution", type=int, default=256, help="grid points per axis (default 256)")
     ap.add_argument("--density-thresh", type=float, default=0.005, help="iso value of the opacity field (default 0.005)")
-    args = ap.parse_args(argv)
+    ap.add_argument("--decimate-target", type=int, default=None, metavar="N",
+                    help="decimate to at most N faces (quadric edge collapse; default: the raw marching-cubes mesh)")
+    return ap
+
+
+def main(argv=None):
+    args = parser().parse_args(argv)
     from .renderer import GaussianModel
     gm = GaussianModel(0)
     gm.load_ply(args.ply)
-    mesh = gm.to("cuda").extract_mesh(density_thresh=args.density_thresh, resolution=args.resolution)
+    kw = {} if args.decimate_target is None else dict(postprocess=decimate, decimate_target=args.decimate_target)
+    mesh = gm.to("cuda").extract_mesh(density_thresh=args.density_thresh, resolution=args.resolution, **kw)
     mesh.export(args.out)
     print(f"{args.out}: {len(mesh.vertices)} vertices, {len(mesh.faces)} faces")
 
