@@ -1500,9 +1500,12 @@ __global__ void __launch_bounds__(256) geometry_backward_kernel(Problem pb, Geom
     dq[1] = 2 * y * (E[0][1] + E[1][0]) + 2 * z * (E[0][2] + E[2][0]) + 2 * r * (E[2][1] - E[1][2]) - 4 * x * (E[2][2] + E[1][1]);
     dq[2] = 2 * x * (E[0][1] + E[1][0]) + 2 * r * (E[0][2] - E[2][0]) + 2 * z * (E[2][1] + E[1][2]) - 4 * y * (E[2][2] + E[0][0]);
     dq[3] = 2 * r * (E[1][0] - E[0][1]) + 2 * x * (E[0][2] + E[2][0]) + 2 * y * (E[2][1] + E[1][2]) - 4 * z * (E[1][1] + E[0][0]);
+    // dsc is dL/d(mod * scale), the reference rasterizer's convention (backward.cu:295-325), which the activated
+    // (single-view) path returns as it is.  The raw (batched) path follows GaussianModel.get_scaling instead:
+    // S = exp(s_raw) * mod outside a rasterizer run with mod = 1, so d/ds_raw = d/dS * mod * exp(s_raw).
     if (pb.raw) {
-      // exp: d/ds_raw = d/dscale * scale ; normalize: (dq - q (q.dq)) / max(|q_raw|, eps)
-      dsc[0] *= scale.x; dsc[1] *= scale.y; dsc[2] *= scale.z;
+      // exp: d/ds_raw = d/d(mod scale) * mod * scale ; normalize: (dq - q (q.dq)) / max(|q_raw|, eps)
+      dsc[0] *= (double)pb.mod * scale.x; dsc[1] *= (double)pb.mod * scale.y; dsc[2] *= (double)pb.mod * scale.z;
       const double dot = r * dq[0] + x * dq[1] + y * dq[2] + z * dq[3];
       dq[0] = (dq[0] - r * dot) * inv_norm; dq[1] = (dq[1] - x * dot) * inv_norm;
       dq[2] = (dq[2] - y * dot) * inv_norm; dq[3] = (dq[3] - z * dot) * inv_norm;

@@ -52,27 +52,34 @@ class _Raster(torch.autograd.Function):
                 t(g["dL_drotations"]), None, None, None, None, None)
 
 
+def activated_scales(scaling, scaling_modifier=None):
+    """GaussianModel.get_scaling (gs_core.py:545-550): exp(scaling), times the model's scaling_modifier when it has one.
+    The rasterizer then runs with scale_modifier = 1, so autograd supplies the modifier's factor in d(scaling)."""
+    scales = torch.exp(scaling)                                   # gs_core.py:330,545-550
+    return scales if scaling_modifier is None else scales * float(scaling_modifier)
+
+
 def render_opencv_cam(xyz, features, scaling, rotation, opacity, H, W, C2W, fxfycxcy,
-                      bg=(1.0, 1.0, 1.0)):
+                      bg=(1.0, 1.0, 1.0), scaling_modifier=None):
     """gs_core.py:874-945 on raw (pre-activation) per-sample tensors; differentiable."""
     cam = build_camera(C2W, fxfycxcy, H, W)
     degree = int(round(features.shape[-2] ** 0.5)) - 1
-    scales = torch.exp(scaling)                                   # gs_core.py:330,545-550
+    scales = activated_scales(scaling, scaling_modifier)
     rots = torch.nn.functional.normalize(rotation)                # :332,553
     opac = torch.sigmoid(opacity)                                 # :333,569
     return _Raster.apply(xyz, features, opac, scales, rots, cam, H, W, degree, bg)
 
 
-def render_batch(xyz, features, scaling, rotation, opacity, H, W, C2W, fxfycxcy):
+def render_batch(xyz, features, scaling, rotation, opacity, H, W, C2W, fxfycxcy, scaling_modifier=None):
     """Renderer.forward + deferred_gaussian_render semantics (renderer.py:34-92,
     gs_core.py:949-1060): [b,P,*] raw params, C2W [b,v,4,4], fxfycxcy [b,v,4] -> [b,v,3,H,W] fp32.
     Differentiable w.r.t. the five parameter tensors (sums over views, like the reference's
-    accumulated .grad)."""
+    accumulated .grad).  `scaling_modifier`: the GaussianModel's (applied to the scales, see activated_scales)."""
     b, v = C2W.shape[0], C2W.shape[1]
     out = []
     for i in range(b):
         for j in range(v):
             out.append(render_opencv_cam(xyz[i].float(), features[i].float(), scaling[i].float(),
                                          rotation[i].float(), opacity[i].float(), H, W, C2W[i, j],
-                                         fxfycxcy[i, j]))
+                                         fxfycxcy[i, j], scaling_modifier=scaling_modifier))
     return torch.stack(out, 0).reshape(b, v, 3, H, W)

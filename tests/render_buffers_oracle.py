@@ -8,7 +8,7 @@ import numpy as np
 import torch
 
 from oracle import raster as _r
-from oracle.renderer import build_camera, render_opencv_cam
+from oracle.renderer import activated_scales, build_camera, render_opencv_cam
 
 
 class _AuxRaster(torch.autograd.Function):
@@ -39,18 +39,19 @@ class _AuxRaster(torch.autograd.Function):
         return t(dmeans), t(g["dL_dopacity"]), t(g["dL_dscales"]), t(g["dL_drotations"]), None, None, None
 
 
-def render_batch_buffers(xyz, features, scaling, rotation, opacity, H, W, C2W, fxfycxcy):
+def render_batch_buffers(xyz, features, scaling, rotation, opacity, H, W, C2W, fxfycxcy, scaling_modifier=None):
     """oracle.renderer.render_batch plus per-pixel depth and alpha, the buffers of the reference's planned
     edict(render=..., depth=..., alpha=...): -> (render [b,v,3,H,W], depth [b,v,1,H,W], alpha [b,v,1,H,W]) from one colour
-    call and one aux call per (sample, view); differentiable w.r.t. the five raw tensors."""
+    call and one aux call per (sample, view); differentiable w.r.t. the five raw tensors.  `scaling_modifier` is applied
+    as oracle.renderer.render_batch applies it."""
     b, v = C2W.shape[0], C2W.shape[1]
     render, aux = [], []
     for i in range(b):
         raw = [t[i].float() for t in (xyz, features, scaling, rotation, opacity)]
         for j in range(v):
-            render.append(render_opencv_cam(*raw, H, W, C2W[i, j], fxfycxcy[i, j]))
+            render.append(render_opencv_cam(*raw, H, W, C2W[i, j], fxfycxcy[i, j], scaling_modifier=scaling_modifier))
             cam = build_camera(C2W[i, j], fxfycxcy[i, j], H, W)
-            aux.append(_AuxRaster.apply(raw[0], torch.sigmoid(raw[4]), torch.exp(raw[2]),
+            aux.append(_AuxRaster.apply(raw[0], torch.sigmoid(raw[4]), activated_scales(raw[2], scaling_modifier),
                                         torch.nn.functional.normalize(raw[3]), cam, H, W))
     aux = torch.stack(aux, 0).reshape(b, v, 2, H, W)
     return torch.stack(render, 0).reshape(b, v, 3, H, W), aux[:, :, :1], aux[:, :, 1:]
