@@ -9,7 +9,10 @@
 // current one.  Tile = 128 x BN (BN = 256 or 128),
 // wgmma m64nBNk16, one k-block group kept in flight while the next is issued.  The inference epilogues stage the
 // finished tile in shared memory and hand it to the TMA unit (a store, or for the in-place residual update a reduce-add
-// in L2), so the consumers go on to the next tile's mainloop while the tile is written out.
+// in L2), so the consumers go on to the next tile's mainloop while the tile is written out.  The two consumer
+// warpgroups run their epilogues at the same time, so the tensor cores idle for as long as an epilogue takes: it loads
+// the bias and gate values of eight column groups at once before using them, rather than waiting for each load in turn
+// (one memory latency per column pair cost qkv and mlp.fc1 a fifth of their time at 4098 tokens).
 //
 // Operand modes (GemmOp): bf16 K-major (the forward and dgrad GEMMs), bf16 MN-major (the weight gradients, gemm_bf16_tn)
 // and e4m3 (the FP8 inference path, gemm_fp8).  The e4m3 mode is the K-major kernel at BN = 128 with a k-block of 128
@@ -83,9 +86,10 @@ enum GemmOp { OP_BF16_K = 0, OP_BF16_MN = 1, OP_E4M3 = 2 };
 
 // OUT_BYTES: element size of the output tile staged in shared memory for the TMA-store epilogue (0: the epilogue
 // writes from registers).  The staging buffer takes what would otherwise be operand stages.  It holds RING column
-// blocks (128 bytes x 64 rows, 8 KB) per consumer warpgroup: the whole 64 x BN fragment, except for a 128 x 256 fp32
-// tile (128 KB staged whole, which would leave two operand stages), which goes out two column blocks at a time and
-// keeps four stages.  SCALE_BYTES: the row scales a stage carries besides its operands (e4m3: BM fp32, else 0).
+// blocks (128 bytes x 64 rows, 8 KB) per consumer warpgroup: the whole 64 x BN fragment of a 128 x 128 tile, and two
+// column blocks at a time of a 128 x 256 tile (staged whole, a bf16 tile would leave three operand stages and an fp32
+// tile two), which keeps four stages.  SCALE_BYTES: the row scales a stage carries besides its operands (e4m3: BM fp32,
+// else 0).
 template <int BN, int OUT_BYTES, int SCALE_BYTES>
 struct GemmCfg {
   static constexpr int SMEM_LIMIT = 227 * 1024;
@@ -94,7 +98,7 @@ struct GemmCfg {
   static constexpr int B_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int OUT_BLOCKS = BN * OUT_BYTES / 128;  // column blocks of a warpgroup's fragment
-  static constexpr int RING = OUT_BLOCKS > 4 ? 2 : OUT_BLOCKS;
+  static constexpr int RING = BN == 256 && OUT_BLOCKS > 2 ? 2 : OUT_BLOCKS;
   static constexpr int OUT_TILE_BYTES = 2 * RING * 8192;
   static constexpr int EXTRA = 1024 /*align slack*/ + 256 /*barriers*/;
   static constexpr int FIT = (SMEM_LIMIT - EXTRA - OUT_TILE_BYTES) / (STAGE_BYTES + S_BYTES);
@@ -103,8 +107,9 @@ struct GemmCfg {
   static_assert(STAGES >= 3 && SMEM_BYTES <= SMEM_LIMIT, "GEMM configuration does not fit in shared memory");
   static_assert(S_BYTES % 16 == 0, "the row scales are one bulk copy per stage: 16-byte multiples");
 };
-static_assert(GemmCfg<256, 4, 0>::RING == 2 && GemmCfg<256, 4, 0>::STAGES == 4,
-              "the in-place gate + residual update on 128 x 256 tiles keeps four operand stages");
+static_assert(GemmCfg<256, 4, 0>::RING == 2 && GemmCfg<256, 4, 0>::STAGES == 4 && GemmCfg<256, 2, 0>::RING == 2 &&
+                  GemmCfg<256, 2, 0>::STAGES == 4,
+              "the bf16 stores and the in-place gate + residual update on 128 x 256 tiles keep four operand stages");
 static_assert(GemmCfg<128, 1, BM * 4>::STAGES == 6 && GemmCfg<128, 4, BM * 4>::STAGES == 4,
               "FP8 stage counts: 6 for fc1 (e4m3 out), 4 for fc2 (in-place fp32)");
 
@@ -138,6 +143,14 @@ __device__ __forceinline__ float epi_dgelu_tanh(float x) {  // d/dx of the above
   return 0.5f * (1.0f + t) + 0.5f * x * (1.0f - t * t) * du;
 }
 
+// The GELU or ReLU of the epilogues that have one.
+template <int EPI>
+__device__ __forceinline__ float2 epi_act(float2 v) {
+  if (EPI == EPI_BIAS_GELU_BF16 || EPI == EPI_BIAS_GELU_E4M3) { v.x = epi_gelu_tanh(v.x); v.y = epi_gelu_tanh(v.y); }
+  if (EPI == EPI_BIAS_RELU_BF16) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); }
+  return v;
+}
+
 // The per-element part every epilogue shares, on one thread's column pair (n, n+1) of output row offset ro: acc + b
 // (with keep_pre, training mode, also stored to ep.aux as bf16), then the GELU or ReLU of the epilogues that have one.
 template <int EPI>
@@ -148,9 +161,7 @@ __device__ __forceinline__ float2 epi_bias_act(const GemmEpilogue& ep, float2 v,
     v.x += b.x; v.y += b.y;
   }
   if (keep_pre) *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(ep.aux) + ro + n) = pack2_bf16(v.x, v.y);
-  if (EPI == EPI_BIAS_GELU_BF16 || EPI == EPI_BIAS_GELU_E4M3) { v.x = epi_gelu_tanh(v.x); v.y = epi_gelu_tanh(v.y); }
-  if (EPI == EPI_BIAS_RELU_BF16) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); }
-  return v;
+  return epi_act<EPI>(v);
 }
 
 template <int BN, bool MN>
@@ -220,7 +231,10 @@ __device__ __forceinline__ void epilogue_tma(const GemmEpilogue& ep, const Fp8Sc
   constexpr int COLS = 128 / OB;            // columns per staging row
   constexpr int JB = RING * COLS / 8;       // 8-column groups per batch
   constexpr bool WHOLE = EPI == EPI_BIAS_GELU_E4M3;  // gemm_fp8 checks N % 128 == 0: the tile has no columns >= N
+  constexpr int PJ = JB < 8 ? JB : 8;       // 8-column groups whose bias and gate are loaded ahead at once
+  static_assert(JB % PJ == 0, "whole load groups per batch");
   const bool leader = wq == 0 && lane == 0;
+  float2 bias_v[PJ], gate_v[PJ];
   const float* gate_row[2] = {nullptr, nullptr};
   if (EPI == EPI_GATE_RESID_F32) {
 #pragma unroll
@@ -256,18 +270,26 @@ __device__ __forceinline__ void epilogue_tma(const GemmEpilogue& ep, const Fp8Sc
       }
 #pragma unroll
       for (int j = j0; j < j0 + JB; j++) {
-        const int n = n0 + 8 * j + 2 * (lane & 3);
-        if (!WHOLE && n0 + 8 * j >= N) break;  // N % 32 == 0: whole 8-column groups are in or out
+        // The bias and gate column pairs of the next PJ groups are loaded together before the first is used, so that
+        // the fragment waits for one memory latency per PJ groups rather than one per group.  Columns >= N (only in
+        // the last tile column when N % BN != 0) read the pair N - 2 instead: they are staged, and clipped by the store.
+        const int jp = (j - j0) % PJ;
+        if (!WHOLE && jp == 0) {
+#pragma unroll
+          for (int q = 0; q < PJ; q++) {
+            const int n = min(n0 + 8 * (j + q) + 2 * (lane & 3), N - 2);
+            if (ep.bias) bias_v[q] = __ldg(reinterpret_cast<const float2*>(ep.bias + n));
+            if (EPI == EPI_GATE_RESID_F32) gate_v[q] = __ldg(reinterpret_cast<const float2*>(gate_row[i] + n));
+          }
+        }
         float2 v = make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
         if constexpr (EPI == EPI_BIAS_GELU_E4M3) {
           v.x *= inv; v.y *= inv;
         } else {
-          v = epi_bias_act<EPI>(ep, v, n);
+          if (ep.bias) { v.x += bias_v[jp].x; v.y += bias_v[jp].y; }
+          v = epi_act<EPI>(v);
         }
-        if (EPI == EPI_GATE_RESID_F32) {
-          const float2 g = __ldg(reinterpret_cast<const float2*>(gate_row[i] + n));
-          v.x *= g.x; v.y *= g.y;
-        }
+        if (EPI == EPI_GATE_RESID_F32) { v.x *= gate_v[jp].x; v.y *= gate_v[jp].y; }
         const int byte = ((8 * j) % COLS + 2 * (lane & 3)) * OB;  // within the 128-byte staging row
         uint8_t* p = stage + (8 * j / COLS % RING) * 8192 + r * 128 + ((((byte >> 4) ^ (lane >> 2)) << 4) | (byte & 15));
         if (OB == 1) *reinterpret_cast<uint16_t*>(p) = pack2_e4m3(v.x, v.y);
@@ -507,6 +529,8 @@ int gemm_bf16(const void* A, const void* W, int M, int N, int K, int epi, const 
               "gemm: operand row strides must be multiples of 8 elements (K=%d lda=%d ldb=%d)", K, ep.lda, ep.ldb);
   DGS_REQUIRE(epi != EPI_DGELU_BF16 || ep.aux, "gemm: EPI_DGELU_BF16 needs aux = saved pre-activation");
   DGS_REQUIRE(((uintptr_t)A % 16) == 0 && ((uintptr_t)W % 16) == 0, "gemm: operands must be 16-byte aligned");
+  // every thread stores column pairs (n, n + 1) of a row, n even: the pairs of every row are aligned when ldc is even
+  DGS_REQUIRE(ep.ldc % 2 == 0, "gemm: the output row stride must be even (got ldc=%d)", ep.ldc);
   const int sms = num_sms();
   DGS_REQUIRE(sms > 0, "gemm: cannot query the device's SM count");
   // The epilogue stages the tile in shared memory for a TMA store (or, in place, a TMA reduce-add) when the output rows
