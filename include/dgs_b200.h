@@ -236,11 +236,15 @@ typedef struct {
   const void* proj_w; const float* proj_b;  /* transformer.{i}.attn.proj  bf16 [L,w,w],  fp32 [L,w]  */
   const void* fc1_w;  const float* fc1_b;   /* transformer.{i}.mlp.fc1    bf16 [L,4w,w], fp32 [L,4w] */
   const void* fc2_w;  const float* fc2_b;   /* transformer.{i}.mlp.fc2    bf16 [L,w,4w], fp32 [L,w]  */
-  const float* ups_ln_w; const void* ups_w; /* upsampler.layernorm.weight fp32 [w]; upsampler.linear.weight split-bf16 [14,3w] */
-  const float* dec_ln_w; const void* dec_w; /* image_token_decoder.*: fp32 [w]; split-bf16 [patch*patch*14, 3w]
+  const float* ups_ln_w; const void* ups_w; /* upsampler.layernorm.weight fp32 [w]; upsampler.linear.weight split-bf16 [C,3w] */
+  const float* dec_ln_w; const void* dec_w; /* image_token_decoder.*: fp32 [w]; split-bf16 [patch*patch*C, 3w]
      "split-bf16 [n, 3k] = [hi|hi|lo]": hi = bf16(W), lo = bf16(W - hi); paired with activations laid out
      [hi|lo|hi] the bf16 MMA then yields x_hi W_hi + x_lo W_hi + x_hi W_lo (fp32-accurate) -- used for the two
      small GEMMs at the ends of the network whose rounding would otherwise dominate the output error. */
+  int sh_degree;            /* gaussians_sh_degree, 0..3 (0 in a zero-initialised struct).  Each head predicts
+                               C = 11 + 3 (sh_degree+1)^2 channels per Gaussian (14, 23, 38, 59), split
+                               [xyz 3 | features 3 (sh_degree+1)^2 | scaling 3 | rotation 4 | opacity 1]; feature (k, c)
+                               is channel 3 + 3k + c.  patch*patch*C must be a multiple of 32. */
 } dgs_dit_weights;
 
 typedef struct {
@@ -254,7 +258,7 @@ typedef struct {
   const float* ray_d;        /* [B,V,3,H,W]                                                           */
   const float* t;            /* [B] timesteps as fp32                                                 */
   float* xyz;                /* out [B,P,3],  P = n_gaussians + V*H*W                                 */
-  float* features;           /* out [B,P,1,3]                                                         */
+  float* features;           /* out [B,P,(sh_degree+1)^2,3]                                           */
   float* scaling;            /* out [B,P,3]                                                           */
   float* rotation;           /* out [B,P,4]                                                           */
   float* opacity;            /* out [B,P,1]                                                           */
@@ -343,8 +347,8 @@ typedef struct {
   const void* proj_wT;  /* bf16 [L, w, w]    */
   const void* fc1_wT;   /* bf16 [L, w, 4w]   */
   const void* fc2_wT;   /* bf16 [L, 4w, w]   */
-  const void* dec_wT;   /* bf16 [w, patch*patch*14]  (image_token_decoder.linear.weight^T)             */
-  const float* ups_w;   /* fp32 [14, w]      (upsampler.linear.weight, master copy)                    */
+  const void* dec_wT;   /* bf16 [w, patch*patch*C]  (image_token_decoder.linear.weight^T; C: see sh_degree) */
+  const float* ups_w;   /* fp32 [C, w]      (upsampler.linear.weight, master copy)                     */
 } dgs_dit_weights_t;
 
 typedef struct {  /* all fp32, OVERWRITTEN by dgs_dit_backward */
@@ -358,15 +362,15 @@ typedef struct {  /* all fp32, OVERWRITTEN by dgs_dit_backward */
   long long layer_stride;
   float* qkv_w; float* qkv_b; float* proj_w; float* proj_b; float* fc1_w; float* fc1_b; float* fc2_w; float* fc2_b;
   float* adaln_w; float* adaln_b;          /* block 0: [6w, w], [6w] */
-  float* ups_ln_w; float* ups_w;           /* [w], [14, w]               */
+  float* ups_ln_w; float* ups_w;           /* [w], [C, w]                */
   float* ups_adaln_w; float* ups_adaln_b;  /* [2w, w], [2w]              */
-  float* dec_ln_w; float* dec_w;           /* [w], [patch*patch*14, w]   */
+  float* dec_ln_w; float* dec_w;           /* [w], [patch*patch*C, w]    */
   float* dec_adaln_w; float* dec_adaln_b;  /* [2w, w], [2w]              */
 } dgs_dit_grads;
 
 typedef struct {  /* gradients w.r.t. the outputs of dgs_dit_forward (what dgs_render_batch_backward returns) */
   const float* d_xyz; const float* d_features; const float* d_scaling; const float* d_rotation; const float* d_opacity;
-} dgs_dit_out_grads;
+} dgs_dit_out_grads;  /* shapes of the dgs_dit_io outputs: d_features [B,P,(sh_degree+1)^2,3] */
 
 size_t dgs_dit_train_state_bytes(const dgs_dit_weights* w, int B, int V, int H, int W); /* DGS_TRAIN_STORE */
 size_t dgs_dit_train_state_bytes_ex(const dgs_dit_weights* w, int B, int V, int H, int W, int train_mode);
@@ -427,13 +431,14 @@ int dgs_dit_export_state(const dgs_dit_weights* w, int B, int V, int H, int W, i
  *   x_pre [M, width]: the assembled tokens [pos embedding | tokenizer output] before the input LayerNorm;
  *   c [B, width]: the conditioning t_embedder(t), before the adaLN SiLU;
  *   mod [B, layers*6*width + 4*width]: the adaLN table (block l at l*6*width; upsampler then decoder shift | scale);
- *   gs_tok [B*G, 14] and img_gs [B*T, patch*patch*14]: the raw head outputs, before the Gaussian epilogue.
+ *   gs_tok [B*G, C] and img_gs [B*T, patch*patch*C]: the raw head outputs, before the Gaussian epilogue (C =
+ *   11 + 3 (sh_degree+1)^2, see dgs_dit_weights).
  * Left by dgs_dit_backward(_ex) on the same train state and workspace (undefined before a backward):
  *   dx0 [M, width]: the gradient of the residual stream entering block 0 (the input LayerNorm's output);
  *   dx_pre [M, width]: the gradient of x_pre;
  *   dmod [B, layers*6*width + 4*width]: the gradient of the adaLN table;
  *   dc [B, width]: the gradient of c (after the SiLU backward);
- *   d_gs_tok [B*G, 14]: the gradient of gs_tok.
+ *   d_gs_tok [B*G, C]: the gradient of gs_tok.
  * A NULL train state, a bad mode or a workspace smaller than dgs_dit_workspace_bytes is DGS_ERR_INVALID_ARGUMENT. */
 int dgs_dit_export_ends(const dgs_dit_weights* w, int B, int V, int H, int W, int train_mode, const void* train_state,
                         const void* workspace, size_t workspace_bytes, float* x_pre, float* c, float* mod, float* gs_tok,
@@ -491,6 +496,19 @@ int dgs_gate_bwd(const float* dx, const void* y, const float* gate, int gate_str
 /* h = (LN(x; eps) [* ln_w]) * (1 + scale[b]) + shift[b] -> bf16 ; x fp32 [B, rows, width] */
 int dgs_ln_modulate(const float* x, const float* ln_w, const float* shift, const float* scale, int mod_stride,
                     void* h, int B, int rows, int width, float eps, void* stream);
+/* The Gaussian heads' epilogue (to_gs + pixel alignment) and its backward, the kernels dgs_dit_forward /
+ * dgs_dit_backward launch: the raw head outputs gs_tok [B*G, C] and img_gs [B*T, patch*patch*C] fp32 (C = 11 +
+ * 3 (sh_degree+1)^2; image rows in (v, hh, ww, ph, pw) order), rays [B,V,3,H,W] -> the outputs of dgs_dit_io
+ * (img_aligned_xyz may be NULL); scene_depth, near_, far_ as in dgs_dit_io.  The backward turns the gradients of those
+ * outputs into d_gs_tok [B*G, C] fp32 and d_img_gs [B*T, patch*patch*C] bf16. */
+int dgs_gaussians_epilogue(const float* gs_tok, const float* img_gs, const float* ray_o, const float* ray_d, float* xyz,
+                           float* features, float* scaling, float* rotation, float* opacity, float* img_aligned_xyz,
+                           int B, int G, int V, int H, int W, int patch, int sh_degree, int scene_depth, float near_,
+                           float far_, void* stream);
+int dgs_gaussians_epilogue_bwd(const float* gs_tok, const float* img_gs, const float* ray_d, const float* d_xyz,
+                               const float* d_features, const float* d_scaling, const float* d_rotation,
+                               const float* d_opacity, float* d_gs_tok, void* d_img_gs, int B, int G, int V, int H,
+                               int W, int patch, int sh_degree, int scene_depth, float near_, float far_, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * B2b. LPIPS-VGG perceptual distance, the lpips term of LossComputer (diffusionGS/utils/losses.py:243-309, which calls

@@ -1,6 +1,8 @@
 // dit_api.cu -- C ABI of the DiT denoiser forward (include/dgs_b200.h, section B2): orchestrates the
 // wgmma GEMMs, the wgmma attention and the glue kernels into DGSDenoiser.image_to_gaussians
 // (diffusionGS/models/denoiser/denoiser.py:306-416).
+#include <algorithm>
+
 #include "dgs_internal.h"
 #include "dit_kernels.h"
 
@@ -8,20 +10,26 @@ using namespace dgs;
 
 namespace {
 
+// Channels per Gaussian of both heads (denoiser.py:94-98, 145-149): xyz 3, SH features 3 (d+1)^2, scaling 3, rotation 4,
+// opacity 1.
+int head_channels(int sh_degree) { return 11 + 3 * (sh_degree + 1) * (sh_degree + 1); }
+
 // The shapes of one DiT call, from the weights' config and the input size B x V x H x W: T image tokens and G free
 // Gaussian tokens per sample, N = T + G, M = B*N rows, Mt = B*T image-token rows; Mp / Mtp round them up to 64.
 struct DitDims {
   int B, T, G, N, M, Mp, Mt, Mtp;
   int D, U;          // width, mlp_hidden
   int heads;
-  int Kin, Ndec;     // patch*patch*9 tokenizer inputs, patch*patch*14 decoder outputs per token
+  int C;             // raw head channels per Gaussian, 11 + 3 (sh_degree+1)^2
+  int Kin, Ndec;     // patch*patch*9 tokenizer inputs, patch*patch*C decoder outputs per token
   int mod_stride;    // L*6w + 4w: the adaLN modulation of every block and of both heads, per sample
   size_t MD, MU;     // elements of an [M, w] and an [M, mlp_hidden] tensor
   size_t lse_n;      // floats of one block's attention log-sum-exp, [B, heads, attention_lse_stride(N)]
   DitDims(const dgs_dit_weights* w, int B_, int V, int H, int W)
       : B(B_), T(V * (H / w->patch) * (W / w->patch)), G(w->n_gaussians), N(T + G), M(B * N), Mp((M + 63) / 64 * 64),
-        Mt(B * T), Mtp((Mt + 63) / 64 * 64), D(w->width), U(w->mlp_hidden), Kin(w->patch * w->patch * 9),
-        Ndec(w->patch * w->patch * 14), heads(w->heads), mod_stride(w->layers * 6 * D + 4 * D), MD((size_t)M * D), MU((size_t)M * U),
+        Mt(B * T), Mtp((Mt + 63) / 64 * 64), D(w->width), U(w->mlp_hidden), C(head_channels(w->sh_degree)),
+        Kin(w->patch * w->patch * 9), Ndec(w->patch * w->patch * C), heads(w->heads),
+        mod_stride(w->layers * 6 * D + 4 * D), MD((size_t)M * D), MU((size_t)M * U),
         lse_n((size_t)B * w->heads * attention_lse_stride(N)) {}
 };
 
@@ -38,8 +46,8 @@ struct DitWorkspace {
   float* c;               // [B, w]
   float* mod;             // [B, L*6w + 4w]
   __nv_bfloat16* hg;      // [B*G, 3w] split-bf16
-  float* gs_tok;          // [B*G, 14]
-  float* img_gs;          // [B*T, p*p*14]
+  float* gs_tok;          // [B*G, C]
+  float* img_gs;          // [B*T, p*p*C]
   // FP8 inference only, carved after the bf16 workspace: the activation scales of the e4m3 copies of h (LN outputs,
   // [w/128][Ms]) and u (GELU output, [4w/128][Ms]); the e4m3 activations themselves live in h / u.
   float* sa_h;
@@ -64,7 +72,7 @@ struct DitWorkspace {
     c = c_.take<float>((size_t)d.B * d.D);
     mod = c_.take<float>((size_t)d.B * d.mod_stride);
     hg = c_.take<__nv_bfloat16>((size_t)d.B * d.G * 3 * d.D);
-    gs_tok = c_.take<float>((size_t)d.B * d.G * 14);
+    gs_tok = c_.take<float>((size_t)d.B * d.G * d.C);
     img_gs = c_.take<float>((size_t)d.Mt * d.Ndec);
     bytes = c_.bytes();
     const size_t Ms = (size_t)fp8_scale_stride(d.M);
@@ -109,17 +117,17 @@ struct TrainState {
   float* dcond;             // [3][B, w]   dsilu(c) / dtemb1 / pre1
   float* ln_stats;          // [M, 2]      (mean, rstd) of the LayerNorm being differentiated
   float* skb_part;          // per-CTA partial sums of the adaLN / timestep-MLP input gradients (skinny_linear_bwd)
-  float* d_gs_tok;          // [B*G, 14]
+  float* d_gs_tok;          // [B*G, C]
   __nv_bfloat16* dyb;       // [M, w]      gated branch gradient / generic [M, w] bf16
   __nv_bfloat16* dh;        // [M, w]
-  __nv_bfloat16* big0;      // [M, 4w]     du / dqkv / d_img_gs
+  __nv_bfloat16* big0;      // [M, max(4w, 3w, Ndec)]  du / dqkv / d_img_gs [Mt, Ndec]
   __nv_bfloat16* bigT0;     // [w, Mp]     transposed token gradient (tokenizer weight gradient only)
   __nv_bfloat16* bigT1;     // [w, Mp]     transposed patches        (tokenizer weight gradient only)
   size_t bytes;
   TrainState(void* base, const dgs_dit_weights* w, const DitDims& d, int mode) {
     const size_t Lx = w->layers, L = mode == DGS_TRAIN_RECOMPUTE ? 1 : Lx;  // slots of the per-layer tensors
     const size_t MD = d.MD, MU = d.MU, D = d.D;
-    const size_t wide = d.U > 3 * d.D ? d.U : 3 * d.D;
+    const size_t wide = std::max({d.U, 3 * d.D, d.Ndec});
     Carver c(base);
     x_pre = c.take<float>(MD);
     x_all = c.take<float>((Lx + 1) * MD);
@@ -141,7 +149,7 @@ struct TrainState {
     dcond = c.take<float>((size_t)3 * d.B * D);
     ln_stats = c.take<float>(2 * (size_t)d.M);
     skb_part = c.take<float>(skinny_linear_bwd_part_floats(d.B, 6 * d.D, d.D));  // the widest: a block's 6w rows
-    d_gs_tok = c.take<float>((size_t)d.B * d.G * 14 + 16);
+    d_gs_tok = c.take<float>((size_t)d.B * d.G * d.C + 16);
     dyb = c.take<__nv_bfloat16>(MD);
     dh = c.take<__nv_bfloat16>(MD);
     big0 = c.take<__nv_bfloat16>((size_t)d.M * wide);
@@ -156,7 +164,12 @@ int check_dit(const dgs_dit_weights* w, int B, int V, int H, int W) {
   DGS_REQUIRE(w->width == 1024 && w->heads * 64 == w->width, "unsupported width/heads %d/%d (1024/16 only)", w->width, w->heads);
   DGS_REQUIRE(w->layers > 0 && w->patch > 0 && w->n_gaussians >= 0 && w->mlp_hidden % 256 == 0, "bad DiT config");
   DGS_REQUIRE(B > 0 && V > 0 && H % w->patch == 0 && W % w->patch == 0, "bad input shape B=%d V=%d H=%d W=%d", B, V, H, W);
-  DGS_REQUIRE((w->patch * w->patch * 14) % 32 == 0 && (w->patch * w->patch * 9) % 8 == 0, "patch %d unsupported", w->patch);
+  DGS_REQUIRE(w->sh_degree >= 0 && w->sh_degree <= 3, "sh_degree %d unsupported (0..3, as the rasterizer evaluates)",
+              w->sh_degree);
+  DGS_REQUIRE((w->patch * w->patch * 9) % 8 == 0, "patch %d unsupported", w->patch);
+  DGS_REQUIRE((w->patch * w->patch * head_channels(w->sh_degree)) % 32 == 0,
+              "patch %d with sh_degree %d: the decoder head's patch^2 * %d outputs per token must be a multiple of 32 "
+              "(the GEMM's N %% 32 rule)", w->patch, w->sh_degree, head_channels(w->sh_degree));
   DGS_REQUIRE(w->mlp_hidden >= 3 * w->width, "mlp_hidden must be >= 3*width (decoder head re-uses that buffer)");
   return DGS_OK;
 }
@@ -345,7 +358,7 @@ int dit_forward(const dgs_dit_weights* w, const dgs_dit_weights_fp8* w8, int fp8
   const float* md = mu + 2 * D;                  // image_token_decoder: shift | scale
   if (G > 0) {
     DGS_TRY(ln_forward(LN_SPLIT_BF16, x_fin, w->ups_ln_w, mu, mu + D, mod_stride, ws.hg, nullptr, B, N, 0, G, D, 1e-5f, st));
-    DGS_TRY(tiny_linear_bf16(ws.hg, (const __nv_bfloat16*)w->ups_w, ws.gs_tok, B * G, 14, 3 * D, st));
+    DGS_TRY(tiny_linear_bf16(ws.hg, (const __nv_bfloat16*)w->ups_w, ws.gs_tok, B * G, d.C, 3 * D, st));
   }
   // the decoder head runs split-bf16 (K = 3*width) so the Gaussian parameters are fp32-accurate functions of the
   // residual stream; its A operand re-uses the (now free) MLP hidden buffer
@@ -360,7 +373,7 @@ int dit_forward(const dgs_dit_weights* w, const dgs_dit_weights_fp8* w8, int fp8
   go.xyz = io->xyz; go.features = io->features; go.scaling = io->scaling; go.rotation = io->rotation;
   go.opacity = io->opacity; go.img_aligned_xyz = io->img_aligned_xyz;
   DGS_TRY(gaussians_epilogue(ws.gs_tok, ws.img_gs, io->ray_o, io->ray_d, go, B, G, io->V, io->H, io->W, p,
-                             io->scene_depth, io->range_near, io->range_far, st));
+                             w->sh_degree, io->scene_depth, io->range_near, io->range_far, st));
   return DGS_OK;
 }
 
@@ -402,14 +415,14 @@ int heads_backward(const dgs_dit_weights* w, const dgs_dit_weights_t* wT, const 
   __nv_bfloat16* d_img = ts.big0;  // [Mt, Ndec]
   DGS_TRY(gaussians_epilogue_bwd(ws.gs_tok, ws.img_gs, io->ray_d, dout->d_xyz, dout->d_features, dout->d_scaling,
                                  dout->d_rotation, dout->d_opacity, ts.d_gs_tok, d_img, B, G, io->V, io->H, io->W,
-                                 w->patch, io->scene_depth, io->range_near, io->range_far, st));
+                                 w->patch, w->sh_degree, io->scene_depth, io->range_near, io->range_far, st));
   // image_token_decoder: dh = d_img W, dW = d_img^T h
   DGS_TRY(dgrad(d_img, wT->dec_wT, ts.dh, d.Mt, D, d.Ndec, EPI_BIAS_BF16, nullptr, st));
   DGS_TRY(wgrad_tn(d_img, d.Ndec, ts.hdec, 3 * D, g->dec_w, d.Ndec, D, d.Mt, st));  // hi part of the [hi|lo|hi] operand
   DGS_TRY(ln_modulate_bwd(x_fin, ts.dh, w->dec_ln_w, md + D, d.mod_stride, B, N, G, T, D, 1e-5f, ts.dx, 0, dmd,
                           dmd + D, g->dec_ln_w, ts.ln_stats, st));
   if (G > 0) {  // upsampler (the free Gaussian tokens, rows 0..G of every sample)
-    DGS_TRY(tiny_linear_bwd(ts.d_gs_tok, wT->ups_w, ws.hg, ts.dyb, g->ups_w, B * G, 14, D, st));
+    DGS_TRY(tiny_linear_bwd(ts.d_gs_tok, wT->ups_w, ws.hg, ts.dyb, g->ups_w, B * G, d.C, D, st));
     DGS_TRY(ln_modulate_bwd(x_fin, ts.dyb, w->ups_ln_w, mu + D, d.mod_stride, B, N, 0, G, D, 1e-5f, ts.dx, 0, dmu,
                             dmu + D, g->ups_ln_w, ts.ln_stats, st));
   }
@@ -694,13 +707,13 @@ int dgs_dit_export_ends(const dgs_dit_weights* w, int B, int V, int H, int W, in
   DGS_TRY(copy(x_pre, ts.x_pre, d.MD));
   DGS_TRY(copy(c, ws.c, (size_t)B * d.D));
   DGS_TRY(copy(mod, ws.mod, mod_n));
-  DGS_TRY(copy(gs_tok, ws.gs_tok, (size_t)B * d.G * 14));
+  DGS_TRY(copy(gs_tok, ws.gs_tok, (size_t)B * d.G * d.C));
   DGS_TRY(copy(img_gs, ws.img_gs, (size_t)d.Mt * d.Ndec));
   DGS_TRY(copy(dx0, ts.dx, d.MD));
   DGS_TRY(copy(dx_pre, ts.dx_pre, d.MD));
   DGS_TRY(copy(dmod, ts.dmod, mod_n));
   DGS_TRY(copy(dc, ts.dcond, (size_t)B * d.D));
-  DGS_TRY(copy(d_gs_tok, ts.d_gs_tok, (size_t)B * d.G * 14));
+  DGS_TRY(copy(d_gs_tok, ts.d_gs_tok, (size_t)B * d.G * d.C));
   return DGS_OK;
 }
 
@@ -869,6 +882,32 @@ int dgs_gemm_bf16(const void* A, const void* Wt, const float* bias, const float*
 int dgs_attention_fwd(const void* qkv, void* out, int B, int N, int heads, void* stream) {
   DGS_REQUIRE(qkv && out, "NULL pointer");
   return attention_fwd(qkv, out, nullptr, B, N, heads, (cudaStream_t)stream);
+}
+
+int dgs_gaussians_epilogue(const float* gs_tok, const float* img_gs, const float* ray_o, const float* ray_d, float* xyz,
+                           float* features, float* scaling, float* rotation, float* opacity, float* img_aligned_xyz,
+                           int B, int G, int V, int H, int W, int patch, int sh_degree, int scene_depth, float near_,
+                           float far_, void* stream) {
+  DGS_REQUIRE((G == 0 || gs_tok) && img_gs && ray_o && ray_d && xyz && features && scaling && rotation && opacity,
+              "NULL pointer");
+  DGS_REQUIRE(B > 0 && G >= 0 && V > 0 && patch > 0 && H % patch == 0 && W % patch == 0, "bad shape");
+  GsOut go;
+  go.xyz = xyz; go.features = features; go.scaling = scaling; go.rotation = rotation; go.opacity = opacity;
+  go.img_aligned_xyz = img_aligned_xyz;
+  return gaussians_epilogue(gs_tok, img_gs, ray_o, ray_d, go, B, G, V, H, W, patch, sh_degree, scene_depth, near_, far_,
+                            (cudaStream_t)stream);
+}
+
+int dgs_gaussians_epilogue_bwd(const float* gs_tok, const float* img_gs, const float* ray_d, const float* d_xyz,
+                               const float* d_features, const float* d_scaling, const float* d_rotation,
+                               const float* d_opacity, float* d_gs_tok, void* d_img_gs, int B, int G, int V, int H,
+                               int W, int patch, int sh_degree, int scene_depth, float near_, float far_, void* stream) {
+  DGS_REQUIRE((G == 0 || (gs_tok && d_gs_tok)) && img_gs && ray_d && d_xyz && d_features && d_scaling && d_rotation &&
+                  d_opacity && d_img_gs, "NULL pointer");
+  DGS_REQUIRE(B > 0 && G >= 0 && V > 0 && patch > 0 && H % patch == 0 && W % patch == 0, "bad shape");
+  return gaussians_epilogue_bwd(gs_tok, img_gs, ray_d, d_xyz, d_features, d_scaling, d_rotation, d_opacity, d_gs_tok,
+                                (__nv_bfloat16*)d_img_gs, B, G, V, H, W, patch, sh_degree, scene_depth, near_, far_,
+                                (cudaStream_t)stream);
 }
 
 int dgs_ln_modulate(const float* x, const float* ln_w, const float* shift, const float* scale, int mod_stride, void* h,

@@ -673,7 +673,7 @@ int silu_bwd_inplace(float* d, const float* pre, int n, cudaStream_t st) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// The tiny linear of the free Gaussian tokens' head (rows = B*G, N = 14), forward and backward.
+// The tiny linear of the free Gaussian tokens' head (rows = B*G, N = C channels), forward and backward.
 // ---------------------------------------------------------------------------------------------
 namespace {
 
@@ -726,10 +726,18 @@ int tiny_linear_bwd(const float* dy, const float* W, const __nv_bfloat16* h3, __
 
 // ---------------------------------------------------------------------------------------------
 // Gaussian heads' epilogue: to_gs + pixel alignment (denoiser.py:103-120, 362-413), one thread per Gaussian, and its
-// backward: gradients w.r.t. the renderer-ready tensors -> gradients of the raw 14-channel head outputs (free tokens
-// fp32, image tokens bf16).
+// backward: gradients w.r.t. the renderer-ready tensors -> gradients of the raw C-channel head outputs (free tokens
+// fp32, image tokens bf16).  Both are templated on the SH degree SH: a Gaussian's raw row is
+// C = 11 + 3 (SH+1)^2 channels [xyz 3 | features NF = 3 (SH+1)^2 | scaling 3 | rotation 4 | opacity 1], kept in
+// registers whole (C <= 59: no spills).
 // ---------------------------------------------------------------------------------------------
 namespace {
+
+template <int SH>
+struct GsLayout {
+  static constexpr int NF = 3 * (SH + 1) * (SH + 1);  // feature channels, coefficient-major, RGB-minor
+  static constexpr int SC = 3 + NF, ROT = SC + 3, OP = ROT + 4, C = OP + 1;
+};
 
 // An image Gaussian sits at o + t d on its pixel's ray, with t a function of sg = sigmoid(mean of its 3 xyz channels):
 //   scene 1: sg * (far - near) + near                 (denoiser_scene.py:263,406-410)
@@ -746,6 +754,7 @@ __device__ __forceinline__ float pixel_depth_dm(int scene, float sg, float near_
   return (scene == 1 ? (far_ - near_) : scene == 2 ? 1.0f : 2.0f * OBJ_DEPTH_HALF_RANGE) * sg * (1.0f - sg);
 }
 
+template <int SH>
 __global__ void __launch_bounds__(256) gaussians_epilogue_kernel(const float* __restrict__ gs_tok,
                                                                  const float* __restrict__ img_gs,
                                                                  const float* __restrict__ ray_o,
@@ -757,18 +766,20 @@ __global__ void __launch_bounds__(256) gaussians_epilogue_kernel(const float* __
   if (idx >= (long long)B * per_b) return;
   const int b = (int)(idx / per_b);
   const long long g = idx - (long long)b * per_b;
-  float a[14];
+  using Ly = GsLayout<SH>;
+  constexpr int C = Ly::C;
+  float a[C];
   float xyz[3];
   if (g < G) {
-    const float* s = gs_tok + ((size_t)b * G + g) * 14;
+    const float* s = gs_tok + ((size_t)b * G + g) * C;
 #pragma unroll
-    for (int k = 0; k < 14; k++) a[k] = s[k];
+    for (int k = 0; k < C; k++) a[k] = s[k];
     xyz[0] = a[0]; xyz[1] = a[1]; xyz[2] = a[2];
   } else {
     const long long q = g - G;  // (v, hh, ww, ph, pw) order == img_gs memory order
-    const float* s = img_gs + ((size_t)b * V * H * W + q) * 14;
+    const float* s = img_gs + ((size_t)b * V * H * W + q) * C;  // scalar loads: rows of odd C are not 8-byte aligned
 #pragma unroll
-    for (int k = 0; k < 14; k++) a[k] = s[k];
+    for (int k = 0; k < C; k++) a[k] = s[k];
     const PatchPixel px = patch_pixel(q, H, W, p);
     const size_t plane = (size_t)H * W, pix = (size_t)px.y * W + px.x;
     const size_t base = ((size_t)b * V + px.bv) * 3 * plane + pix;
@@ -786,16 +797,18 @@ __global__ void __launch_bounds__(256) gaussians_epilogue_kernel(const float* __
   }
   const size_t o = (size_t)idx;
   out.xyz[3 * o] = xyz[0]; out.xyz[3 * o + 1] = xyz[1]; out.xyz[3 * o + 2] = xyz[2];
-  out.features[3 * o] = a[3]; out.features[3 * o + 1] = a[4]; out.features[3 * o + 2] = a[5];
-  out.scaling[3 * o] = fminf(a[6] - 2.3f, -1.2f);  // denoiser.py:118
-  out.scaling[3 * o + 1] = fminf(a[7] - 2.3f, -1.2f);
-  out.scaling[3 * o + 2] = fminf(a[8] - 2.3f, -1.2f);
-  *reinterpret_cast<float4*>(out.rotation + 4 * o) = make_float4(a[9], a[10], a[11], a[12]);
-  out.opacity[o] = a[13] - 2.0f;  // denoiser.py:119
+#pragma unroll
+  for (int k = 0; k < Ly::NF; k++) out.features[Ly::NF * o + k] = a[3 + k];  // [.., (SH+1)^2, 3]: a plain copy
+  out.scaling[3 * o] = fminf(a[Ly::SC] - 2.3f, -1.2f);  // denoiser.py:118
+  out.scaling[3 * o + 1] = fminf(a[Ly::SC + 1] - 2.3f, -1.2f);
+  out.scaling[3 * o + 2] = fminf(a[Ly::SC + 2] - 2.3f, -1.2f);
+  *reinterpret_cast<float4*>(out.rotation + 4 * o) = make_float4(a[Ly::ROT], a[Ly::ROT + 1], a[Ly::ROT + 2], a[Ly::ROT + 3]);
+  out.opacity[o] = a[Ly::OP] - 2.0f;  // denoiser.py:119
 }
 
 struct GsGrad { const float* xyz; const float* features; const float* scaling; const float* rotation; const float* opacity; };
 
+template <int SH>
 __global__ void __launch_bounds__(256) gaussians_epilogue_bwd_kernel(const float* __restrict__ gs_tok,
                                                                      const float* __restrict__ img_gs,
                                                                      const float* __restrict__ ray_d, GsGrad d,
@@ -809,8 +822,10 @@ __global__ void __launch_bounds__(256) gaussians_epilogue_bwd_kernel(const float
   const int b = (int)(idx / per_b);
   const long long g = idx - (long long)b * per_b;
   const size_t o = (size_t)idx;
-  float da[14];
-  const float* src = (g < G) ? gs_tok + ((size_t)b * G + g) * 14 : img_gs + ((size_t)b * V * H * W + (g - G)) * 14;
+  using Ly = GsLayout<SH>;
+  constexpr int C = Ly::C;
+  float da[C];
+  const float* src = (g < G) ? gs_tok + ((size_t)b * G + g) * C : img_gs + ((size_t)b * V * H * W + (g - G)) * C;
   const float gx = d.xyz[3 * o], gy = d.xyz[3 * o + 1], gz = d.xyz[3 * o + 2];
   if (g < G) {
     da[0] = gx; da[1] = gy; da[2] = gz;
@@ -824,22 +839,30 @@ __global__ void __launch_bounds__(256) gaussians_epilogue_bwd_kernel(const float
     const float dt = gx * d0 + gy * d1 + gz * d2;  // xyz = o + t d
     da[0] = da[1] = da[2] = dt * pixel_depth_dm(scene, sg, near_, far_) * (1.0f / 3.0f);
   }
-  da[3] = d.features[3 * o]; da[4] = d.features[3 * o + 1]; da[5] = d.features[3 * o + 2];
 #pragma unroll
-  for (int k = 0; k < 3; k++) da[6 + k] = (src[6 + k] - 2.3f <= -1.2f) ? d.scaling[3 * o + k] : 0.f;  // clamp(max=-1.2)
+  for (int k = 0; k < Ly::NF; k++) da[3 + k] = d.features[Ly::NF * o + k];
+#pragma unroll
+  for (int k = 0; k < 3; k++)
+    da[Ly::SC + k] = (src[Ly::SC + k] - 2.3f <= -1.2f) ? d.scaling[3 * o + k] : 0.f;  // clamp(max=-1.2)
   const float4 dr = *reinterpret_cast<const float4*>(d.rotation + 4 * o);
-  da[9] = dr.x; da[10] = dr.y; da[11] = dr.z; da[12] = dr.w;
-  da[13] = d.opacity[o];
+  da[Ly::ROT] = dr.x; da[Ly::ROT + 1] = dr.y; da[Ly::ROT + 2] = dr.z; da[Ly::ROT + 3] = dr.w;
+  da[Ly::OP] = d.opacity[o];
   if (g < G) {
-    float* dst = d_gs_tok + ((size_t)b * G + g) * 14;
+    float* dst = d_gs_tok + ((size_t)b * G + g) * C;
 #pragma unroll
-    for (int k = 0; k < 14; k++) dst[k] = da[k];
+    for (int k = 0; k < C; k++) dst[k] = da[k];
   } else {
-    __nv_bfloat16* dst = d_img_gs + ((size_t)b * V * H * W + (g - G)) * 14;
+    __nv_bfloat16* dst = d_img_gs + ((size_t)b * V * H * W + (g - G)) * C;
+    if constexpr (C % 2 == 0) {
 #pragma unroll
-    for (int k = 0; k < 14; k += 2) {
-      __nv_bfloat162 pk = __floats2bfloat162_rn(da[k], da[k + 1]);
-      *reinterpret_cast<__nv_bfloat162*>(dst + k) = pk;
+      for (int k = 0; k < C; k += 2) {
+        __nv_bfloat162 pk = __floats2bfloat162_rn(da[k], da[k + 1]);
+        *reinterpret_cast<__nv_bfloat162*>(dst + k) = pk;
+      }
+    } else {  // odd C: every other row starts on a 2-byte boundary, so no pair stores.  Consecutive threads write
+              // consecutive rows, so a warp's stores still fill whole sectors of one contiguous 32 C * 2-byte range.
+#pragma unroll
+      for (int k = 0; k < C; k++) dst[k] = __float2bfloat16_rn(da[k]);
     }
   }
 }
@@ -847,11 +870,21 @@ __global__ void __launch_bounds__(256) gaussians_epilogue_bwd_kernel(const float
 }  // namespace
 
 int gaussians_epilogue(const float* gs_tokens, const float* img_gs, const float* ray_o, const float* ray_d, GsOut out,
-                       int B, int G, int V, int H, int W, int patch, int scene_mode, float near_, float far_,
-                       cudaStream_t st) {
+                       int B, int G, int V, int H, int W, int patch, int sh_degree, int scene_mode, float near_,
+                       float far_, cudaStream_t st) {
   const long long total = (long long)B * ((long long)G + (long long)V * H * W);
-  gaussians_epilogue_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(gs_tokens, img_gs, ray_o, ray_d, out, B, G,
-                                                                              V, H, W, patch, scene_mode, near_, far_);
+  const dim3 grid((unsigned)((total + 255) / 256));
+  switch (sh_degree) {
+    case 0: gaussians_epilogue_kernel<0><<<grid, 256, 0, st>>>(gs_tokens, img_gs, ray_o, ray_d, out, B, G, V, H, W, patch,
+                                                                scene_mode, near_, far_); break;
+    case 1: gaussians_epilogue_kernel<1><<<grid, 256, 0, st>>>(gs_tokens, img_gs, ray_o, ray_d, out, B, G, V, H, W, patch,
+                                                                scene_mode, near_, far_); break;
+    case 2: gaussians_epilogue_kernel<2><<<grid, 256, 0, st>>>(gs_tokens, img_gs, ray_o, ray_d, out, B, G, V, H, W, patch,
+                                                                scene_mode, near_, far_); break;
+    case 3: gaussians_epilogue_kernel<3><<<grid, 256, 0, st>>>(gs_tokens, img_gs, ray_o, ray_d, out, B, G, V, H, W, patch,
+                                                                scene_mode, near_, far_); break;
+    default: DGS_REQUIRE(false, "gaussians_epilogue: sh_degree %d out of [0, 3]", sh_degree);
+  }
   DGS_POST_LAUNCH();
   return DGS_OK;
 }
@@ -859,12 +892,21 @@ int gaussians_epilogue(const float* gs_tokens, const float* img_gs, const float*
 int gaussians_epilogue_bwd(const float* gs_tok, const float* img_gs, const float* ray_d, const float* dxyz,
                            const float* dfeatures, const float* dscaling, const float* drotation, const float* dopacity,
                            float* d_gs_tok, __nv_bfloat16* d_img_gs, int B, int G, int V, int H, int W, int patch,
-                           int scene_mode, float near_, float far_, cudaStream_t st) {
+                           int sh_degree, int scene_mode, float near_, float far_, cudaStream_t st) {
   GsGrad d{dxyz, dfeatures, dscaling, drotation, dopacity};
   const long long total = (long long)B * ((long long)G + (long long)V * H * W);
-  gaussians_epilogue_bwd_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(gs_tok, img_gs, ray_d, d, d_gs_tok,
-                                                                                  d_img_gs, B, G, V, H, W, patch,
-                                                                                  scene_mode, near_, far_);
+  const dim3 grid((unsigned)((total + 255) / 256));
+  switch (sh_degree) {
+    case 0: gaussians_epilogue_bwd_kernel<0><<<grid, 256, 0, st>>>(gs_tok, img_gs, ray_d, d, d_gs_tok, d_img_gs, B, G, V,
+                                                                    H, W, patch, scene_mode, near_, far_); break;
+    case 1: gaussians_epilogue_bwd_kernel<1><<<grid, 256, 0, st>>>(gs_tok, img_gs, ray_d, d, d_gs_tok, d_img_gs, B, G, V,
+                                                                    H, W, patch, scene_mode, near_, far_); break;
+    case 2: gaussians_epilogue_bwd_kernel<2><<<grid, 256, 0, st>>>(gs_tok, img_gs, ray_d, d, d_gs_tok, d_img_gs, B, G, V,
+                                                                    H, W, patch, scene_mode, near_, far_); break;
+    case 3: gaussians_epilogue_bwd_kernel<3><<<grid, 256, 0, st>>>(gs_tok, img_gs, ray_d, d, d_gs_tok, d_img_gs, B, G, V,
+                                                                    H, W, patch, scene_mode, near_, far_); break;
+    default: DGS_REQUIRE(false, "gaussians_epilogue_bwd: sh_degree %d out of [0, 3]", sh_degree);
+  }
   DGS_POST_LAUNCH();
   return DGS_OK;
 }

@@ -82,14 +82,15 @@ int posed_patchify(const float* images, const float* ray_o, const float* ray_d, 
                    int H, int W, int patch, int plucker_mode, cudaStream_t st);
 // x[b, 0:G] = pos_embed ; x[b, G:] = tok[b] ; (then the caller applies the input LayerNorm)
 int assemble_tokens(const float* tok, const float* pos_embed, float* x, int B, int G, int T, int D, cudaStream_t st);
-// small-M linear for the 2 free Gaussian tokens: out[r, n] = h[r,:] . W[n,:]   (N = 14)
+// small-M linear for the 2 free Gaussian tokens: out[r, n] = h[r,:] . W[n,:]   (N = C head channels)
 int tiny_linear_bf16(const __nv_bfloat16* h, const __nv_bfloat16* W, float* out, int rows, int N, int K,
                      cudaStream_t st);
 // to_gs + pixel alignment (denoiser.py:103-120, 362-413): raw head outputs -> renderer tensors
 struct GsOut { float* xyz; float* features; float* scaling; float* rotation; float* opacity; float* img_aligned_xyz; };
-int gaussians_epilogue(const float* gs_tokens /*[B,G,14]*/, const float* img_gs /*[B*V*hh*ww, p*p*14]*/,
+// C = 11 + 3 (sh_degree+1)^2 raw channels per Gaussian, sh_degree 0..3; features out [B, P, (sh_degree+1)^2, 3]
+int gaussians_epilogue(const float* gs_tokens /*[B,G,C]*/, const float* img_gs /*[B*V*hh*ww, p*p*C]*/,
                        const float* ray_o, const float* ray_d, GsOut out, int B, int G, int V, int H, int W, int patch,
-                       int scene_mode, float near_, float far_, cudaStream_t st);
+                       int sh_degree, int scene_mode, float near_, float far_, cudaStream_t st);
 
 // ---- dit_glue.cu: backward ---------------------------------------------------------------------
 // out[c, m] = bf16(in[row(m), c]); m = b*rows_out + j -> input row b*rows_in + row_off + j; out [C, round_up(M,64)]
@@ -125,7 +126,7 @@ int silu_bwd_inplace(float* d, const float* pre, int n, cudaStream_t st);
 int gaussians_epilogue_bwd(const float* gs_tok, const float* img_gs, const float* ray_d, const float* dxyz,
                            const float* dfeatures, const float* dscaling, const float* drotation, const float* dopacity,
                            float* d_gs_tok, __nv_bfloat16* d_img_gs, int B, int G, int V, int H, int W, int patch,
-                           int scene_mode, float near_, float far_, cudaStream_t st);
+                           int sh_degree, int scene_mode, float near_, float far_, cudaStream_t st);
 int tiny_linear_bwd(const float* dy, const float* W, const __nv_bfloat16* h3, __nv_bfloat16* dh, float* dW, int rows,
                     int N, int K, cudaStream_t st);
 int pos_embed_bwd(const float* dx, float* dpos, int B, int G, int N, int D, cudaStream_t st);

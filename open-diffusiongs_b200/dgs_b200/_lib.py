@@ -32,7 +32,8 @@ class DitWeights(C.Structure):
                 ("n_gaussians", C.c_int), ("mlp_hidden", C.c_int)] + [
         (n, C.c_void_p) for n in (
             "tokenizer_w", "pos_embed", "in_ln_w", "t0_w", "t0_b", "t2_w", "t2_b", "adaln_w", "adaln_b", "qkv_w",
-            "qkv_b", "proj_w", "proj_b", "fc1_w", "fc1_b", "fc2_w", "fc2_b", "ups_ln_w", "ups_w", "dec_ln_w", "dec_w")]
+            "qkv_b", "proj_w", "proj_b", "fc1_w", "fc1_b", "fc2_w", "fc2_b", "ups_ln_w", "ups_w", "dec_ln_w", "dec_w")] + [
+        ("sh_degree", C.c_int)]
 
 
 class DitIO(C.Structure):
@@ -173,6 +174,8 @@ def lib():
         L.dgs_ln_modulate_bwd.argtypes = [vp, vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, vp,
                                           C.c_int, vp, vp, vp, vp, vp]
         L.dgs_gate_bwd.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp]
+        L.dgs_gaussians_epilogue.argtypes = [vp] * 10 + [C.c_int] * 8 + [C.c_float, C.c_float, vp]
+        L.dgs_gaussians_epilogue_bwd.argtypes = [vp] * 10 + [C.c_int] * 8 + [C.c_float, C.c_float, vp]
         L.dgs_rays_from_cameras.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp]
         L.dgs_q_sample.argtypes = [vp, vp, vp, vp, vp, C.c_int, C.c_longlong, vp, vp]
         L.dgs_p_sample_step.argtypes = [vp, vp, vp, vp, vp, vp, vp, C.c_int, C.c_longlong, vp, vp]
@@ -243,6 +246,7 @@ EXPORTED = [  # every symbol include/dgs_b200.h declares (checked by tests/test_
     "dgs_rays_from_cameras", "dgs_q_sample", "dgs_p_sample_step",
     "dgs_dit_train_state_bytes", "dgs_dit_backward", "dgs_transpose_bf16", "dgs_adamw_step", "dgs_attention_fwd_train",
     "dgs_attention_bwd", "dgs_gemm_bf16_ex", "dgs_ln_modulate_bwd", "dgs_gate_bwd", "dgs_cast_transpose_f32", "dgs_gemm_bf16_tn",
+    "dgs_gaussians_epilogue", "dgs_gaussians_epilogue_bwd",
     "dgs_dit_train_state_bytes_ex", "dgs_dit_backward_ex", "dgs_event_create", "dgs_event_destroy", "dgs_stream_wait_event",
     "dgs_adamw_ema_step", "dgs_render_batch_forward_mse", "dgs_render_batch_backward_mse", "dgs_dit_export_state",
     "dgs_dit_export_ends", "dgs_lpips_workspace_bytes", "dgs_lpips_state_bytes", "dgs_lpips_forward", "dgs_lpips_backward",

@@ -97,6 +97,12 @@ class _TEmbedParams(nn.Module):
         self.mlp = nn.Sequential(nn.Linear(freq, dim, bias=True), nn.SiLU(), nn.Linear(dim, dim, bias=True))
 
 
+def head_channels(sh_degree):
+    """Channels per Gaussian of both heads (denoiser.py:94-98, 145-149): [xyz 3 | features 3 (d+1)^2 | scaling 3 |
+    rotation 4 | opacity 1] = 14, 23, 38, 59 for d = 0..3."""
+    return 11 + 3 * (sh_degree + 1) ** 2
+
+
 def _init_linear(m):  # utils_transformer.py:30-36
     if isinstance(m, nn.Linear):
         nn.init.normal_(m.weight, mean=0.0, std=0.02)
@@ -117,8 +123,14 @@ class DGSDenoiser(nn.Module):
                              "every shipped reference config sets in_channels: 9")
         if c.ray_pe_type not in ("relative_plk", "plk"):
             raise ValueError(f"ray_pe_type={c.ray_pe_type!r} (expected 'relative_plk' or 'plk')")
-        if c.gaussians_sh_degree != 0:
-            raise NotImplementedError("the DiT heads are built for gaussians_sh_degree == 0 (every shipped config)")
+        if c.gaussians_sh_degree not in (0, 1, 2, 3):
+            raise ValueError(f"gaussians_sh_degree={c.gaussians_sh_degree!r} (expected 0..3: the rasterizer evaluates "
+                             "spherical harmonics up to degree 3)")
+        ch = head_channels(c.gaussians_sh_degree)
+        if c.patch_size ** 2 * ch % 32:
+            raise ValueError(f"patch_size={c.patch_size} with gaussians_sh_degree={c.gaussians_sh_degree}: the decoder "
+                             f"head's patch_size^2 * {ch} outputs per token must be a multiple of 32 (the GEMM's N % 32 "
+                             "rule)")
         self.t_embedder = _TEmbedParams(w)
         nn.init.normal_(self.t_embedder.mlp[0].weight, std=0.02)
         nn.init.normal_(self.t_embedder.mlp[2].weight, std=0.02)
@@ -131,9 +143,9 @@ class DGSDenoiser(nn.Module):
         self.transformer_input_layernorm = nn.LayerNorm(w, bias=False)
         self.transformer = nn.ModuleList([_BlockParams(w) for _ in range(c.num_layers)])
         self.transformer.apply(_init_linear)
-        self.upsampler = _HeadParams(w, 14)
+        self.upsampler = _HeadParams(w, ch)
         self.upsampler.apply(_init_linear)
-        self.image_token_decoder = _HeadParams(w, c.patch_size ** 2 * 14)
+        self.image_token_decoder = _HeadParams(w, c.patch_size ** 2 * ch)
         self.image_token_decoder.apply(_init_linear)
         self.gs_renderer = Renderer(c)
         self.register_buffer("_dummy", torch.zeros(0, dtype=torch.float32), persistent=False)  # dGS/utils/base.py:115
@@ -154,7 +166,8 @@ class DGSDenoiser(nn.Module):
         return tuple((p.data_ptr(), p._version) for p in self.parameters())
 
     def _pack_dict(self, skip=()):
-        """fp32 master parameters -> {field of dgs_dit_weights: tensor}; `skip` = fields somebody else fills."""
+        """fp32 master parameters -> {field of dgs_dit_weights: tensor} for every field after the six dimensions, the
+        last of which, sh_degree, is the plain int of the config; `skip` = fields somebody else fills."""
         bf = lambda t: t.detach().to(torch.bfloat16).contiguous()  # noqa: E731
 
         def split(t):  # split-bf16 weight [n, 3k] = [hi | hi | lo]  (see include/dgs_b200.h)
@@ -182,7 +195,8 @@ class DGSDenoiser(nn.Module):
             fc2_w=lambda: bf(stack(lambda b: b.mlp.fc2.weight)), fc2_b=lambda: f32(stack(lambda b: b.mlp.fc2.bias)),
             ups_ln_w=lambda: f32(self.upsampler.layernorm.weight), ups_w=lambda: split(self.upsampler.linear.weight),
             dec_ln_w=lambda: f32(self.image_token_decoder.layernorm.weight),
-            dec_w=lambda: split(self.image_token_decoder.linear.weight))
+            dec_w=lambda: split(self.image_token_decoder.linear.weight),
+            sh_degree=lambda: int(self.cfg.gaussians_sh_degree))
         return {k: fn() for k, fn in make.items() if k not in skip}
 
     def packed_weights(self, force=False):
@@ -195,7 +209,7 @@ class DGSDenoiser(nn.Module):
                        n_gaussians=c.n_gaussians, mlp_hidden=4 * c.width)
         assert tuple(self.image_tokenizer[1].weight.shape) == (c.width, 9 * c.patch_size ** 2), "tokenizer weight shape"
         for k, v in t.items():
-            setattr(w, k, v.data_ptr())
+            setattr(w, k, v if k == "sh_degree" else v.data_ptr())
         self._packed, self._packed_key = (w, t), key
         return self._packed
 
@@ -281,7 +295,8 @@ class DGSDenoiser(nn.Module):
         w, _keep = self.packed_weights()
         with torch.cuda.device(dev):
             new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)  # noqa: E731
-            out = AttrDict(xyz=new(B, P, 3), features=new(B, P, 1, 3), scaling=new(B, P, 3), rotation=new(B, P, 4),
+            n_sh = (c.gaussians_sh_degree + 1) ** 2
+            out = AttrDict(xyz=new(B, P, 3), features=new(B, P, n_sh, 3), scaling=new(B, P, 3), rotation=new(B, P, 4),
                            opacity=new(B, P, 1))
             img_xyz = new(B, V, 3, H, W)
             n_tok = c.n_gaussians + V * (H // c.patch_size) * (W // c.patch_size)

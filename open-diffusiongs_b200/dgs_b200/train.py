@@ -16,6 +16,7 @@ import contextlib
 import torch.distributed as dist
 
 from ._lib import DitBwdOpts, DitGrads, DitOutGrads, DitWeightsT, check
+from .denoiser import head_channels
 from .dist import GradArena, gradient_group
 
 
@@ -140,7 +141,7 @@ class DitTrainer:
                 check(L.dgs_cast_transpose_f32(p0.data_ptr(), stride, len(T), p0.shape[0], p0.shape[1], t[k].data_ptr(),
                                                self._wT_keep[k + "T"].data_ptr(), _stream(dev)))
         if not first:
-            for k, v in m._pack_dict(skip=tuple(self._BIG)).items():
+            for k, v in m._pack_dict(skip=tuple(self._BIG) + ("sh_degree",)).items():
                 t[k].copy_(v)
         m._packed_key = m._pack_key()
         self._wT_keep["dec_wT"] = m.image_token_decoder.linear.weight.detach().t().to(torch.bfloat16).contiguous()
@@ -197,7 +198,8 @@ class DitTrainer:
         """Copies of the tensors on either side of the blocks (dgs_dit_export_ends), all fp32: {name: tensor} for
         `names` out of ENDS_FIELDS.  From the last training forward at shape (B, V, H, W): x_pre [B, N, width] (tokens
         before the input LayerNorm), c [B, width] (conditioning before the adaLN SiLU), mod [B, L*6*width + 4*width]
-        (adaLN table), gs_tok [B, G, 14] and img_gs [B, T, p*p*14] (raw head outputs).  From the backward that
+        (adaLN table), gs_tok [B, G, C] and img_gs [B, T, p*p*C] (raw head outputs, C = 11 + 3 (sh_degree+1)^2
+        channels per Gaussian).  From the backward that
         followed it (undefined before one): dx0 [B, N, width] (gradient entering block 0), dx_pre, dmod, dc and
         d_gs_tok, the gradients of x_pre, mod, c and gs_tok."""
         unknown = set(names) - set(self.ENDS_FIELDS)
@@ -207,11 +209,11 @@ class DitTrainer:
             raise RuntimeError("DitTrainer.export_ends: no training forward has run")
         c = self.model.cfg
         w, _ = self.model.packed_weights()
-        p, G, D = c.patch_size, c.n_gaussians, c.width
+        p, G, D, Ch = c.patch_size, c.n_gaussians, c.width, head_channels(c.gaussians_sh_degree)
         T = V * (H // p) * (W // p)
         N, R = G + T, c.num_layers * 6 * D + 4 * D
-        shapes = dict(x_pre=(B, N, D), c=(B, D), mod=(B, R), gs_tok=(B, G, 14), img_gs=(B, T, p * p * 14),
-                      dx0=(B, N, D), dx_pre=(B, N, D), dmod=(B, R), dc=(B, D), d_gs_tok=(B, G, 14))
+        shapes = dict(x_pre=(B, N, D), c=(B, D), mod=(B, R), gs_tok=(B, G, Ch), img_gs=(B, T, p * p * Ch),
+                      dx0=(B, N, D), dx_pre=(B, N, D), dmod=(B, R), dc=(B, D), d_gs_tok=(B, G, Ch))
         dev = self.master.device
         out = {k: torch.empty(shapes[k], dtype=torch.float32, device=dev) for k in names}
         args = [out[k].data_ptr() if k in out else None for k in self.ENDS_FIELDS]
@@ -401,8 +403,9 @@ class _DitFunction(torch.autograd.Function):
         dev = images.device
         B, V, _, H, W = images.shape
         P = model.cfg.n_gaussians + V * H * W
+        n_sh = (model.cfg.gaussians_sh_degree + 1) ** 2
         z = lambda g, *s: (torch.zeros(*s, device=dev) if g is None else g.float().contiguous())  # noqa: E731
-        gs = [z(d_xyz, B, P, 3), z(d_features, B, P, 1, 3), z(d_scaling, B, P, 3), z(d_rotation, B, P, 4),
+        gs = [z(d_xyz, B, P, 3), z(d_features, B, P, n_sh, 3), z(d_scaling, B, P, 3), z(d_rotation, B, P, 4),
               z(d_opacity, B, P, 1)]
         dout = DitOutGrads(*(g.data_ptr() for g in gs))
         opts = tr._bwd_opts()
