@@ -370,6 +370,9 @@ typedef struct {  /* all fp32, OVERWRITTEN by dgs_dit_backward */
 
 typedef struct {  /* gradients w.r.t. the outputs of dgs_dit_forward (what dgs_render_batch_backward returns) */
   const float* d_xyz; const float* d_features; const float* d_scaling; const float* d_rotation; const float* d_opacity;
+  /* the gradient of img_aligned_xyz (what dgs_geometry_loss_backward returns): the same values as the image Gaussians'
+     xyz in the pixel layout, so it is added to their d_xyz.  NULL: none, and the backward is unchanged bit for bit */
+  const float* d_img_aligned_xyz; /* [B,V,3,H,W] or NULL */
 } dgs_dit_out_grads;  /* shapes of the dgs_dit_io outputs: d_features [B,P,(sh_degree+1)^2,3] */
 
 size_t dgs_dit_train_state_bytes(const dgs_dit_weights* w, int B, int V, int H, int W); /* DGS_TRAIN_STORE */
@@ -499,8 +502,9 @@ int dgs_ln_modulate(const float* x, const float* ln_w, const float* shift, const
 /* The Gaussian heads' epilogue (to_gs + pixel alignment) and its backward, the kernels dgs_dit_forward /
  * dgs_dit_backward launch: the raw head outputs gs_tok [B*G, C] and img_gs [B*T, patch*patch*C] fp32 (C = 11 +
  * 3 (sh_degree+1)^2; image rows in (v, hh, ww, ph, pw) order), rays [B,V,3,H,W] -> the outputs of dgs_dit_io
- * (img_aligned_xyz may be NULL); scene_depth, near_, far_ as in dgs_dit_io.  The backward turns the gradients of those
- * outputs into d_gs_tok [B*G, C] fp32 and d_img_gs [B*T, patch*patch*C] bf16. */
+ * (img_aligned_xyz may be NULL); scene_depth, near_, far_ as in dgs_dit_io.  The backward turns the gradients of the
+ * five Gaussian outputs (not of img_aligned_xyz: dgs_dit_backward takes that one) into d_gs_tok [B*G, C] fp32 and
+ * d_img_gs [B*T, patch*patch*C] bf16. */
 int dgs_gaussians_epilogue(const float* gs_tok, const float* img_gs, const float* ray_o, const float* ray_d, float* xyz,
                            float* features, float* scaling, float* rotation, float* opacity, float* img_aligned_xyz,
                            int B, int G, int V, int H, int W, int patch, int sh_degree, int scene_depth, float near_,
@@ -573,6 +577,34 @@ int dgs_ssim_forward(int n, int H, int W, const float* x, const float* y, float 
  * 1 - ssim).  x and y are the forward's images.  The gradient w.r.t. y is not computed. */
 int dgs_ssim_backward(int n, int H, int W, const float* x, const float* y, const void* state, const float* dout,
                       float* d_x, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * B2e. The geometry terms of LossComputer on the pixel-aligned Gaussian centres img_xyz [B, V, 3, H, W]
+ * (diffusionGS/utils/losses.py:286-291, 323-364), all tensors fp32 and contiguous:
+ *   pointsdist[b] = mean over (v, h, w) of (dist - trgt)^2,  dist = |img_xyz - ray_o|,
+ *                   trgt = (dist - mean) / (std + 1e-8) * 0.5 + |ray_o| (detached), mean and unbiased std of dist over
+ *                   each view's H*W pixels, |ray_o| per pixel;
+ *   l2_xyz        = sum (img_xyz m - gt_xyz m)^2 / sum m, m = masks [B, V, 1, H, W] over the 3 channels (an all-zero
+ *                   mask gives NaN, as in the reference).
+ * Per-pixel arithmetic is fp32, every sum fp64 in a fixed order without atomics: the same bits on every run, and
+ * pointsdist[b] does not depend on the other samples.  B, V, H, W > 0, B*V <= 65535, H*W <= 2^30, else
+ * DGS_ERR_INVALID_ARGUMENT.
+ * ---------------------------------------------------------------------------------------------- */
+/* Workspace of one forward: fp64 partial sums, 64 per view. */
+size_t dgs_geometry_loss_workspace_bytes(int B, int V);
+/* pointsdist (device [B]) is computed when not NULL, and needs ray_o; l2_xyz (device [1]) when not NULL, and needs
+ * gt_xyz and masks.  state: device fp32 [2*B*V + 1] -- each view's (mean, std) of dist, then sum m -- that the backward
+ * reads; keep it untouched until then. */
+int dgs_geometry_loss_forward(int B, int V, int H, int W, const float* img_xyz, const float* ray_o, const float* gt_xyz,
+                              const float* masks, float* pointsdist, float* l2_xyz, float* state, void* workspace,
+                              size_t workspace_bytes, void* stream);
+/* d_img_xyz [B, V, 3, H, W] (overwritten) = g_pointsdist[b] d pointsdist[b] / d img + g_l2_xyz[0] d l2_xyz / d img, the
+ * upstream gradients as DEVICE scalars (no host sync); either may be NULL (that term is 0), but each one given needs
+ * its term computed by the forward that wrote `state`.  The pointsdist part is 0 where dist == 0.  No gradient w.r.t.
+ * ray_o, gt_xyz or masks. */
+int dgs_geometry_loss_backward(int B, int V, int H, int W, const float* img_xyz, const float* ray_o, const float* gt_xyz,
+                               const float* masks, const float* state, const float* g_pointsdist, const float* g_l2_xyz,
+                               float* d_img_xyz, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * B2d. Mesh extraction after the sampler loop: GaussianModel.extract_fields / extract_mesh

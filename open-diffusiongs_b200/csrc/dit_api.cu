@@ -414,8 +414,9 @@ int heads_backward(const dgs_dit_weights* w, const dgs_dit_weights_t* wT, const 
   ProfScope ps(st, PROF_DIT_BWD_ELEM);
   __nv_bfloat16* d_img = ts.big0;  // [Mt, Ndec]
   DGS_TRY(gaussians_epilogue_bwd(ws.gs_tok, ws.img_gs, io->ray_d, dout->d_xyz, dout->d_features, dout->d_scaling,
-                                 dout->d_rotation, dout->d_opacity, ts.d_gs_tok, d_img, B, G, io->V, io->H, io->W,
-                                 w->patch, w->sh_degree, io->scene_depth, io->range_near, io->range_far, st));
+                                 dout->d_rotation, dout->d_opacity, dout->d_img_aligned_xyz, ts.d_gs_tok, d_img, B, G,
+                                 io->V, io->H, io->W, w->patch, w->sh_degree, io->scene_depth, io->range_near,
+                                 io->range_far, st));
   // image_token_decoder: dh = d_img W, dW = d_img^T h
   DGS_TRY(dgrad(d_img, wT->dec_wT, ts.dh, d.Mt, D, d.Ndec, EPI_BIAS_BF16, nullptr, st));
   DGS_TRY(wgrad_tn(d_img, d.Ndec, ts.hdec, 3 * D, g->dec_w, d.Ndec, D, d.Mt, st));  // hi part of the [hi|lo|hi] operand
@@ -905,9 +906,9 @@ int dgs_gaussians_epilogue_bwd(const float* gs_tok, const float* img_gs, const f
   DGS_REQUIRE((G == 0 || (gs_tok && d_gs_tok)) && img_gs && ray_d && d_xyz && d_features && d_scaling && d_rotation &&
                   d_opacity && d_img_gs, "NULL pointer");
   DGS_REQUIRE(B > 0 && G >= 0 && V > 0 && patch > 0 && H % patch == 0 && W % patch == 0, "bad shape");
-  return gaussians_epilogue_bwd(gs_tok, img_gs, ray_d, d_xyz, d_features, d_scaling, d_rotation, d_opacity, d_gs_tok,
-                                (__nv_bfloat16*)d_img_gs, B, G, V, H, W, patch, sh_degree, scene_depth, near_, far_,
-                                (cudaStream_t)stream);
+  return gaussians_epilogue_bwd(gs_tok, img_gs, ray_d, d_xyz, d_features, d_scaling, d_rotation, d_opacity, nullptr,
+                                d_gs_tok, (__nv_bfloat16*)d_img_gs, B, G, V, H, W, patch, sh_degree, scene_depth, near_,
+                                far_, (cudaStream_t)stream);
 }
 
 int dgs_ln_modulate(const float* x, const float* ln_w, const float* shift, const float* scale, int mod_stride, void* h,

@@ -806,7 +806,12 @@ __global__ void __launch_bounds__(256) gaussians_epilogue_kernel(const float* __
   out.opacity[o] = a[Ly::OP] - 2.0f;  // denoiser.py:119
 }
 
-struct GsGrad { const float* xyz; const float* features; const float* scaling; const float* rotation; const float* opacity; };
+// img_xyz: NULL, or the gradient of img_aligned_xyz [B,V,3,H,W] -- the image Gaussians' xyz in the pixel layout, so it
+// adds to their d xyz exactly
+struct GsGrad {
+  const float* xyz; const float* features; const float* scaling; const float* rotation; const float* opacity;
+  const float* img_xyz;
+};
 
 template <int SH>
 __global__ void __launch_bounds__(256) gaussians_epilogue_bwd_kernel(const float* __restrict__ gs_tok,
@@ -826,13 +831,18 @@ __global__ void __launch_bounds__(256) gaussians_epilogue_bwd_kernel(const float
   constexpr int C = Ly::C;
   float da[C];
   const float* src = (g < G) ? gs_tok + ((size_t)b * G + g) * C : img_gs + ((size_t)b * V * H * W + (g - G)) * C;
-  const float gx = d.xyz[3 * o], gy = d.xyz[3 * o + 1], gz = d.xyz[3 * o + 2];
+  float gx = d.xyz[3 * o], gy = d.xyz[3 * o + 1], gz = d.xyz[3 * o + 2];
   if (g < G) {
     da[0] = gx; da[1] = gy; da[2] = gz;
   } else {
     const PatchPixel px = patch_pixel(g - G, H, W, p);
     const size_t plane = (size_t)H * W, pix = (size_t)px.y * W + px.x;
     const size_t base = ((size_t)b * V + px.bv) * 3 * plane + pix;
+    if (d.img_xyz) {
+      gx += d.img_xyz[base];
+      gy += d.img_xyz[base + plane];
+      gz += d.img_xyz[base + 2 * plane];
+    }
     const float d0 = ray_d[base], d1 = ray_d[base + plane], d2 = ray_d[base + 2 * plane];
     const float m = (src[0] + src[1] + src[2]) / 3.0f;
     const float sg = 1.0f / (1.0f + expf(-m));
@@ -891,9 +901,9 @@ int gaussians_epilogue(const float* gs_tokens, const float* img_gs, const float*
 
 int gaussians_epilogue_bwd(const float* gs_tok, const float* img_gs, const float* ray_d, const float* dxyz,
                            const float* dfeatures, const float* dscaling, const float* drotation, const float* dopacity,
-                           float* d_gs_tok, __nv_bfloat16* d_img_gs, int B, int G, int V, int H, int W, int patch,
-                           int sh_degree, int scene_mode, float near_, float far_, cudaStream_t st) {
-  GsGrad d{dxyz, dfeatures, dscaling, drotation, dopacity};
+                           const float* d_img_xyz, float* d_gs_tok, __nv_bfloat16* d_img_gs, int B, int G, int V, int H,
+                           int W, int patch, int sh_degree, int scene_mode, float near_, float far_, cudaStream_t st) {
+  GsGrad d{dxyz, dfeatures, dscaling, drotation, dopacity, d_img_xyz};
   const long long total = (long long)B * ((long long)G + (long long)V * H * W);
   const dim3 grid((unsigned)((total + 255) / 256));
   switch (sh_degree) {

@@ -125,8 +125,9 @@ int skinny_linear_bwd(const float* in, const float* W, const float* dout, int ld
 int silu_bwd_inplace(float* d, const float* pre, int n, cudaStream_t st);
 int gaussians_epilogue_bwd(const float* gs_tok, const float* img_gs, const float* ray_d, const float* dxyz,
                            const float* dfeatures, const float* dscaling, const float* drotation, const float* dopacity,
-                           float* d_gs_tok, __nv_bfloat16* d_img_gs, int B, int G, int V, int H, int W, int patch,
-                           int sh_degree, int scene_mode, float near_, float far_, cudaStream_t st);
+                           const float* d_img_xyz /* [B,V,3,H,W] or NULL */, float* d_gs_tok, __nv_bfloat16* d_img_gs,
+                           int B, int G, int V, int H, int W, int patch, int sh_degree, int scene_mode, float near_,
+                           float far_, cudaStream_t st);
 int tiny_linear_bwd(const float* dy, const float* W, const __nv_bfloat16* h3, __nv_bfloat16* dh, float* dW, int rows,
                     int N, int K, cudaStream_t st);
 int pos_embed_bwd(const float* dx, float* dpos, int B, int G, int N, int D, cudaStream_t st);

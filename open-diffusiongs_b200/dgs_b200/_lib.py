@@ -94,7 +94,8 @@ class DitGrads(C.Structure):  # dgs_dit_grads
 
 
 class DitOutGrads(C.Structure):  # dgs_dit_out_grads
-    _fields_ = [(n, C.c_void_p) for n in ("d_xyz", "d_features", "d_scaling", "d_rotation", "d_opacity")]
+    _fields_ = [(n, C.c_void_p) for n in ("d_xyz", "d_features", "d_scaling", "d_rotation", "d_opacity",
+                                          "d_img_aligned_xyz")]
 
 
 _lib = None
@@ -193,6 +194,10 @@ def lib():
         L.dgs_ssim_forward.argtypes = [C.c_int, C.c_int, C.c_int, vp, vp, C.c_float, C.c_int, vp, vp, vp, vp, C.c_size_t,
                                        vp]
         L.dgs_ssim_backward.argtypes = [C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]
+        L.dgs_geometry_loss_workspace_bytes.restype = C.c_size_t
+        L.dgs_geometry_loss_workspace_bytes.argtypes = [C.c_int, C.c_int]
+        L.dgs_geometry_loss_forward.argtypes = [C.c_int] * 4 + [vp] * 8 + [C.c_size_t, vp]
+        L.dgs_geometry_loss_backward.argtypes = [C.c_int] * 4 + [vp] * 9
         L.dgs_dit_workspace_bytes_fp8.restype = C.c_size_t
         L.dgs_dit_workspace_bytes_fp8.argtypes = [C.POINTER(DitWeights), C.c_int, C.c_int, C.c_int, C.c_int]
         L.dgs_dit_forward_fp8.argtypes = [C.POINTER(DitWeights), C.POINTER(DitWeightsFp8), C.POINTER(DitIO), vp, C.c_size_t,
@@ -251,6 +256,7 @@ EXPORTED = [  # every symbol include/dgs_b200.h declares (checked by tests/test_
     "dgs_adamw_ema_step", "dgs_render_batch_forward_mse", "dgs_render_batch_backward_mse", "dgs_dit_export_state",
     "dgs_dit_export_ends", "dgs_lpips_workspace_bytes", "dgs_lpips_state_bytes", "dgs_lpips_forward", "dgs_lpips_backward",
     "dgs_ssim_workspace_bytes", "dgs_ssim_state_bytes", "dgs_ssim_forward", "dgs_ssim_backward",
+    "dgs_geometry_loss_workspace_bytes", "dgs_geometry_loss_forward", "dgs_geometry_loss_backward",
     "dgs_dit_workspace_bytes_fp8", "dgs_dit_forward_fp8", "dgs_quantize_rows_e4m3", "dgs_ln_modulate_fp8", "dgs_gemm_fp8",
     "dgs_mesh_field", "dgs_marching_cubes", "dgs_render_batch_forward_aux", "dgs_render_batch_backward_aux",
     "dgs_dit_workspace_bytes_fp8_ex", "dgs_dit_forward_fp8_ex", "dgs_attention_quantize_e4m3", "dgs_attention_fwd_fp8",

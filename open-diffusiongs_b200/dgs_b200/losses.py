@@ -16,12 +16,18 @@ What runs where:
   kernels (`LossComputer(ssim_module=SsimLoss())`).  Every shipped yaml weights it 0: the reference evaluates it anyway
   and multiplies by 0; here the term is skipped unless a module is supplied, and `combine` refuses a non-zero lambda_ssim
   without one.
-* pointsdist (lambda 0 in every shipped yaml): skipped unless `compute_pointsdist=True`.
-* l2_xyz: plain device ops (a masked MSE over img_aligned_xyz, losses.py:286-291).
+* pointsdist (diffusionGS_rel.yaml weights it 1 for global steps 0-149, then 0; the other shipped yamls 0): skipped unless
+  `compute_pointsdist=True`.  On CUDA tensors it runs on `dgs_b200.geometry_loss` (dgs_geometry_loss_forward /
+  _backward), with its gradient flowing into img_aligned_xyz and, through the DiT backward, into the model.
+* l2_xyz (lambda_xyz 0.025 from step 151 in diffusionGS_rel.yaml, from step 0 in diffusionGS_rel_512.yaml): the masked
+  MSE over img_aligned_xyz (losses.py:286-291), on the same kernels as pointsdist for CUDA tensors.
+On CPU tensors both geometry terms are the reference's torch expressions.
 """
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
+
+from .geometry_loss import geometry_losses
 
 
 def C(value, epoch: int = 0, global_step: int = 0) -> float:
@@ -64,10 +70,6 @@ class LossComputer(nn.Module):
         if l2_loss is None:
             per_el = F.mse_loss(rendering, target, reduction="none").reshape(b, v, -1, h, w)
             l2_loss = per_el.mean(dim=(1, 2, 3, 4))  # losses.py:279-281
-        if img_aligned_xyz is not None and gt_img_aligned_xyz is not None:
-            l2_loss_xyz = F.mse_loss(img_aligned_xyz * masks, gt_img_aligned_xyz * masks, reduction="sum") / masks.sum()
-        else:
-            l2_loss_xyz = torch.zeros_like(l2_loss)
         if self.lpips_loss_module is not None:
             lp = self.lpips_loss_module(F.interpolate(rendering, size=[256, 256], mode="bilinear") * 2.0 - 1.0,
                                         F.interpolate(target, size=[256, 256], mode="bilinear") * 2.0 - 1.0)
@@ -78,13 +80,24 @@ class LossComputer(nn.Module):
             ssim_loss = self.ssim_loss_module(rendering, target).reshape(b, v).mean(dim=1)  # losses.py:314-318
         else:
             ssim_loss = torch.zeros(b, device=rendering.device)
-        if self.compute_pointsdist and img_aligned_xyz is not None:
-            trgt_mean = torch.norm(ray_o, dim=2, p=2, keepdim=True)  # losses.py:323-358
-            dist = (img_aligned_xyz - ray_o).norm(dim=2, p=2, keepdim=True)
-            dd = dist.detach()
-            trgt = (dd - dd.mean(dim=(2, 3, 4), keepdim=True)) / (dd.std(dim=(2, 3, 4), keepdim=True) + 1e-8) * 0.5 + trgt_mean
-            pointsdist_loss = ((dist - trgt) ** 2).mean(dim=(1, 2, 3, 4))
+        want_xyz = img_aligned_xyz is not None and gt_img_aligned_xyz is not None
+        want_pd = self.compute_pointsdist and img_aligned_xyz is not None
+        pointsdist_loss = l2_loss_xyz = None
+        if img_aligned_xyz is not None and img_aligned_xyz.is_cuda:  # both terms from one pass of the geometry kernels
+            pointsdist_loss, l2_loss_xyz = geometry_losses(img_aligned_xyz, ray_o, gt_img_aligned_xyz if want_xyz else None,
+                                                           masks if want_xyz else None, pointsdist=want_pd)
         else:
+            if want_xyz:  # losses.py:286-291
+                l2_loss_xyz = F.mse_loss(img_aligned_xyz * masks, gt_img_aligned_xyz * masks, reduction="sum") / masks.sum()
+            if want_pd:  # losses.py:323-358
+                trgt_mean = torch.norm(ray_o, dim=2, p=2, keepdim=True)
+                dist = (img_aligned_xyz - ray_o).norm(dim=2, p=2, keepdim=True)
+                dd = dist.detach()
+                trgt = (dd - dd.mean(dim=(2, 3, 4), keepdim=True)) / (dd.std(dim=(2, 3, 4), keepdim=True) + 1e-8) * 0.5 + trgt_mean
+                pointsdist_loss = ((dist - trgt) ** 2).mean(dim=(1, 2, 3, 4))
+        if l2_loss_xyz is None:
+            l2_loss_xyz = torch.zeros_like(l2_loss)
+        if pointsdist_loss is None:
             pointsdist_loss = torch.zeros(b, device=rendering.device)
         return l2_loss, lpips_loss, ssim_loss, pointsdist_loss, l2_loss_xyz
 
@@ -103,7 +116,8 @@ class LossComputer(nn.Module):
                 if name == "loss_ssim" and self.ssim_loss_module is None:
                     raise RuntimeError("lambda_ssim != 0 but no SSIM module was supplied")
                 if name == "loss_pointsdist" and not self.compute_pointsdist:
-                    raise RuntimeError("lambda_pointsdist != 0 needs LossComputer(compute_pointsdist=True)")
+                    raise RuntimeError("lambda_pointsdist != 0 needs LossComputer(compute_pointsdist=True) "
+                                       "(diffusionGS_rel.yaml weights it 1 for global steps 0-149)")
                 total = total + value * lam
         out["loss"] = total
         return out

@@ -388,11 +388,11 @@ class _DitFunction(torch.autograd.Function):
             tr._pending = False
             raise
         ctx.model, ctx.keep = model, keep
-        ctx.mark_non_differentiable(img_xyz)
+        ctx.set_materialize_grads(False)  # an unused output arrives as None: zeros below, NULL for img_xyz
         return out.xyz, out.features, out.scaling, out.rotation, out.opacity, img_xyz
 
     @staticmethod
-    def backward(ctx, d_xyz, d_features, d_scaling, d_rotation, d_opacity, _d_img):
+    def backward(ctx, d_xyz, d_features, d_scaling, d_rotation, d_opacity, d_img):
         model = ctx.model
         tr = model._trainer
         if ctx.keep is None or not tr._pending:
@@ -407,7 +407,9 @@ class _DitFunction(torch.autograd.Function):
         z = lambda g, *s: (torch.zeros(*s, device=dev) if g is None else g.float().contiguous())  # noqa: E731
         gs = [z(d_xyz, B, P, 3), z(d_features, B, P, n_sh, 3), z(d_scaling, B, P, 3), z(d_rotation, B, P, 4),
               z(d_opacity, B, P, 1)]
-        dout = DitOutGrads(*(g.data_ptr() for g in gs))
+        # d(img_aligned_xyz) (the geometry loss terms) is added to the image Gaussians' d xyz inside the backward
+        d_img = None if d_img is None else d_img.float().contiguous()
+        dout = DitOutGrads(*(g.data_ptr() for g in gs), None if d_img is None else d_img.data_ptr())
         opts = tr._bwd_opts()
         overlapped = opts is not None
         trace = tr._take_trace(B, V, H, W)
