@@ -475,8 +475,10 @@ int dgs_gemm_bf16(const void* A, const void* W, const float* bias, const float* 
                   int K, int epi, int ldc, int gate_stride, int rows_per_sample, void* stream);
 /* qkv [B,N,3,heads,64] bf16 -> out [B,N,heads*64] bf16 = softmax(q k^T / 8) v */
 int dgs_attention_fwd(const void* qkv, void* out, int B, int N, int heads, void* stream);
-/* training pair: the forward also writes lse2 [B, heads, round_up(N,128)] fp32; the backward turns (qkv, out, lse2,
- * dout [B,N,heads*64] bf16) into dqkv [B,N,3,heads,64] bf16; dsum = scratch of the lse2 size. */
+/* training pair: the forward also writes lse2 [B, heads, round_up(N,128)] fp32 (entries n < N only: the pads
+ * [N, round_up(N,128)) are left as they are); the backward turns (qkv, out, lse2, dout [B,N,heads*64] bf16) into
+ * dqkv [B,N,3,heads,64] bf16; dsum = scratch of the lse2 size.  The backward takes heads <= 64 (else
+ * DGS_ERR_INVALID_ARGUMENT) and, as a side effect, sets the lse2 pad entries to +inf and the dsum pad entries to 0. */
 int dgs_attention_fwd_train(const void* qkv, void* out, float* lse2, int B, int N, int heads, void* stream);
 int dgs_attention_bwd(const void* qkv, const void* out, const void* dout, float* lse2, float* dsum, void* dqkv, int B,
                       int N, int heads, void* stream);
