@@ -21,7 +21,7 @@
 extern "C" {
 #endif
 
-#define DGS_VERSION 100
+#define DGS_VERSION 101
 
 typedef enum {
   DGS_OK = 0,
@@ -137,28 +137,14 @@ typedef struct {
                            saved per-pixel state.  Same images, final_T, n_contrib and gradients either way. */
 } dgs_render_batch_args;
 
-int dgs_render_batch_forward(const dgs_render_batch_args* args, dgs_alloc_fn geom_alloc, void* geom_user,
-                             dgs_alloc_fn binning_alloc, void* binning_user, dgs_alloc_fn image_alloc,
-                             void* image_user, float* out_images, long long* num_rendered,
-                             long long* chunk_instances /* out [2]: instances binned in phase A / phase B */,
-                             void* stream);
-
-/* d_* are caller-allocated, same shapes as the inputs; they are fully overwritten.  scratch_alloc
- * provides the per-(view, Gaussian) screen-space gradient records (44 B each), free after the call. */
-int dgs_render_batch_backward(const dgs_render_batch_args* args, long long R,
-                              const long long* chunk_instances /* [2] from the forward */, const void* geom_buffer,
-                              const void* binning_buffer /* 1st binning_alloc result */,
-                              const void* binning_buffer_b /* 2nd (phase B) or NULL */, const void* image_buffer,
-                              const float* dL_dimages, float* d_xyz, float* d_features,
-                              float* d_scaling, float* d_rotation, float* d_opacity,
-                              dgs_alloc_fn scratch_alloc, void* scratch_user, void* stream);
-
-/* The same pair with the image-space MSE of the training loss fused in (LossComputer.forward's l2 term,
- * diffusionGS/utils/losses.py:261-284: l2_loss[b] = mean over (v,3,h,w) of (rendering - target)^2, later averaged over b and
- * weighted by lambda_diffusion, diffusion_gs_system.py:94-124).  Forward: the blend kernel adds sum (render - target)^2 of
- * sample b into loss_sum[b] (caller-zeroed, fp64) while the pixel is in registers.  Backward: the blend-backward kernel forms
+/* Optional fused terms of the pair below; either pointer may be NULL.
+ *
+ * mse: the image-space MSE of the training loss (LossComputer.forward's l2 term, diffusionGS/utils/losses.py:261-284:
+ * l2_loss[b] = mean over (v,3,h,w) of (rendering - target)^2, later averaged over b and weighted by lambda_diffusion,
+ * diffusion_gs_system.py:94-124).  Forward: the blend kernel adds sum (render - target)^2 of sample b into loss_sum[b]
+ * (caller-zeroed, fp64) while the pixel is in registers.  Backward: the blend-backward kernel forms
  * dL/dpix = dL_dimages (may be NULL) + coef[b] * (render - target) itself, with coef[b] = dL/dl2_loss[b] * 2 / (V*3*H*W)
- * computed by the caller on the device -- no per-element loss or gradient image exists.  mse == NULL: the plain pair. */
+ * computed by the caller on the device -- no per-element loss or gradient image exists. */
 typedef struct {
   const float* target;   /* [B,V,target_channels,H,W] fp32 in (0,1)                                       */
   int target_channels;   /* 3, or 4 = rgb + mask (the mask plane is skipped, losses.py:274-276)           */
@@ -166,40 +152,40 @@ typedef struct {
   const float* coef;     /* backward: in  [B] (device)                                                     */
   const float* images;   /* backward: in  the forward's out_images                                         */
 } dgs_render_mse;
-int dgs_render_batch_forward_mse(const dgs_render_batch_args* args, dgs_alloc_fn geom_alloc, void* geom_user,
-                                 dgs_alloc_fn binning_alloc, void* binning_user, dgs_alloc_fn image_alloc,
-                                 void* image_user, float* out_images, long long* num_rendered, long long* chunk_instances,
-                                 const dgs_render_mse* mse, void* stream);
-int dgs_render_batch_backward_mse(const dgs_render_batch_args* args, long long R, const long long* chunk_instances,
-                                  const void* geom_buffer, const void* binning_buffer, const void* binning_buffer_b,
-                                  const void* image_buffer, const float* dL_dimages, const dgs_render_mse* mse,
-                                  float* d_xyz, float* d_features, float* d_scaling, float* d_rotation, float* d_opacity,
-                                  dgs_alloc_fn scratch_alloc, void* scratch_user, void* stream);
 
-/* The same pair with per-pixel depth and alpha maps, from the blend the colour uses (same order, alpha >= 1/255 test, 0.99
- * clamp and T < 1e-4 stop; w_i = alpha_i T_i the colour's weight):
+/* aux: per-pixel depth and alpha maps, from the blend the colour uses (same order, alpha >= 1/255 test, 0.99 clamp and
+ * T < 1e-4 stop; w_i = alpha_i T_i the colour's weight):
  *   depth[b,v,0,y,x] = sum_i w_i z_i   (z_i the Gaussian's view-space depth; background 0: the ACCUMULATED depth,
  *                                       expected depth is depth / alpha)
  *   alpha[b,v,0,y,x] = 1 - final T     (accumulated opacity)
- * aux == NULL: exactly the _mse pair (mse may be NULL too; a fused MSE combines with aux).  The backward takes the upstream
- * gradients of either map (either may be NULL); with neither it runs the plain kernels, otherwise its scratch records grow
- * to 48 B per (view, Gaussian).  Images, final_T, n_contrib and loss_sum do not depend on aux. */
+ * The backward takes the upstream gradients of either map (either may be NULL); with neither it runs the plain kernels,
+ * otherwise its scratch records grow to 48 B per (view, Gaussian).  Images, final_T, n_contrib and loss_sum do not
+ * depend on aux. */
 typedef struct {
   float* depth;             /* forward out [B,V,1,H,W], required when aux != NULL */
   float* alpha;             /* forward out [B,V,1,H,W], required when aux != NULL */
   const float* dL_ddepth;   /* backward in [B,V,1,H,W], or NULL */
   const float* dL_dalpha;   /* backward in [B,V,1,H,W], or NULL */
 } dgs_render_aux;
-int dgs_render_batch_forward_aux(const dgs_render_batch_args* args, dgs_alloc_fn geom_alloc, void* geom_user,
-                                 dgs_alloc_fn binning_alloc, void* binning_user, dgs_alloc_fn image_alloc,
-                                 void* image_user, float* out_images, long long* num_rendered, long long* chunk_instances,
-                                 const dgs_render_mse* mse, const dgs_render_aux* aux, void* stream);
-int dgs_render_batch_backward_aux(const dgs_render_batch_args* args, long long R, const long long* chunk_instances,
-                                  const void* geom_buffer, const void* binning_buffer, const void* binning_buffer_b,
-                                  const void* image_buffer, const float* dL_dimages, const dgs_render_mse* mse,
-                                  const dgs_render_aux* aux, float* d_xyz, float* d_features, float* d_scaling,
-                                  float* d_rotation, float* d_opacity, dgs_alloc_fn scratch_alloc, void* scratch_user,
-                                  void* stream);
+
+/* Forward: the three arenas come from the callbacks and must be handed back to the backward.  *num_rendered receives the
+ * instance count R.  mse and aux may be NULL (the plain render); a fused MSE combines with aux. */
+int dgs_render_batch_forward(const dgs_render_batch_args* args, dgs_alloc_fn geom_alloc, void* geom_user,
+                             dgs_alloc_fn binning_alloc, void* binning_user, dgs_alloc_fn image_alloc,
+                             void* image_user, float* out_images, long long* num_rendered,
+                             long long* chunk_instances /* out [2]: instances binned in phase A / phase B */,
+                             const dgs_render_mse* mse, const dgs_render_aux* aux, void* stream);
+
+/* Backward: d_* are caller-allocated, same shapes as the inputs; they are fully overwritten.  scratch_alloc provides the
+ * per-(view, Gaussian) screen-space gradient records (44 B each), free after the call.  Some upstream gradient must be
+ * present: dL_dimages, mse (coef) or an aux map gradient; dL_dimages may be NULL when another is. */
+int dgs_render_batch_backward(const dgs_render_batch_args* args, long long R,
+                              const long long* chunk_instances /* [2] from the forward */, const void* geom_buffer,
+                              const void* binning_buffer /* 1st binning_alloc result */,
+                              const void* binning_buffer_b /* 2nd (phase B) or NULL */, const void* image_buffer,
+                              const float* dL_dimages, const dgs_render_mse* mse, const dgs_render_aux* aux,
+                              float* d_xyz, float* d_features, float* d_scaling, float* d_rotation, float* d_opacity,
+                              dgs_alloc_fn scratch_alloc, void* scratch_user, void* stream);
 
 /* Introspection used by the parity tests: copies of per-(view, Gaussian) / per-pixel forward state
  * out of the opaque arenas into caller DEVICE buffers (any may be NULL):

@@ -1970,23 +1970,7 @@ static Problem batch_problem(const dgs_render_batch_args* a) {
 int dgs_render_batch_forward(const dgs_render_batch_args* a, dgs_alloc_fn geom_alloc, void* geom_user,
                              dgs_alloc_fn bin_alloc, void* bin_user, dgs_alloc_fn img_alloc, void* img_user,
                              float* out_images, long long* num_rendered, long long* chunk_instances,
-                             void* stream) {
-  return dgs_render_batch_forward_mse(a, geom_alloc, geom_user, bin_alloc, bin_user, img_alloc, img_user, out_images,
-                                      num_rendered, chunk_instances, nullptr, stream);
-}
-
-int dgs_render_batch_forward_mse(const dgs_render_batch_args* a, dgs_alloc_fn geom_alloc, void* geom_user,
-                                 dgs_alloc_fn bin_alloc, void* bin_user, dgs_alloc_fn img_alloc, void* img_user,
-                                 float* out_images, long long* num_rendered, long long* chunk_instances,
-                                 const dgs_render_mse* mse, void* stream) {
-  return dgs_render_batch_forward_aux(a, geom_alloc, geom_user, bin_alloc, bin_user, img_alloc, img_user, out_images,
-                                      num_rendered, chunk_instances, mse, nullptr, stream);
-}
-
-int dgs_render_batch_forward_aux(const dgs_render_batch_args* a, dgs_alloc_fn geom_alloc, void* geom_user,
-                                 dgs_alloc_fn bin_alloc, void* bin_user, dgs_alloc_fn img_alloc, void* img_user,
-                                 float* out_images, long long* num_rendered, long long* chunk_instances,
-                                 const dgs_render_mse* mse, const dgs_render_aux* aux, void* stream) {
+                             const dgs_render_mse* mse, const dgs_render_aux* aux, void* stream) {
   int rc = check_batch_args(a);
   if (rc) return rc;
   DGS_REQUIRE(geom_alloc && bin_alloc && img_alloc && out_images && num_rendered && chunk_instances,
@@ -2012,31 +1996,10 @@ int dgs_render_batch_forward_aux(const dgs_render_batch_args* a, dgs_alloc_fn ge
 
 int dgs_render_batch_backward(const dgs_render_batch_args* a, long long R, const long long* chunk_instances,
                               const void* geom_buffer, const void* binning_buffer, const void* binning_buffer_b,
-                              const void* image_buffer, const float* dL_dimages,
-                              float* d_xyz, float* d_features, float* d_scaling, float* d_rotation,
-                              float* d_opacity, dgs_alloc_fn scratch_alloc, void* scratch_user, void* stream) {
-  DGS_REQUIRE(dL_dimages, "NULL state buffer");
-  return dgs_render_batch_backward_mse(a, R, chunk_instances, geom_buffer, binning_buffer, binning_buffer_b, image_buffer,
-                                       dL_dimages, nullptr, d_xyz, d_features, d_scaling, d_rotation, d_opacity,
-                                       scratch_alloc, scratch_user, stream);
-}
-
-int dgs_render_batch_backward_mse(const dgs_render_batch_args* a, long long R, const long long* chunk_instances,
-                                  const void* geom_buffer, const void* binning_buffer, const void* binning_buffer_b,
-                                  const void* image_buffer, const float* dL_dimages, const dgs_render_mse* mse,
-                                  float* d_xyz, float* d_features, float* d_scaling, float* d_rotation,
-                                  float* d_opacity, dgs_alloc_fn scratch_alloc, void* scratch_user, void* stream) {
-  return dgs_render_batch_backward_aux(a, R, chunk_instances, geom_buffer, binning_buffer, binning_buffer_b, image_buffer,
-                                       dL_dimages, mse, nullptr, d_xyz, d_features, d_scaling, d_rotation, d_opacity,
-                                       scratch_alloc, scratch_user, stream);
-}
-
-int dgs_render_batch_backward_aux(const dgs_render_batch_args* a, long long R, const long long* chunk_instances,
-                                  const void* geom_buffer, const void* binning_buffer, const void* binning_buffer_b,
-                                  const void* image_buffer, const float* dL_dimages, const dgs_render_mse* mse,
-                                  const dgs_render_aux* aux, float* d_xyz, float* d_features, float* d_scaling,
-                                  float* d_rotation, float* d_opacity, dgs_alloc_fn scratch_alloc, void* scratch_user,
-                                  void* stream) {
+                              const void* image_buffer, const float* dL_dimages, const dgs_render_mse* mse,
+                              const dgs_render_aux* aux, float* d_xyz, float* d_features, float* d_scaling,
+                              float* d_rotation, float* d_opacity, dgs_alloc_fn scratch_alloc, void* scratch_user,
+                              void* stream) {
   int rc = check_batch_args(a);
   if (rc) return rc;
   const bool has_aux = aux && (aux->dL_ddepth || aux->dL_dalpha);  // no aux gradient: the plain kernels

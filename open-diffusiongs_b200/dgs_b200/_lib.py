@@ -1,11 +1,16 @@
-"""ctypes binding of libdgs_b200.so (include/dgs_b200.h).  There is NO fallback: if the CUDA
-library is missing, importing any compute entry point raises."""
+"""ctypes binding of libdgs_b200.so (include/dgs_b200.h) and the torch-side helpers every wrapper module passes
+through it (stream, ptr, f32, Alloc).  There is NO fallback: if the CUDA library is missing, importing any compute entry
+point raises."""
 import ctypes as C
 import os
+import sys
+
+import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libdgs_b200.so")
 
+DGS_VERSION = 101  # the DGS_VERSION of include/dgs_b200.h whose signatures the argtypes below describe
 ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_size_t, C.c_void_p)
 
 
@@ -113,8 +118,13 @@ def lib():
                 f"libdgs_b200.so not found at {LIB_PATH}: build it with "
                 "`python open-diffusiongs_b200/csrc/build.py` (there is no CPU/PyTorch fallback)")
         L = C.CDLL(LIB_PATH)
-        L.dgs_last_error.restype = C.c_char_p
         L.dgs_version.restype = C.c_int
+        if L.dgs_version() != DGS_VERSION:
+            # calling through these argtypes would pass wrong arguments to any entry point whose signature changed
+            raise DgsError(
+                f"{LIB_PATH} is libdgs_b200 version {L.dgs_version()}, these bindings are version {DGS_VERSION}: "
+                "rebuild it with `python open-diffusiongs_b200/csrc/build.py --force`")
+        L.dgs_last_error.restype = C.c_char_p
         L.dgs_kernel_launch_count.restype = C.c_ulonglong
         L.dgs_profile_read.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
         for name in ("dgs_raster_geom_bytes", "dgs_raster_binning_bytes", "dgs_raster_image_bytes"):
@@ -127,10 +137,11 @@ def lib():
                                          vp, vp, C.POINTER(C.c_int), vp]
         L.dgs_raster_backward.argtypes = [C.POINTER(RasterArgs), C.c_int] + [vp] * 15
         L.dgs_mark_visible.argtypes = [C.c_int, vp, vp, vp, vp, vp]
-        L.dgs_render_batch_forward.argtypes = [C.POINTER(RenderBatchArgs), ALLOC_FN, vp, ALLOC_FN, vp,
-                                               ALLOC_FN, vp, vp, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong), vp]
+        L.dgs_render_batch_forward.argtypes = [C.POINTER(RenderBatchArgs), ALLOC_FN, vp, ALLOC_FN, vp, ALLOC_FN, vp, vp,
+                                               C.POINTER(C.c_longlong), C.POINTER(C.c_longlong), C.POINTER(RenderMse),
+                                               C.POINTER(RenderAux), vp]
         L.dgs_render_batch_backward.argtypes = [C.POINTER(RenderBatchArgs), C.c_longlong, C.POINTER(C.c_longlong)] + \
-            [vp] * 10 + [ALLOC_FN, vp, vp]
+            [vp] * 5 + [C.POINTER(RenderMse), C.POINTER(RenderAux)] + [vp] * 5 + [ALLOC_FN, vp, vp]
         L.dgs_raster_export_state.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_longlong] + [vp] * 13
         L.dgs_dit_workspace_bytes.restype = C.c_size_t
         L.dgs_dit_workspace_bytes.argtypes = [C.POINTER(DitWeights), C.c_int, C.c_int, C.c_int, C.c_int]
@@ -155,16 +166,6 @@ def lib():
         L.dgs_stream_wait_event.argtypes = [vp, vp]
         L.dgs_adamw_ema_step.argtypes = [vp, vp, vp, vp, vp, C.c_size_t] + [C.c_float] * 5 + [C.c_int, C.c_float, vp,
                                                                                                C.c_float, vp]
-        L.dgs_render_batch_forward_mse.argtypes = [C.POINTER(RenderBatchArgs), ALLOC_FN, vp, ALLOC_FN, vp, ALLOC_FN, vp, vp,
-                                                   C.POINTER(C.c_longlong), C.POINTER(C.c_longlong),
-                                                   C.POINTER(RenderMse), vp]
-        L.dgs_render_batch_backward_mse.argtypes = [C.POINTER(RenderBatchArgs), C.c_longlong, C.POINTER(C.c_longlong)] + \
-            [vp] * 5 + [C.POINTER(RenderMse)] + [vp] * 5 + [ALLOC_FN, vp, vp]
-        L.dgs_render_batch_forward_aux.argtypes = [C.POINTER(RenderBatchArgs), ALLOC_FN, vp, ALLOC_FN, vp, ALLOC_FN, vp, vp,
-                                                   C.POINTER(C.c_longlong), C.POINTER(C.c_longlong),
-                                                   C.POINTER(RenderMse), C.POINTER(RenderAux), vp]
-        L.dgs_render_batch_backward_aux.argtypes = [C.POINTER(RenderBatchArgs), C.c_longlong, C.POINTER(C.c_longlong)] + \
-            [vp] * 5 + [C.POINTER(RenderMse), C.POINTER(RenderAux)] + [vp] * 5 + [ALLOC_FN, vp, vp]
         L.dgs_transpose_bf16.argtypes = [vp, C.c_int, C.c_int, C.c_int, vp, vp, vp]
         L.dgs_adamw_step.argtypes = [vp, vp, vp, vp, C.c_size_t] + [C.c_float] * 5 + [C.c_int, C.c_float, vp, vp]
         L.dgs_cast_transpose_f32.argtypes = [vp, C.c_longlong, C.c_int, C.c_int, C.c_int, vp, vp, vp]
@@ -242,6 +243,53 @@ def check(rc):
         raise DgsError(f"libdgs_b200 status {rc}: {lib().dgs_last_error().decode()}")
 
 
+def stream(dev):
+    """The current torch stream of `dev`, as the void* every entry point takes."""
+    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+
+
+def ptr(t):
+    """Device pointer of `t`; None or an empty tensor is NULL, the C ABI's "not provided"."""
+    return None if t is None or t.numel() == 0 else t.data_ptr()
+
+
+def f32(t):
+    """`t` as a detached, contiguous fp32 tensor, the element type the kernels read (None stays None)."""
+    return None if t is None else t.detach().to(torch.float32).contiguous()
+
+
+class Alloc:
+    """dgs_alloc_fn backed by torch uint8 tensors (the reference's resizeFunctional, rasterize_points.cu:27-33).
+
+    With a `cache` dict, request i is served from the grow-only buffer cache[(key, i)] when i is below `cached` (every
+    request when `cached` is None), so repeated calls do no allocator traffic; other requests get a fresh tensor, e.g.
+    outputs the caller keeps.  `tensors` holds every buffer handed out, in request order, and `tensor` the last one."""
+
+    def __init__(self, device, cache=None, key=None, cached=None):
+        self.device, self.cache, self.key, self.cached = device, cache, key, cached
+        self.tensor = torch.empty(0, dtype=torch.uint8, device=device)
+        self.tensors = []
+        self.cb = ALLOC_FN(self._alloc)
+
+    def _alloc(self, nbytes, _user):
+        try:
+            i = len(self.tensors)
+            if self.cache is not None and (self.cached is None or i < self.cached):
+                k = (self.key, i)
+                t = self.cache.get(k)
+                if t is None or t.numel() < nbytes or t.device != self.device:
+                    self.cache.pop(k, None)  # let the allocator reuse the old buffer for its successor
+                    t = self.cache[k] = torch.empty(int(nbytes * 1.25) + 256, dtype=torch.uint8, device=self.device)
+            else:
+                t = torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=self.device)
+            self.tensor = t
+            self.tensors.append(t)
+            return t.data_ptr()
+        except Exception as e:  # noqa: BLE001  (reported as DGS_ERR_ALLOC by the C side)
+            print(f"[dgs_b200] allocation of {nbytes} bytes failed: {e!r}"[:600], file=sys.stderr)
+            return None
+
+
 EXPORTED = [  # every symbol include/dgs_b200.h declares (checked by tests/test_abi.py)
     "dgs_version", "dgs_last_error", "dgs_kernel_launch_count", "dgs_profile_enable", "dgs_profile_read",
     "dgs_raster_geom_bytes", "dgs_raster_binning_bytes",
@@ -253,12 +301,12 @@ EXPORTED = [  # every symbol include/dgs_b200.h declares (checked by tests/test_
     "dgs_attention_bwd", "dgs_gemm_bf16_ex", "dgs_ln_modulate_bwd", "dgs_gate_bwd", "dgs_cast_transpose_f32", "dgs_gemm_bf16_tn",
     "dgs_gaussians_epilogue", "dgs_gaussians_epilogue_bwd",
     "dgs_dit_train_state_bytes_ex", "dgs_dit_backward_ex", "dgs_event_create", "dgs_event_destroy", "dgs_stream_wait_event",
-    "dgs_adamw_ema_step", "dgs_render_batch_forward_mse", "dgs_render_batch_backward_mse", "dgs_dit_export_state",
+    "dgs_adamw_ema_step", "dgs_dit_export_state",
     "dgs_dit_export_ends", "dgs_lpips_workspace_bytes", "dgs_lpips_state_bytes", "dgs_lpips_forward", "dgs_lpips_backward",
     "dgs_ssim_workspace_bytes", "dgs_ssim_state_bytes", "dgs_ssim_forward", "dgs_ssim_backward",
     "dgs_geometry_loss_workspace_bytes", "dgs_geometry_loss_forward", "dgs_geometry_loss_backward",
     "dgs_dit_workspace_bytes_fp8", "dgs_dit_forward_fp8", "dgs_quantize_rows_e4m3", "dgs_ln_modulate_fp8", "dgs_gemm_fp8",
-    "dgs_mesh_field", "dgs_marching_cubes", "dgs_render_batch_forward_aux", "dgs_render_batch_backward_aux",
+    "dgs_mesh_field", "dgs_marching_cubes",
     "dgs_dit_workspace_bytes_fp8_ex", "dgs_dit_forward_fp8_ex", "dgs_attention_quantize_e4m3", "dgs_attention_fwd_fp8",
     "dgs_mesh_decimate",
 ]

@@ -15,7 +15,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from ._lib import DitIO, DitWeights, DitWeightsFp8, check
+from ._lib import DitIO, DitWeights, DitWeightsFp8, check, f32, stream
 from .renderer import Renderer
 
 _REGISTRY = {}
@@ -176,7 +176,6 @@ class DGSDenoiser(nn.Module):
             lo = (t - hi.float()).to(torch.bfloat16)
             return torch.cat([hi, hi, lo], dim=1).contiguous()
 
-        f32 = lambda t: t.detach().float().contiguous()  # noqa: E731
         T = self.transformer
         stack = lambda get: torch.stack([get(b).detach() for b in T])  # noqa: E731
         heads = (self.upsampler, self.image_token_decoder)
@@ -220,7 +219,7 @@ class DGSDenoiser(nn.Module):
         if self._packed_fp8 is not None and self._packed_fp8_key == key:
             return self._packed_fp8
         L = _lib.lib()
-        stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        st = stream(self.device)
         w8, t = DitWeightsFp8(), {}
         for name, get in (("qkv", lambda b: b.attn.qkv.weight), ("fc1", lambda b: b.mlp.fc1.weight),
                           ("fc2", lambda b: b.mlp.fc2.weight)):
@@ -228,7 +227,7 @@ class DGSDenoiser(nn.Module):
             n_layers, n, k = src.shape
             q = torch.empty(n_layers, n, k, dtype=torch.uint8, device=src.device)
             s = torch.empty(n_layers, n, dtype=torch.float32, device=src.device)
-            check(L.dgs_quantize_rows_e4m3(src.data_ptr(), n_layers * n, k, q.data_ptr(), s.data_ptr(), stream))
+            check(L.dgs_quantize_rows_e4m3(src.data_ptr(), n_layers * n, k, q.data_ptr(), s.data_ptr(), st))
             t[name + "_w"], t[name + "_s"] = q, s
             setattr(w8, name + "_w", q.data_ptr())
             setattr(w8, name + "_s", s.data_ptr())
@@ -321,12 +320,12 @@ class DGSDenoiser(nn.Module):
                        rotation=out.rotation.data_ptr(), opacity=out.opacity.data_ptr(),
                        img_aligned_xyz=img_xyz.data_ptr(), tokens_out=None if tokens is None else tokens.data_ptr(),
                        train_state=None if train_state is None else train_state.data_ptr(), train_mode=int(train_mode))
-            stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            st = stream(dev)
             if fp8:
                 w8, _keep8 = self.packed_weights_fp8()
-                check(L.dgs_dit_forward_fp8_ex(C.byref(w), C.byref(w8), C.byref(io), flags, ws.data_ptr(), nbytes, stream))
+                check(L.dgs_dit_forward_fp8_ex(C.byref(w), C.byref(w8), C.byref(io), flags, ws.data_ptr(), nbytes, st))
             else:
-                check(L.dgs_dit_forward(C.byref(w), C.byref(io), ws.data_ptr(), nbytes, stream))
+                check(L.dgs_dit_forward(C.byref(w), C.byref(io), ws.data_ptr(), nbytes, st))
         keep = (io, ws, nbytes, images, ray_o, ray_d, tf, w, _keep)  # what a later dgs_dit_backward needs alive
         return out, img_xyz, tokens, keep
 

@@ -4,14 +4,13 @@
 and `transform_input(image, c2w, fxfycxcy)` (reference `TransformInput`, diffusionGS/systems/utils.py:621-757).
 The arithmetic on tensors runs in libdgs_b200.so; the (tiny, one-off) schedule tables are built in fp64 numpy exactly
 as the reference does and uploaded ONCE per device."""
-import ctypes as C
 import math
 
 import numpy as np
 import torch
 
 from . import _lib
-from ._lib import check
+from ._lib import check, stream
 
 
 def _betas_squaredcos_cap_v2(n, max_beta=0.999):  # gaussian_diffusion.py:139-167
@@ -35,10 +34,6 @@ def _space_timesteps(n, section_counts):  # respace.py:16-66 (the "ddimN" string
             cur += stride
         start += size
     return set(out)
-
-
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
 class GaussianDiffusionB200:
@@ -91,7 +86,7 @@ class GaussianDiffusionB200:
         with torch.cuda.device(x.device):
             check(_lib.lib().dgs_q_sample(x.data_ptr(), n.data_ptr(), tab["sqrt_alphas_cumprod"].data_ptr(),
                                           tab["sqrt_one_minus_alphas_cumprod"].data_ptr(), tt.data_ptr(), x.shape[0],
-                                          x[0].numel(), out.data_ptr(), _stream(x.device)))
+                                          x[0].numel(), out.data_ptr(), stream(x.device)))
         return out
 
     def p_sample_step(self, pred_xstart, x_t, t, noise=None):
@@ -106,7 +101,7 @@ class GaussianDiffusionB200:
                                                tab["posterior_mean_coef1"].data_ptr(),
                                                tab["posterior_mean_coef2"].data_ptr(),
                                                tab["model_log_variance"].data_ptr(), tt.data_ptr(), x.shape[0],
-                                               x[0].numel(), out.data_ptr(), _stream(x.device)))
+                                               x[0].numel(), out.data_ptr(), stream(x.device)))
         return out
 
 
@@ -204,5 +199,5 @@ def transform_input(image, c2w, fxfycxcy, patch_size=None):
     ray_d = torch.empty_like(ray_o)
     with torch.cuda.device(dev):
         check(_lib.lib().dgs_rays_from_cameras(m.data_ptr(), f.data_ptr(), b * v, h, w, ray_o.data_ptr(), ray_d.data_ptr(),
-                                               _stream(dev)))
+                                               stream(dev)))
     return ray_o, ray_d

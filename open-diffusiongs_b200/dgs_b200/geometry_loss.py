@@ -6,24 +6,10 @@ pointsdist and l2_loss_xyz (diffusionGS/utils/losses.py:286-291, 323-364) over t
 Both are differentiable in img_aligned_xyz only (the reference detaches the pointsdist target; ray_o, the ground truth
 and the masks are data).  LossComputer.forward uses this on CUDA tensors.
 """
-import ctypes as C
-
 import torch
 
 from . import _lib
-from ._lib import check
-
-
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-
-
-def _f32(t):
-    return None if t is None else t.detach().to(torch.float32).contiguous()
-
-
-def _ptr(t):
-    return None if t is None else t.data_ptr()
+from ._lib import check, f32, ptr, stream
 
 
 class _GeometryLossFunction(torch.autograd.Function):
@@ -31,16 +17,16 @@ class _GeometryLossFunction(torch.autograd.Function):
     def forward(ctx, img_xyz, ray_o, gt_xyz, masks, want_pd, want_xyz):
         B, V, _, H, W = img_xyz.shape
         dev = img_xyz.device
-        img, o, gt, m = _f32(img_xyz), _f32(ray_o), _f32(gt_xyz), _f32(masks)
+        img, o, gt, m = f32(img_xyz), f32(ray_o), f32(gt_xyz), f32(masks)
         L = _lib.lib()
         pd = torch.empty(B, dtype=torch.float32, device=dev) if want_pd else torch.zeros(B, device=dev)
         l2 = torch.empty((), dtype=torch.float32, device=dev) if want_xyz else torch.zeros((), device=dev)
         state = torch.empty(2 * B * V + 1, dtype=torch.float32, device=dev)
         ws = torch.empty(L.dgs_geometry_loss_workspace_bytes(B, V), dtype=torch.uint8, device=dev)
         with torch.cuda.device(dev):
-            check(L.dgs_geometry_loss_forward(B, V, H, W, img.data_ptr(), _ptr(o), _ptr(gt), _ptr(m),
+            check(L.dgs_geometry_loss_forward(B, V, H, W, img.data_ptr(), ptr(o), ptr(gt), ptr(m),
                                               pd.data_ptr() if want_pd else None, l2.data_ptr() if want_xyz else None,
-                                              state.data_ptr(), ws.data_ptr(), ws.numel(), _stream(dev)))
+                                              state.data_ptr(), ws.data_ptr(), ws.numel(), stream(dev)))
         if not want_pd:
             ctx.mark_non_differentiable(pd)
         if not want_xyz:
@@ -60,9 +46,9 @@ class _GeometryLossFunction(torch.autograd.Function):
         g_xyz = None if g_xyz is None else g_xyz.to(torch.float32).reshape(1).contiguous()
         d_img = torch.empty_like(img)
         with torch.cuda.device(img.device):
-            check(_lib.lib().dgs_geometry_loss_backward(B, V, H, W, img.data_ptr(), _ptr(o), _ptr(gt), _ptr(m),
-                                                        state.data_ptr(), _ptr(g_pd), _ptr(g_xyz), d_img.data_ptr(),
-                                                        _stream(img.device)))
+            check(_lib.lib().dgs_geometry_loss_backward(B, V, H, W, img.data_ptr(), ptr(o), ptr(gt), ptr(m),
+                                                        state.data_ptr(), ptr(g_pd), ptr(g_xyz), d_img.data_ptr(),
+                                                        stream(img.device)))
         return d_img.to(ctx.in_dtype), None, None, None, None, None
 
 

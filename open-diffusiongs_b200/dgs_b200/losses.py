@@ -5,7 +5,7 @@
 What runs where:
 * l2 (lambda_diffusion = 1): FUSED into the rasterizer -- `Renderer.forward_mse` returns the per-sample MSE out of the
   blend-forward kernel and the blend-backward kernel forms dL/dpix = lambda * 2 (c - gt) / n itself
-  (dgs_render_batch_forward_mse / _backward_mse).  `LossComputer.forward(..., l2_loss=...)` takes that value; without it
+  (dgs_render_batch_forward / _backward with a dgs_render_mse).  `LossComputer.forward(..., l2_loss=...)` takes that value; without it
   the l2 term is computed from the images with torch device ops (same numbers, the unfused form).
 * lpips (lambda_lpips 0.5 from step 151 in diffusionGS_rel.yaml, 0.1 in diffusionGS_scene.yaml): `dgs_b200.lpips.LPIPS`, the
   LPIPS-VGG16 distance on the library's kernels, with its weights read from the reference's checkpoints

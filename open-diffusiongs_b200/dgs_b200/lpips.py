@@ -13,7 +13,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from ._lib import LpipsWeights, check
+from ._lib import LpipsWeights, check, stream
 from .checkpoint import LPIPS_PREFIXES, lpips_state_dict
 
 CONV_INDEX = (0, 2, 5, 7, 10, 12, 14, 17, 19, 21, 24, 26, 28)   # torchvision vgg16().features indices of the 13 convs
@@ -127,7 +127,7 @@ class _LpipsFunction(torch.autograd.Function):
         state = torch.empty(L.dgs_lpips_state_bytes(n, H, W), dtype=torch.uint8, device=dev) if train else None
         ws = module.workspace(n, H, W, dev)
         check(L.dgs_lpips_forward(C.byref(w), n, H, W, in0.data_ptr(), in1.data_ptr(), out.data_ptr(),
-                                  state.data_ptr() if train else None, ws.data_ptr(), ws.numel(), _stream(dev)))
+                                  state.data_ptr() if train else None, ws.data_ptr(), ws.numel(), stream(dev)))
         if train:
             ctx.saved = (w, keep, state, module, (n, H, W), in_dtype)
         return out.view(n, 1, 1, 1)
@@ -140,13 +140,9 @@ class _LpipsFunction(torch.autograd.Function):
         d_in0 = torch.empty(n, 3, H, W, dtype=torch.float32, device=dev)
         ws = module.workspace(n, H, W, dev)
         check(_lib.lib().dgs_lpips_backward(C.byref(w), n, H, W, state.data_ptr(), d.data_ptr(), d_in0.data_ptr(),
-                                            ws.data_ptr(), ws.numel(), _stream(dev)))
+                                            ws.data_ptr(), ws.numel(), stream(dev)))
         ctx.saved = None
         return d_in0.to(in_dtype), None, None
-
-
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
 class LPIPS(nn.Module):

@@ -20,46 +20,9 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import ALLOC_FN, check
+from ._lib import Alloc, check, f32, stream
 
-_SCRATCH = {}  # grow-only scratch buffers, re-used across calls: {(device, slot): uint8 tensor}
-
-
-class _Alloc:
-    """dgs_alloc_fn: the first `cached` requests come from the grow-only scratch cache, later ones (outputs the caller
-    keeps) are fresh tensors."""
-
-    def __init__(self, device, name, cached):
-        self.device, self.name, self.cached = device, name, cached
-        self.tensors = []
-        self.cb = ALLOC_FN(self._alloc)
-
-    def _alloc(self, nbytes, _user):
-        try:
-            i = len(self.tensors)
-            if i < self.cached:
-                key = (str(self.device), self.name, i)
-                t = _SCRATCH.get(key)
-                if t is None or t.numel() < nbytes:
-                    _SCRATCH.pop(key, None)
-                    t = torch.empty(int(nbytes * 1.25) + 256, dtype=torch.uint8, device=self.device)
-                    _SCRATCH[key] = t
-            else:
-                t = torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=self.device)
-            self.tensors.append(t)
-            return t.data_ptr()
-        except Exception as e:  # noqa: BLE001  (reported as DGS_ERR_ALLOC by the C side)
-            import sys
-            print(f"[dgs_b200] mesh allocation of {nbytes} bytes failed: {e!r}"[:600], file=sys.stderr)
-            return None
-
-
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-
-
-def _f32(t):
-    return t.detach().to(torch.float32).contiguous()
+_SCRATCH = {}  # grow-only scratch buffers, re-used across calls: {((device, name), i): uint8 tensor}
 
 
 def opacity_field(xyz, scaling, rotation, opacity, scaling_modifier=None, resolution=128, num_blocks=16, relax_ratio=1.5,
@@ -72,7 +35,7 @@ def opacity_field(xyz, scaling, rotation, opacity, scaling_modifier=None, resolu
     if not xyz.is_cuda:
         raise _lib.DgsError("extract_fields needs CUDA tensors (no CPU path)")
     dev = xyz.device
-    xyz, scaling, rotation, opacity = (_f32(t) for t in (xyz, scaling, rotation, opacity))
+    xyz, scaling, rotation, opacity = (f32(t) for t in (xyz, scaling, rotation, opacity))
     P = xyz.shape[0]
     with torch.cuda.device(dev):
         if P > 0:
@@ -86,14 +49,14 @@ def opacity_field(xyz, scaling, rotation, opacity, scaling_modifier=None, resolu
         occ = torch.empty([resolution] * 3, dtype=torch.float32, device=dev)
         counts = torch.empty([nc] * 3, dtype=torch.int32, device=dev) if return_counts else None
         pairs = C.c_longlong(0)
-        alloc = _Alloc(dev, "field", 2)
+        alloc = Alloc(dev, _SCRATCH, (str(dev), "field"), cached=2)
         smod = 1.0 if scaling_modifier is None else float(scaling_modifier)
         # the reference multiplies fp32 tensors by these Python floats, i.e. by their fp32 roundings
         check(_lib.lib().dgs_mesh_field(P, xyz.data_ptr(), scaling.data_ptr(), rotation.data_ptr(), opacity.data_ptr(),
                                         float(np.float32(smod)), center.data_ptr(), float(np.float32(scale)), resolution,
                                         num_blocks, float(relax_ratio), lin.data_ptr(), occ.data_ptr(),
                                         counts.data_ptr() if return_counts else None, C.byref(pairs), alloc.cb, None,
-                                        _stream(dev)))
+                                        stream(dev)))
     if return_counts:
         return occ, center, scale, counts, pairs.value
     return occ, center, scale
@@ -107,13 +70,13 @@ def marching_cubes(field, iso):
     if field.dim() != 3:
         raise ValueError(f"marching_cubes: expected a 3-d field, got shape {tuple(field.shape)}")
     dev = field.device
-    f = _f32(field)
-    alloc = _Alloc(dev, "mc", 1)
+    f = f32(field)
+    alloc = Alloc(dev, _SCRATCH, (str(dev), "mc"), cached=1)
     vp, tp = C.c_void_p(), C.c_void_p()
     nv, nt = C.c_longlong(0), C.c_longlong(0)
     with torch.cuda.device(dev):
         check(_lib.lib().dgs_marching_cubes(f.data_ptr(), *f.shape, float(iso), alloc.cb, None, C.byref(vp), C.byref(tp),
-                                            C.byref(nv), C.byref(nt), _stream(dev)))
+                                            C.byref(nv), C.byref(nt), stream(dev)))
     V, F = nv.value, nt.value
     verts = alloc.tensors[1][:V * 12].view(torch.float32).view(V, 3) if V else torch.zeros(0, 3, device=dev)
     faces = alloc.tensors[2][:F * 12].view(torch.int32).view(F, 3) if F else torch.zeros(0, 3, dtype=torch.int32,
@@ -156,13 +119,13 @@ def decimate(vertices, faces, target_faces):
         dev = vertices.device
         v = vertices.detach().to(torch.float32).contiguous()
         f = faces.detach().to(torch.int32).contiguous()
-    alloc = _Alloc(dev, "decimate", 1)
+    alloc = Alloc(dev, _SCRATCH, (str(dev), "decimate"), cached=1)
     vp, fp = C.c_void_p(), C.c_void_p()
     nv, nf, rounds = C.c_longlong(0), C.c_longlong(0), C.c_int(0)
     with torch.cuda.device(dev):
         check(_lib.lib().dgs_mesh_decimate(v.data_ptr(), len(v), f.data_ptr(), len(f), int(target), alloc.cb, None,
                                            C.byref(vp), C.byref(fp), C.byref(nv), C.byref(nf), C.byref(rounds),
-                                           _stream(dev)))
+                                           stream(dev)))
     V, F = nv.value, nf.value
     ov = alloc.tensors[1][:V * 12].view(torch.float32).view(V, 3) if V else torch.zeros(0, 3, device=dev)
     of = alloc.tensors[2][:F * 12].view(torch.int32).view(F, 3).long() if F else torch.zeros(0, 3, dtype=torch.int64,

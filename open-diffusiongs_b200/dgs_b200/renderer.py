@@ -15,12 +15,21 @@ from . import raster as _raster
 
 
 class BatchedGaussianRender(torch.autograd.Function):
-    """Replaces DeferredGaussianRender (gs_core.py:949-1060); same inputs, same gradient outputs
-    (sum over views of d/d{xyz, features, scaling, rotation, opacity}, all w.r.t. the RAW tensors)."""
+    """Replaces DeferredGaussianRender (gs_core.py:949-1060): every (sample, view) pair in one launch set, with gradients
+    w.r.t. the RAW xyz, features, scaling, rotation and opacity, summed over views.  -> (images [b,v,3,H,W], l2_loss,
+    depth, alpha), where the last three are None unless asked for:
+    * target [b,v,3|4,H,W]: l2_loss [b] = mean over (v,3,h,w) of (images - target[:, :, :3])^2, the l2 term of
+      LossComputer.forward (diffusionGS/utils/losses.py:261-284).  The per-sample sums come out of the blend-forward
+      kernel and the backward forms the MSE part of dL/dpix inside the blend-backward kernel from (images, target,
+      dL/dl2_loss) -- no per-element loss or gradient image.
+    * buffers=True: depth [b,v,1,H,W] = sum_i w_i z_i (accumulated view-space depth) and alpha [b,v,1,H,W] = 1 - final T
+      of the same blend.
+    An output that receives no gradient costs nothing in the backward."""
 
     @staticmethod
-    def forward(ctx, xyz, features, scaling, rotation, opacity, height, width, C2W, fxfycxcy,
-                scaling_modifier=None, use_gssplat=False, arena_cache=None):
+    def forward(ctx, xyz, features, scaling, rotation, opacity, height, width, C2W, fxfycxcy, scaling_modifier=None,
+                arena_cache=None, target=None, buffers=False):
+        ctx.set_materialize_grads(False)
         needs_bwd = any(ctx.needs_input_grad[:5])
         # Arenas: the inference path re-uses ONE grow-only set (arena_cache["infer"]); a forward that will be
         # differentiated checks a set out of a pool and its backward returns it, so steady-state training does no
@@ -34,114 +43,43 @@ class BatchedGaussianRender(torch.autograd.Function):
             else:
                 cache = arena_cache.setdefault("infer", {})
         with torch.no_grad():
-            images, state = _raster.render_batch_forward(xyz, features, scaling, rotation, opacity, height, width,
-                                                         C2W, fxfycxcy, scaling_modifier, arena_cache=cache)
+            loss_sum = None if target is None else torch.zeros(C2W.shape[0], dtype=torch.float64, device=xyz.device)
+            images, *maps, state = _raster.render_batch_forward(xyz, features, scaling, rotation, opacity, height, width,
+                                                                C2W, fxfycxcy, scaling_modifier, arena_cache=cache,
+                                                                mse_target=target, mse_loss_sum=loss_sum, aux=buffers)
+            ctx.n = C2W.shape[1] * 3 * int(height) * int(width)
+            l2 = None if target is None else (loss_sum / ctx.n).float()
         ctx.state = state
         ctx.pool = (arena_cache, cache) if needs_bwd and arena_cache is not None else None
         ctx.in_dtypes = (xyz.dtype, features.dtype, scaling.dtype, rotation.dtype, opacity.dtype)
-        ctx.num_rendered = state["R"]
-        return images
+        return (images, l2, *(maps or (None, None)))
 
     @staticmethod
-    def backward(ctx, grad_output):
-        cache = ctx.pool[1] if ctx.pool else None
-        grads = _raster.render_batch_backward(ctx.state, grad_output, arena_cache=cache)
-        ctx.state = None  # release the arenas ...
-        if ctx.pool:      # ... back into the pool for the next step
-            ctx.pool[0]["pool"].append(cache)
-            ctx.pool = None
-        grads = tuple(g.to(dt) for g, dt in zip(grads, ctx.in_dtypes))
-        return (*grads, None, None, None, None, None, None, None)
-
-
-class BatchedGaussianRenderMSE(torch.autograd.Function):
-    """Render + the l2 term of LossComputer.forward (diffusionGS/utils/losses.py:261-284) as ONE node:
-    -> (images [b,v,3,H,W], l2_loss [b] = mean over (v,3,h,w) of (images - target[:, :, :3])^2).
-    The per-sample sums come out of the blend-forward kernel and the backward forms the MSE part of dL/dpix inside the
-    blend-backward kernel from (images, target, dL/dl2_loss) -- no per-element loss or gradient image."""
-
-    @staticmethod
-    def forward(ctx, xyz, features, scaling, rotation, opacity, height, width, C2W, fxfycxcy, target,
-                scaling_modifier=None, arena_cache=None):
-        ctx.set_materialize_grads(False)
-        needs_bwd = any(ctx.needs_input_grad[:5])
-        cache = None
-        if arena_cache is not None:
-            if needs_bwd:
-                pool = arena_cache.setdefault("pool", [])
-                cache = pool.pop() if pool else {}
-            else:
-                cache = arena_cache.setdefault("infer", {})
-        b, v = C2W.shape[0], C2W.shape[1]
-        with torch.no_grad():
-            loss_sum = torch.zeros(b, dtype=torch.float64, device=xyz.device)
-            images, state = _raster.render_batch_forward(xyz, features, scaling, rotation, opacity, height, width, C2W,
-                                                         fxfycxcy, scaling_modifier, arena_cache=cache,
-                                                         mse_target=target, mse_loss_sum=loss_sum)
-            n = v * 3 * int(height) * int(width)
-            l2 = (loss_sum / n).float()
-        ctx.state, ctx.n = state, n
-        ctx.pool = (arena_cache, cache) if needs_bwd and arena_cache is not None else None
-        ctx.in_dtypes = (xyz.dtype, features.dtype, scaling.dtype, rotation.dtype, opacity.dtype)
-        return images, l2
-
-    @staticmethod
-    def backward(ctx, g_images, g_l2):
-        cache = ctx.pool[1] if ctx.pool else None
-        if g_images is None and g_l2 is None:
-            raise RuntimeError("BatchedGaussianRenderMSE.backward without any upstream gradient")
-        coef = None if g_l2 is None else (g_l2.float() * (2.0 / ctx.n)).contiguous()
-        grads = _raster.render_batch_backward(ctx.state, g_images, arena_cache=cache, mse_coef=coef)
-        ctx.state = None
-        if ctx.pool:
-            ctx.pool[0]["pool"].append(cache)
-            ctx.pool = None
-        grads = tuple(g.to(dt) for g, dt in zip(grads, ctx.in_dtypes))
-        return (*grads, None, None, None, None, None, None, None)
-
-
-class BatchedGaussianRenderBuffers(torch.autograd.Function):
-    """BatchedGaussianRender plus the depth and alpha maps of the same blend -> (images [b,v,3,H,W],
-    depth [b,v,1,H,W] = sum_i w_i z_i (accumulated view-space depth), alpha [b,v,1,H,W] = 1 - final T).  An output that
-    receives no gradient costs nothing in the backward; with none of depth and alpha it is the plain backward."""
-
-    @staticmethod
-    def forward(ctx, xyz, features, scaling, rotation, opacity, height, width, C2W, fxfycxcy, scaling_modifier=None,
-                arena_cache=None):
-        ctx.set_materialize_grads(False)
-        needs_bwd = any(ctx.needs_input_grad[:5])
-        cache = None
-        if arena_cache is not None:
-            if needs_bwd:
-                pool = arena_cache.setdefault("pool", [])
-                cache = pool.pop() if pool else {}
-            else:
-                cache = arena_cache.setdefault("infer", {})
-        with torch.no_grad():
-            images, depth, alpha, state = _raster.render_batch_forward(xyz, features, scaling, rotation, opacity, height,
-                                                                       width, C2W, fxfycxcy, scaling_modifier,
-                                                                       arena_cache=cache, aux=True)
-        ctx.state = state
-        ctx.pool = (arena_cache, cache) if needs_bwd and arena_cache is not None else None
-        ctx.in_dtypes = (xyz.dtype, features.dtype, scaling.dtype, rotation.dtype, opacity.dtype)
-        return images, depth, alpha
-
-    @staticmethod
-    def backward(ctx, g_images, g_depth, g_alpha):
+    def backward(ctx, g_images, g_l2, g_depth, g_alpha):
         cache = ctx.pool[1] if ctx.pool else None
         grads = (None,) * 5
-        if g_images is not None or g_depth is not None or g_alpha is not None:
-            grads = _raster.render_batch_backward(ctx.state, g_images, arena_cache=cache, grad_depth=g_depth,
-                                                  grad_alpha=g_alpha)
-            grads = tuple(g.to(dt) for g, dt in zip(grads, ctx.in_dtypes))
-        ctx.state = None
-        if ctx.pool:
-            ctx.pool[0]["pool"].append(cache)
-            ctx.pool = None
-        return (*grads, None, None, None, None, None, None)
+        try:
+            if any(g is not None for g in (g_images, g_l2, g_depth, g_alpha)):
+                coef = None if g_l2 is None else (g_l2.float() * (2.0 / ctx.n)).contiguous()
+                grads = _raster.render_batch_backward(ctx.state, g_images, arena_cache=cache, mse_coef=coef,
+                                                      grad_depth=g_depth, grad_alpha=g_alpha)
+                grads = tuple(g.to(dt) for g, dt in zip(grads, ctx.in_dtypes))
+        finally:
+            ctx.state = None  # release the arenas ...
+            if ctx.pool:      # ... back into the pool for the next step
+                ctx.pool[0]["pool"].append(cache)
+                ctx.pool = None
+        return (*grads, None, None, None, None, None, None, None, None)
 
 
-batched_gaussian_render = BatchedGaussianRender.apply
+def batched_gaussian_render(xyz, features, scaling, rotation, opacity, height, width, C2W, fxfycxcy,
+                            scaling_modifier=None, use_gssplat=False, arena_cache=None):
+    """DeferredGaussianRender.apply's positional signature (gs_core.py:949-1064) -> images [b,v,3,H,W].  `use_gssplat`
+    is accepted for parity and unused: both reference branches compute the same images."""
+    return BatchedGaussianRender.apply(xyz, features, scaling, rotation, opacity, height, width, C2W, fxfycxcy,
+                                       scaling_modifier, arena_cache)[0]
+
+
 deferred_gaussian_render = batched_gaussian_render  # reference name (gs_core.py:1064)
 
 
@@ -415,9 +353,8 @@ class Renderer(nn.Module):
         C2W [b,v,4,4], fxfycxcy [b,v,4] -> [b,v,3,height,width] fp32.  `deferred` is accepted for
         signature parity: both reference branches compute the same images; here both map to the
         batched kernel set."""
-        out = batched_gaussian_render(xyz, features, scaling, rotation, opacity, height, width, C2W, fxfycxcy,
-                                      self.scaling_modifier, getattr(self.config, "use_gssplat", False),
-                                      self._arena_cache)
+        out = BatchedGaussianRender.apply(xyz, features, scaling, rotation, opacity, height, width, C2W, fxfycxcy,
+                                          self.scaling_modifier, self._arena_cache)[0]
         self.last_num_rendered = _raster.LAST_NUM_RENDERED
         return out
 
@@ -426,10 +363,10 @@ class Renderer(nn.Module):
         """forward() + the image-space MSE of the training loss in the same launch set:
         -> (renderings [b,v,3,H,W], l2_loss [b]) with l2_loss exactly LossComputer.forward's first output
         (losses.py:261-284; target [b,v,3|4,H,W], a 4th mask channel is ignored as there)."""
-        out = BatchedGaussianRenderMSE.apply(xyz, features, scaling, rotation, opacity, height, width, C2W, fxfycxcy, target,
-                                             self.scaling_modifier, self._arena_cache)
+        images, l2, _, _ = BatchedGaussianRender.apply(xyz, features, scaling, rotation, opacity, height, width, C2W,
+                                                       fxfycxcy, self.scaling_modifier, self._arena_cache, target)
         self.last_num_rendered = _raster.LAST_NUM_RENDERED
-        return out
+        return images, l2
 
     @torch.amp.custom_fwd(device_type="cuda", cast_inputs=torch.float32)
     def forward_buffers(self, xyz, features, scaling, rotation, opacity, height, width, C2W, fxfycxcy):
@@ -438,8 +375,9 @@ class Renderer(nn.Module):
         edict(render=..., depth=..., alpha=...).  depth = sum_i w_i z_i with w_i the colour's blend weight and z_i the
         Gaussian's view-space depth (background 0), the ACCUMULATED depth: expected depth is depth / alpha.
         alpha = 1 - final transmittance.  render equals forward()'s output bit for bit; all three are differentiable."""
-        render, depth, alpha = BatchedGaussianRenderBuffers.apply(xyz, features, scaling, rotation, opacity, height, width,
-                                                                  C2W, fxfycxcy, self.scaling_modifier, self._arena_cache)
+        render, _, depth, alpha = BatchedGaussianRender.apply(xyz, features, scaling, rotation, opacity, height, width,
+                                                              C2W, fxfycxcy, self.scaling_modifier, self._arena_cache,
+                                                              None, True)
         self.last_num_rendered = _raster.LAST_NUM_RENDERED
         return dict(render=render, depth=depth, alpha=alpha)
 

@@ -8,13 +8,12 @@ The window is the 11-tap Gaussian with sigma 1.5, filtered over the valid (H-10)
 least 11.  The gradient is taken w.r.t. the first input only.  `ssim_psnr` is the evaluation form (skimage's sample
 covariance, and PSNR from the same pass) that `dgs_b200.metrics` uses.
 """
-import ctypes as C
 
 import torch
 import torch.nn as nn
 
 from . import _lib
-from ._lib import check
+from ._lib import check, stream
 
 WIN_SIZE, WIN_SIGMA, K_DEFAULT = 11, 1.5, (0.01, 0.03)
 
@@ -35,10 +34,6 @@ def prepare_inputs(x, y):
     return x.to(torch.float32).contiguous(), y.to(torch.float32).contiguous()
 
 
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-
-
 def _forward(x, y, data_range, sample_covariance, want_psnr, train):
     """fp32 contiguous CUDA inputs -> (ssim [n], psnr [n] or None, state or None)"""
     n, _, H, W = x.shape
@@ -50,7 +45,7 @@ def _forward(x, y, data_range, sample_covariance, want_psnr, train):
     ws = torch.empty(L.dgs_ssim_workspace_bytes(n, H, W), dtype=torch.uint8, device=dev)
     check(L.dgs_ssim_forward(n, H, W, x.data_ptr(), y.data_ptr(), float(data_range), int(sample_covariance),
                              out.data_ptr(), psnr.data_ptr() if want_psnr else None,
-                             state.data_ptr() if train else None, ws.data_ptr(), ws.numel(), _stream(dev)))
+                             state.data_ptr() if train else None, ws.data_ptr(), ws.numel(), stream(dev)))
     return out, psnr, state
 
 
@@ -72,7 +67,7 @@ class _SsimFunction(torch.autograd.Function):
         d = dout.reshape(n).to(torch.float32).contiguous()
         d_x = torch.empty_like(x)
         check(_lib.lib().dgs_ssim_backward(n, H, W, x.data_ptr(), y.data_ptr(), state.data_ptr(), d.data_ptr(),
-                                           d_x.data_ptr(), _stream(x.device)))
+                                           d_x.data_ptr(), stream(x.device)))
         ctx.saved = None
         return d_x.to(in_dtype), None, None
 

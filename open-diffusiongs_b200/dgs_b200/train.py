@@ -15,13 +15,9 @@ import contextlib
 
 import torch.distributed as dist
 
-from ._lib import DitBwdOpts, DitGrads, DitOutGrads, DitWeightsT, check
+from ._lib import DitBwdOpts, DitGrads, DitOutGrads, DitWeightsT, check, stream
 from .denoiser import head_channels
 from .dist import GradArena, gradient_group
-
-
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
 class DitTrainer:
@@ -139,7 +135,7 @@ class DitTrainer:
             for k, get in self._BIG.items():
                 p0 = get(T[0])
                 check(L.dgs_cast_transpose_f32(p0.data_ptr(), stride, len(T), p0.shape[0], p0.shape[1], t[k].data_ptr(),
-                                               self._wT_keep[k + "T"].data_ptr(), _stream(dev)))
+                                               self._wT_keep[k + "T"].data_ptr(), stream(dev)))
         if not first:
             for k, v in m._pack_dict(skip=tuple(self._BIG) + ("sh_degree",)).items():
                 t[k].copy_(v)
@@ -189,7 +185,7 @@ class DitTrainer:
         args = [out[k].data_ptr() if k in out else None for k in self.STATE_FIELDS]
         with torch.cuda.device(dev):
             check(_lib.lib().dgs_dit_export_state(C.byref(w), B, V, H, W, self.train_mode, self._state.data_ptr(), int(layer),
-                                                  *args, _stream(dev)))
+                                                  *args, stream(dev)))
         return out
 
     ENDS_FIELDS = ("x_pre", "c", "mod", "gs_tok", "img_gs", "dx0", "dx_pre", "dmod", "dc", "d_gs_tok")
@@ -220,7 +216,7 @@ class DitTrainer:
         ws = self.model._workspace
         with torch.cuda.device(dev):
             check(_lib.lib().dgs_dit_export_ends(C.byref(w), B, V, H, W, self.train_mode, self._state.data_ptr(),
-                                                 ws.data_ptr(), ws.numel(), *args, _stream(dev)))
+                                                 ws.data_ptr(), ws.numel(), *args, stream(dev)))
         return out
 
     def trace_backward(self, names=_lib.BWD_TRACE_FIELDS):
@@ -338,7 +334,7 @@ class DitTrainer:
                                                 self.master.numel(), self.lr, self.betas[0], self.betas[1], self.eps,
                                                 self.weight_decay, self.steps, gscale,
                                                 None if scale is None else scale.data_ptr(),
-                                                0.0 if self.ema_decay is None else float(self.ema_decay), _stream(dev)))
+                                                0.0 if self.ema_decay is None else float(self.ema_decay), stream(dev)))
         if self._accum is not None:
             self._accum.zero_()
         self._micro = 0
@@ -419,7 +415,7 @@ class _DitFunction(torch.autograd.Function):
         with torch.cuda.device(dev):
             check(_lib.lib().dgs_dit_backward_ex(C.byref(w), C.byref(tr._wT), C.byref(io), C.byref(dout),
                                                  C.byref(tr._grads), None if opts is None else C.byref(opts),
-                                                 ws.data_ptr(), nbytes, _stream(dev)))
+                                                 ws.data_ptr(), nbytes, stream(dev)))
         ctx.keep = None
         tr._end_backward(overlapped=overlapped)
         # parameter gradients were written straight into the arena (p.grad views); nothing to hand to autograd

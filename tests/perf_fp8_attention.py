@@ -32,11 +32,6 @@ def card():
     return dict(gpu=name, power_limit=power, max_sm_clock=clock)
 
 
-def _stream():
-    import ctypes as C
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
 def _time(fn, iters):
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     a.record()
@@ -49,7 +44,7 @@ def _time(fn, iters):
 
 def kernels(N, windows, iters, H=16, B=1):
     from dgs_b200 import _lib
-    L, st = _lib.lib(), _stream()
+    L, st = _lib.lib(), _lib.stream(DEV)
     g = torch.Generator(DEV).manual_seed(0)
     qkv = (torch.randn(B, N, 3 * H * 64, device=DEV, generator=g) * 1.5).to(torch.bfloat16)
     out = torch.empty(B, N, H * 64, dtype=torch.bfloat16, device=DEV)

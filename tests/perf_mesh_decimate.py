@@ -29,11 +29,11 @@ from perf_mesh import NAMES, card, timed  # noqa: E402
 def rounds(v, f, target):
     """The round count of one call, through the C ABI"""
     from dgs_b200 import _lib, mesh
-    alloc = mesh._Alloc(v.device, "decimate", 1)
+    alloc = _lib.Alloc(v.device, mesh._SCRATCH, (str(v.device), "decimate"), cached=1)
     out = [C.c_void_p(), C.c_void_p(), C.c_longlong(), C.c_longlong()]
     n = C.c_int(0)
     _lib.check(_lib.lib().dgs_mesh_decimate(v.data_ptr(), len(v), f.data_ptr(), len(f), int(target), alloc.cb, None,
-                                            *[C.byref(o) for o in out], C.byref(n), mesh._stream(v.device)))
+                                            *[C.byref(o) for o in out], C.byref(n), _lib.stream(v.device)))
     torch.cuda.synchronize()
     return n.value
 

@@ -5,12 +5,11 @@
   the depth and alpha maps (aux=True, the launch set Renderer.forward_buffers runs), whose backward receives gradients on all
   three maps; median forward and backward ms from CUDA events, the two alternating window by window, and their spread;
   whether the render is bitwise equal with and without the maps;
-* with --baseline-lib (a libdgs_b200.so of another build, which may predate the maps): every workload of
+* with --baseline-lib (a libdgs_b200.so of another build of the same ABI version): every workload of
   tests/perf_raster.py, this build against that one (bitwise equality of the outputs, gradient differences, timings);
 * the card's name, power.limit and clocks.sm / clocks.max.sm, read in the same run before and after.
 Prints one JSON line."""
 import contextlib
-import ctypes
 import io
 import json
 import sys
@@ -18,29 +17,7 @@ import sys
 import torch
 
 import perf_raster as pr
-from dgs_b200 import _lib, raster
-from perf_dit_linears import load_lib
-
-
-def load_baseline(path):
-    """perf_raster's load_lib for a build that may predate the depth / alpha entry points: those get inert stand-ins (the
-    baseline only runs plain renders, which do not call them)."""
-    class Lenient(ctypes.CDLL):
-        def __getattr__(self, name):
-            try:
-                return super().__getattr__(name)
-            except AttributeError:
-                if not name.endswith("_aux"):
-                    raise
-                stub = ctypes.CFUNCTYPE(ctypes.c_int)(lambda: 1)
-                setattr(self, name, stub)
-                return stub
-    saved = _lib.C.CDLL
-    try:
-        _lib.C.CDLL = Lenient
-        return load_lib(path)
-    finally:
-        _lib.C.CDLL = saved
+from dgs_b200 import raster
 
 
 def run_aux(name, wl):
@@ -68,15 +45,14 @@ def main():
     out = sys.argv[sys.argv.index("--out") + 1] if "--out" in sys.argv else None
     res = dict(card=pr.card(), workloads={})
     if "--baseline-lib" in sys.argv:
-        saved_argv, saved_load = sys.argv, pr.load_lib
+        saved_argv = sys.argv
         sys.argv = [a for i, a in enumerate(saved_argv) if a != "--out" and (i == 0 or saved_argv[i - 1] != "--out")]
-        pr.load_lib = load_baseline
         buf = io.StringIO()
         try:
             with contextlib.redirect_stdout(buf):
                 pr.main()
         finally:
-            sys.argv, pr.load_lib = saved_argv, saved_load
+            sys.argv = saved_argv
         res["existing_vs_baseline"] = json.loads(buf.getvalue().strip().splitlines()[-1])
     obj = dict(B=1, V=4, P=2 + 4 * 256 * 256, W=256, H=256, dist="init", near_log2=-1)
     for name, kw in (("obj256_depth_alpha", obj), ("fine400k_depth_alpha", dict(obj, P=400000, dist="fine"))):

@@ -2,6 +2,9 @@
 import ctypes
 import os
 import re
+import subprocess
+
+import pytest
 
 from dgs_b200 import _lib
 
@@ -50,11 +53,25 @@ def test_backward_trace_structs_mirror_the_header():
     assert not _lib.DitBwdOpts().trace  # zero-filled: no trace unless one is attached
 
 
-def test_version_and_error_string():
+def test_abi_version_101_and_error_string():
     _ensure_built()
     L = _lib.lib()
-    assert L.dgs_version() == 100
+    assert L.dgs_version() == _lib.DGS_VERSION == 101
     assert isinstance(L.dgs_last_error(), bytes)
+
+
+def test_library_of_another_version_is_refused(tmp_path, monkeypatch):
+    """lib() reads dgs_version() before it sets any argtypes: a library of another ABI version raises DgsError instead of
+    being called with the wrong arguments."""
+    src = tmp_path / "stub.c"
+    src.write_text("int dgs_version(void) { return 100; }\n")
+    so = tmp_path / "libdgs_b200.so"
+    subprocess.check_call(["gcc", "-shared", "-fPIC", "-o", str(so), str(src)])
+    monkeypatch.setattr(_lib, "LIB_PATH", str(so))
+    monkeypatch.setattr(_lib, "_lib", None)
+    with pytest.raises(_lib.DgsError, match=r"version 100.*version 101.*build\.py"):
+        _lib.lib()
+    assert _lib._lib is None
 
 
 def test_argument_validation_without_gpu():
