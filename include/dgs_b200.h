@@ -176,6 +176,15 @@ int dgs_render_batch_forward(const dgs_render_batch_args* args, dgs_alloc_fn geo
                              long long* chunk_instances /* out [2]: instances binned in phase A / phase B */,
                              const dgs_render_mse* mse, const dgs_render_aux* aux, void* stream);
 
+/* Video frames: the forward above without mse or aux, whose blend writes uint8 frames [B*V,H,W,3] (HWC) instead of
+ * out_images -- each value is the reference's quantisation of the fp32 image, (image * 255).clip(0, 255).astype(uint8)
+ * (gs_core.py:1215-1216), so the frames equal that of dgs_render_batch_forward's images bit for bit.  Nothing is kept
+ * for a backward.  P == 0 is legal and leaves `frames` as the caller filled it (zeros: the reference's image of an empty
+ * model is zero, not the background); the input pointers may then be NULL. */
+int dgs_render_frames(const dgs_render_batch_args* args, dgs_alloc_fn geom_alloc, void* geom_user,
+                      dgs_alloc_fn binning_alloc, void* binning_user, dgs_alloc_fn image_alloc, void* image_user,
+                      uint8_t* frames /* [B*V, H, W, 3] */, long long* num_rendered, void* stream);
+
 /* Backward: d_* are caller-allocated, same shapes as the inputs; they are fully overwritten.  scratch_alloc provides the
  * per-(view, Gaussian) screen-space gradient records (44 B each), free after the call.  Some upstream gradient must be
  * present: dL_dimages, mse (coef) or an aux map gradient; dL_dimages may be NULL when another is. */

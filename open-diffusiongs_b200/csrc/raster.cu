@@ -852,6 +852,15 @@ struct AuxFwd {
   float* depth = nullptr;  // [NV,1,H,W]; two-phase: phase A leaves its partial sum here for phase B
   float* alpha = nullptr;  // [NV,1,H,W]
 };
+// Video frames (the FRAMES instantiations): each pixel leaves the kernel as the reference's uint8 frame value,
+// (image * 255).clip(0, 255).astype(uint8) of the fp32 colour (gs_core.py:1215-1216), HWC [NV,H,W,3]; no fp32 image is
+// written.  The frames pointer travels in out_color's slot, so the other instantiations keep their parameters (and code).
+struct FramesFwd {
+  // the product rounded on its own (no FMA contraction with the blend); fmaxf maps NaN to 0; the cast truncates
+  __device__ __forceinline__ static uint8_t quantise(float c) {
+    return (uint8_t)fminf(fmaxf(__fmul_rn(c, 255.f), 0.f), 255.f);
+  }
+};
 struct AuxBwd {
   const float* ddepth = nullptr;  // [NV,1,H,W] or null
   const float* dalpha = nullptr;  // [NV,1,H,W] or null
@@ -863,7 +872,8 @@ struct AuxBwd {
 // MODE 0: the whole list in one pass.  MODE 1: phase A of two (the nearest Gaussians); saves the per-pixel blend state
 // and counts the tiles that still have unfinished pixels.  MODE 2: phase B, continues from that state.
 // AUX: also the depth and alpha maps; z rides in the .w of s_rgb (the clamped bits the blend does not read).
-template <int MODE, bool AUX = false>
+// FRAMES: out_color points to uint8 frames (see FramesFwd), written wherever the fp32 image would be.
+template <int MODE, bool AUX = false, bool FRAMES = false>
 __global__ void __launch_bounds__(TILE_PIX) blend_forward_kernel(Problem pb, GeomState gs, ImgState im,
                                                                  const uint32_t* __restrict__ point_list,
                                                                  float* __restrict__ out_color, MseFwd mse, AuxFwd aux) {
@@ -992,11 +1002,18 @@ __global__ void __launch_bounds__(TILE_PIX) blend_forward_kernel(Problem pb, Geo
     const size_t ibase = (size_t)view * pb.W * pb.H;
     im.final_T[ibase + pid] = T;
     im.n_contrib[ibase + pid] = last;
-    float* oc = out_color + 3 * ibase;
-    const size_t plane = (size_t)pb.W * pb.H;
-    oc[pid] = C0 + T * pb.bg[0];
-    oc[plane + pid] = C1 + T * pb.bg[1];
-    oc[2 * plane + pid] = C2 + T * pb.bg[2];
+    if constexpr (FRAMES) {
+      uint8_t* px = reinterpret_cast<uint8_t*>(out_color) + 3 * (ibase + pid);
+      px[0] = FramesFwd::quantise(C0 + T * pb.bg[0]);
+      px[1] = FramesFwd::quantise(C1 + T * pb.bg[1]);
+      px[2] = FramesFwd::quantise(C2 + T * pb.bg[2]);
+    } else {
+      float* oc = out_color + 3 * ibase;
+      const size_t plane = (size_t)pb.W * pb.H;
+      oc[pid] = C0 + T * pb.bg[0];
+      oc[plane + pid] = C1 + T * pb.bg[1];
+      oc[2 * plane + pid] = C2 + T * pb.bg[2];
+    }
     if constexpr (AUX) {
       aux.depth[ibase + pid] = D;
       aux.alpha[ibase + pid] = 1.0f - T;
@@ -1570,6 +1587,7 @@ struct Forward {  // one forward's problem, arenas and launch context, shared by
   float* out_color;
   MseFwd mse;
   AuxFwd aux;
+  uint8_t* frames;   // set: uint8 frames [NV,H,W,3] instead of out_color
   cudaStream_t st;
   int debug;
   size_t N, ntiles;  // view-Gaussians, view-tiles
@@ -1588,7 +1606,10 @@ static int alloc_binning(const Forward& f, long long R, BinState* bs) {
 template <int MODE>
 static int blend_forward(const Forward& f, const uint32_t* point_list) {
   ProfScope ps(f.st, PROF_RASTER_BLEND_FWD);
-  if (!f.aux.depth)
+  if (f.frames)
+    blend_forward_kernel<MODE, false, true><<<(unsigned)f.ntiles, TILE_PIX, 0, f.st>>>(
+        f.pb, f.gs, f.im, point_list, reinterpret_cast<float*>(f.frames), f.mse, f.aux);
+  else if (!f.aux.depth)
     blend_forward_kernel<MODE><<<(unsigned)f.ntiles, TILE_PIX, 0, f.st>>>(f.pb, f.gs, f.im, point_list, f.out_color, f.mse,
                                                                           f.aux);
   else
@@ -1790,9 +1811,9 @@ static int bin_two_phase(const Forward& f, const Split& sp, long long* R_far) {
 // projection -> small-scene binning, or depth ranking and scan -> split decision -> bin pass(es) + blend
 static int run_forward(Problem pb, const CameraInput& cam, const Allocators& al, float* out_color, int* radii,
                        long long* R_out, long long chunk_R[2], cudaStream_t st, int debug, MseFwd mse = MseFwd(),
-                       AuxFwd aux = AuxFwd()) {
+                       AuxFwd aux = AuxFwd(), uint8_t* frames = nullptr) {
   Forward f;
-  f.pb = pb; f.al = al; f.out_color = out_color; f.mse = mse; f.aux = aux; f.st = st; f.debug = debug;
+  f.pb = pb; f.al = al; f.out_color = out_color; f.mse = mse; f.aux = aux; f.frames = frames; f.st = st; f.debug = debug;
   f.N = (size_t)pb.NV * pb.P;
   f.ntiles = (size_t)pb.NV * pb.tiles;
   DGS_REQUIRE(f.N < (size_t)INT32_MAX, "n_views * P = %zu does not fit the 32-bit scan", f.N);
@@ -1992,6 +2013,30 @@ int dgs_render_batch_forward(const dgs_render_batch_args* a, dgs_alloc_fn geom_a
   const Allocators al = {geom_alloc, geom_user, bin_alloc, bin_user, img_alloc, img_user};
   return run_forward(pb, cam, al, out_images, nullptr, num_rendered, chunk_instances, (cudaStream_t)stream, a->debug,
                      mf, af);
+}
+
+int dgs_render_frames(const dgs_render_batch_args* a, dgs_alloc_fn geom_alloc, void* geom_user, dgs_alloc_fn bin_alloc,
+                      void* bin_user, dgs_alloc_fn img_alloc, void* img_user, uint8_t* frames, long long* num_rendered,
+                      void* stream) {
+  DGS_REQUIRE(a != nullptr, "args is NULL");
+  // P == 0 is legal: the caller's zero-filled frames stand, the reference's image of an empty model
+  // (rasterize_points.cu:68,81)
+  if (a->P == 0) {
+    DGS_REQUIRE(a->B > 0 && a->V > 0 && a->W > 0 && a->H > 0, "bad sizes");
+    DGS_REQUIRE(frames && num_rendered, "NULL output");
+    *num_rendered = 0;
+    return DGS_OK;
+  }
+  int rc = check_batch_args(a);
+  if (rc) return rc;
+  DGS_REQUIRE(geom_alloc && bin_alloc && img_alloc && frames && num_rendered, "NULL output/allocator");
+  Problem pb = batch_problem(a);
+  CameraInput cam;
+  cam.c2w = a->c2w; cam.fxfycxcy = a->fxfycxcy;
+  const Allocators al = {geom_alloc, geom_user, bin_alloc, bin_user, img_alloc, img_user};
+  long long chunk_R[2] = {0, 0};
+  return run_forward(pb, cam, al, nullptr, nullptr, num_rendered, chunk_R, (cudaStream_t)stream, a->debug, MseFwd(),
+                     AuxFwd(), frames);
 }
 
 int dgs_render_batch_backward(const dgs_render_batch_args* a, long long R, const long long* chunk_instances,

@@ -140,6 +140,8 @@ def lib():
         L.dgs_render_batch_forward.argtypes = [C.POINTER(RenderBatchArgs), ALLOC_FN, vp, ALLOC_FN, vp, ALLOC_FN, vp, vp,
                                                C.POINTER(C.c_longlong), C.POINTER(C.c_longlong), C.POINTER(RenderMse),
                                                C.POINTER(RenderAux), vp]
+        L.dgs_render_frames.argtypes = [C.POINTER(RenderBatchArgs), ALLOC_FN, vp, ALLOC_FN, vp, ALLOC_FN, vp, vp,
+                                        C.POINTER(C.c_longlong), vp]
         L.dgs_render_batch_backward.argtypes = [C.POINTER(RenderBatchArgs), C.c_longlong, C.POINTER(C.c_longlong)] + \
             [vp] * 5 + [C.POINTER(RenderMse), C.POINTER(RenderAux)] + [vp] * 5 + [ALLOC_FN, vp, vp]
         L.dgs_raster_export_state.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_longlong] + [vp] * 13
@@ -308,5 +310,5 @@ EXPORTED = [  # every symbol include/dgs_b200.h declares (checked by tests/test_
     "dgs_dit_workspace_bytes_fp8", "dgs_dit_forward_fp8", "dgs_quantize_rows_e4m3", "dgs_ln_modulate_fp8", "dgs_gemm_fp8",
     "dgs_mesh_field", "dgs_marching_cubes",
     "dgs_dit_workspace_bytes_fp8_ex", "dgs_dit_forward_fp8_ex", "dgs_attention_quantize_e4m3", "dgs_attention_fwd_fp8",
-    "dgs_mesh_decimate",
+    "dgs_mesh_decimate", "dgs_render_frames",
 ]

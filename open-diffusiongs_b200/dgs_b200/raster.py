@@ -192,6 +192,70 @@ def _render_batch_forward_one(xyz, features, scaling, rotation, opacity, H, W, C
     return (out, *maps, state)
 
 
+# Default budget of render_frames' geometry and image arenas, per chunk of views.  The geometry state is about 100 B per
+# (view, Gaussian): 2 GiB holds about 20 views of a million Gaussians, plenty to fill the GPU, where a whole 150-view
+# turntable would take 15 GB of a card that other work may share.  (The binning arena, which grows with the chunk's
+# instance count, comes on top.)
+FRAMES_ARENA_BYTES = 2 << 30
+
+
+def frames_chunk_views(V, P, H, W, max_arena_bytes=FRAMES_ARENA_BYTES):
+    """Views per render_frames call: the largest n <= V whose geometry and image arenas for n views of P Gaussians at
+    H x W fit in max_arena_bytes; at least 1.  The binning arena depends on the instance count and is not part of it."""
+    L = _lib.lib()
+    fits = lambda n: L.dgs_raster_geom_bytes(n, P) + L.dgs_raster_image_bytes(n, W, H) <= max_arena_bytes  # noqa: E731
+    lo, hi = 1, V
+    while lo < hi:
+        mid = (lo + hi + 1) // 2
+        lo, hi = (mid, hi) if fits(mid) else (lo, mid - 1)
+    return lo
+
+
+def render_frames(xyz, features, scaling, rotation, opacity, H, W, C2W, fxfycxcy, scale_modifier=None,
+                  max_arena_bytes=FRAMES_ARENA_BYTES, arena_cache=None, near_log2=None):
+    """Video frames of every (sample, view) pair -> uint8 [B,V,H,W,3] on xyz's device: each value is the reference's
+    (image * 255).clip(0, 255).astype(uint8) of render_batch_forward's image for the same inputs (gs_core.py:1215-1216),
+    written by the blend kernel itself (dgs_render_frames), with no fp32 image in between.  Inference only: nothing is
+    kept for a backward.
+
+    The views of each sample are rendered frames_chunk_views(V, P, H, W, max_arena_bytes) at a time, into their slice of
+    the one output, so the arenas do not grow with the frame count; every chunk re-uses one grow-only arena set
+    (`arena_cache`, a dict; a fresh one when None).  A chunk of more than 2^31-1 instances is rendered in halves, as
+    render_batch_forward does.  With no Gaussians (P = 0) the frames are black: the reference's rasterizer returns its
+    zero-filled image for an empty model, not the background."""
+    _require_cuda(xyz, "xyz")
+    dev = xyz.device
+    tens = [f32(t) for t in (xyz, features, scaling, rotation, opacity, C2W, fxfycxcy)]
+    B, V, P = tens[5].shape[0], tens[5].shape[1], tens[0].shape[1]
+    H, W = int(H), int(W)
+    near_log2 = -1 if near_log2 is None else near_log2
+    cache = {} if arena_cache is None else arena_cache
+    n = frames_chunk_views(V, P, H, W, max_arena_bytes)
+    total = 0
+    with torch.cuda.device(dev):
+        frames = torch.zeros(B, V, H, W, 3, dtype=torch.uint8, device=dev)
+        b, v0 = 0, 0
+        while b < B:
+            v1 = min(V, v0 + n)
+            cams = (t[b:b + 1, v0:v1] for t in tens[5:])
+            a = _batch_args(*(t[b:b + 1] for t in tens[:5]), *cams, H, W, scale_modifier, near_log2=near_log2)
+            geom, binning, img = (Alloc(dev, cache, k) for k in ("geom", "binning", "img"))
+            R = C.c_longlong(0)
+            try:
+                check(_lib.lib().dgs_render_frames(C.byref(a), geom.cb, None, binning.cb, None, img.cb, None,
+                                                   frames[b, v0:v1].data_ptr(), C.byref(R), stream(dev)))
+            except DgsError as e:
+                if "exceeds 2^31-1" not in str(e) or v1 - v0 < 2:
+                    raise
+                n = (v1 - v0) // 2  # this chunk again, and the ones after it, in halves
+                continue
+            total += R.value
+            b, v0 = (b + 1, 0) if v1 == V else (b, v1)
+    global LAST_NUM_RENDERED
+    LAST_NUM_RENDERED = total
+    return frames
+
+
 def _view_slice(t, v0, v1):
     return None if t is None else t[:, v0:v1]
 

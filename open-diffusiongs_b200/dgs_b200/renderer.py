@@ -12,6 +12,7 @@ import torch
 import torch.nn as nn
 
 from . import raster as _raster
+from .cameras import get_interpolated_poses_many, get_turntable_cameras  # noqa: F401  (the reference's video helpers)
 
 
 class BatchedGaussianRender(torch.autograd.Function):
@@ -336,6 +337,30 @@ def _read_ply_vertices(path):
         dtype = np.dtype([(name, order + t) for name, t in props])
         data = np.frombuffer(f.read(dtype.itemsize * n), dtype=dtype, count=n)
     return data
+
+
+def _model_frames(pc, c2ws, fxfycxcy, h, w):
+    """render_opencv_cam (gs_core.py:874-945: white background, pc.get_scaling with scale_modifier = 1) of every view,
+    quantised as the reference quantises it -> uint8 numpy [v, h, w, 3], with one device-to-host copy."""
+    dev = pc._xyz.device
+    with torch.no_grad():
+        frames = _raster.render_frames(pc._xyz[None], pc.get_features[None], pc._scaling[None], pc._rotation[None],
+                                       pc._opacity[None], h, w, c2ws.to(dev)[None], fxfycxcy.to(dev)[None],
+                                       pc.scaling_modifier)
+    return frames[0].cpu().numpy()
+
+
+def render_turntable(pc, rendering_resolution=384, num_views=8):
+    """gs_core.py:1201-1219: `num_views` frames of get_turntable_cameras at rendering_resolution^2 -> uint8 numpy
+    [h, num_views * w, 3], the views side by side."""
+    w, h, v, fxfycxcy, c2ws = get_turntable_cameras(h=rendering_resolution, w=rendering_resolution, num_views=num_views)
+    frames = _model_frames(pc, torch.from_numpy(c2ws).float(), torch.from_numpy(fxfycxcy).float(), h, w)
+    return frames.transpose(1, 0, 2, 3).reshape(h, v * w, 3)
+
+
+def render_generic(pc, c2ws, fxfycxcy, h=512, w=512):
+    """gs_core.py:1300-1316: c2ws [v, 4, 4], fxfycxcy [v, 4] -> uint8 numpy [v, h, w, 3]."""
+    return _model_frames(pc, c2ws, fxfycxcy.float(), h, w)
 
 
 class Renderer(nn.Module):
