@@ -663,6 +663,38 @@ int dgs_mesh_decimate(const float* vertices, long long num_vertices, const int* 
                       long long target_faces, dgs_alloc_fn alloc, void* alloc_user, float** out_vertices,
                       int** out_faces, long long* out_num_vertices, long long* out_num_faces, int* rounds,
                       void* stream);
+/* Mesh cleaning: the reference's clean_mesh (utils/mesh_utils.py:88-147) with remesh=False, i.e. pymeshlab's
+ * meshing_remove_unreferenced_vertices, merge_close_vertices, remove_duplicate_faces, remove_null_faces,
+ * remove_connected_component_by_diameter / _by_face_number and repair_non_manifold_edges(method=0) /
+ * _vertices(vertdispratio=0), as the nine stages below.  vertices (device fp32 [V, 3]) and faces (device int32 [F, 3],
+ * every index in [0, V); checked on the device, a bad face is DGS_ERR_INVALID_ARGUMENT naming it; a repeated index is
+ * legal).  Every decision is made in fp64 from the fp32 positions (each product and sum rounded, sums left to right,
+ * correctly rounded sqrt); output positions are copies of input positions.  diag(S) = |max - min| over a vertex set S.
+ *   1. the vertices no face references are dropped (index order kept);
+ *   2. v_pct > 0: r = (v_pct / 100) diag(referenced).  In index order a vertex is a seed iff no earlier seed lies at
+ *      distance |p - q| < r (strict); every other vertex becomes the lowest-index seed within r.  Faces are re-indexed
+ *      and a face that repeats a vertex is dropped.  (pymeshlab's ClusterVertex may pick a different seed set: this is
+ *      the lexicographically-first maximal independent set of the radius graph);
+ *   3. faces with the same sorted index triple (either winding) are dropped but the lowest-index one;
+ *   4. faces whose doubled area |(b - a) x (c - a)| is exactly 0 are dropped;
+ *   5. min_d > 0: components (faces joined through shared edges; a non-manifold edge joins all its faces, a shared
+ *      vertex does not) whose box diagonal is < (min_d / 100) diag(vertices of the faces left by 4) are dropped;
+ *   6. min_f > 0: components with < min_f faces are dropped;
+ *   7. repair: the faces with an edge of more than 2 faces, in (doubled area, face index) order, are each dropped iff
+ *      one of their edges still has more than 2 live faces at that moment;
+ *   8. repair: a vertex's faces form fans (joined through shared edges that contain it); the fan holding its lowest
+ *      face keeps it, every other fan gets a copy at the same position, appended after all vertices in order of
+ *      (vertex, the fan's lowest face);
+ *   9. the referenced vertices are kept in index order and the faces in face order, winding kept.
+ * The result is the same bits on every run.  *merge_rounds (NULL or host) receives the number of parallel rounds stage 2
+ * took; stage_faces (NULL or host [9]) the face count after each stage.  alloc is called once for scratch (about 270 B
+ * per face plus 50 B per vertex, free after the call), then, after the last host sync, for *out_vertices (fp32 [V', 3])
+ * and *out_faces (int32 [F', 3]) when F' > 0; an empty result is V' = F' = 0 with NULL outputs.  The stream is
+ * synchronised once to check the indices, once per merge round and once per stage that needs a count. */
+int dgs_mesh_clean(const float* vertices, long long num_vertices, const int* faces, long long num_faces, double v_pct,
+                   long long min_f, double min_d, int repair, dgs_alloc_fn alloc, void* alloc_user,
+                   float** out_vertices, int** out_faces, long long* out_num_vertices, long long* out_num_faces,
+                   int* merge_rounds, long long* stage_faces, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * B3. The elementwise callers either side of the path.

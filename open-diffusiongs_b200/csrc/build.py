@@ -13,9 +13,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.abspath(os.path.join(HERE, "..", ".."))
 OUT_DIR = os.path.join(HERE, "..", "dgs_b200", "lib")
 OUT = os.path.abspath(os.path.join(OUT_DIR, "libdgs_b200.so"))
-SOURCES = ["core.cu", "raster.cu", "dit_glue.cu", "gemm_sm90.cu", "attention_sm90.cu", "attention_bwd_sm90.cu", "dit_api.cu", "diffusion_steps.cu", "lpips.cu", "ssim.cu", "geometry_loss.cu", "mesh.cu", "mesh_decimate.cu"]
+SOURCES = ["core.cu", "raster.cu", "dit_glue.cu", "gemm_sm90.cu", "attention_sm90.cu", "attention_bwd_sm90.cu", "dit_api.cu", "diffusion_steps.cu", "lpips.cu", "ssim.cu", "geometry_loss.cu", "mesh.cu", "mesh_decimate.cu", "mesh_clean.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-O3"]
+FILE_FLAGS = {"mesh_clean.cu": ["-fmad=false"]}  # its fp64 decisions round every product and sum, as its oracle does
 
 
 def _stale(obj, deps):
@@ -39,7 +40,7 @@ def build(force=False, verbose=False):
         obj = os.path.join(obj_dir, src.replace(".cu", ".o"))
         objs.append(obj)
         if force or _stale(obj, [sp] + headers):
-            cmd = ["nvcc"] + NVCC_FLAGS + ["-I", os.path.join(ROOT, "include"), "-I", HERE, "-c", sp, "-o", obj]
+            cmd = ["nvcc"] + NVCC_FLAGS + FILE_FLAGS.get(src, []) + ["-I", os.path.join(ROOT, "include"), "-I", HERE, "-c", sp, "-o", obj]
             if verbose:
                 print(" ".join(cmd))
             procs.append((src, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))

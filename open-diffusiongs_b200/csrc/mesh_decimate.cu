@@ -30,11 +30,11 @@
 #include <algorithm>
 
 #include "dgs_internal.h"
+#include "mesh_edges.cuh"
 
 namespace dgs {
 namespace {
 
-constexpr int kThreads = 256;
 constexpr unsigned long long kNoKey = ~0ull;
 constexpr double kMaxCondition = 1e7;  // Frobenius condition number above which the 3 x 3 system is not solved
 
@@ -64,7 +64,6 @@ __device__ __forceinline__ double3 round_f32(double3 v) {
   return make_double3((double)(float)v.x, (double)(float)v.y, (double)(float)v.z);
 }
 __device__ __forceinline__ bool has(int3 f, int x) { return f.x == x || f.y == x || f.z == x; }
-__device__ __forceinline__ int corner(int3 f, int k) { return k == 0 ? f.x : k == 1 ? f.y : f.z; }
 
 __device__ Quadric face_quadric(const float* __restrict__ pos, int3 f) {
   const double3 p0 = load(pos, f.x);
@@ -168,23 +167,6 @@ __global__ void validate_kernel(int F, int V, const int3* __restrict__ faces, Co
   if (!ok) atomicMin(&ctr->bad_face, (unsigned long long)f);
 }
 
-// (vertex, face) incidences in face order; a stable sort by vertex makes each vertex's faces one run in face order
-__global__ void incidence_kernel(int n, const int3* __restrict__ faces, uint32_t* __restrict__ keys,
-                                 uint32_t* __restrict__ vals) {
-  const int h = blockIdx.x * blockDim.x + threadIdx.x;
-  if (h >= n) return;
-  keys[h] = (uint32_t)corner(faces[h / 3], h % 3);
-  vals[h] = (uint32_t)(h / 3);
-}
-
-__global__ void ranges_kernel(int n, const uint32_t* __restrict__ keys, uint2* __restrict__ ranges) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const uint32_t k = keys[i];
-  if (i == 0 || keys[i - 1] != k) ranges[k].x = i;
-  if (i == n - 1 || keys[i + 1] != k) ranges[k].y = i + 1;
-}
-
 __global__ void vertex_quadric_kernel(int V, const float* __restrict__ pos, const int3* __restrict__ faces,
                                       const uint2* __restrict__ vrange, const uint32_t* __restrict__ vfaces,
                                       Quadric* __restrict__ Q) {
@@ -201,22 +183,6 @@ __global__ void vertex_quadric_kernel(int V, const float* __restrict__ pos, cons
 }
 
 // ---------------------------------------------------------------------------------------------------------- edges
-__global__ void halfedge_kernel(int n, const int3* __restrict__ faces, int vbits, unsigned long long* __restrict__ keys,
-                                uint32_t* __restrict__ vals) {
-  const int h = blockIdx.x * blockDim.x + threadIdx.x;
-  if (h >= n) return;
-  const int3 f = faces[h / 3];
-  const int u = corner(f, h % 3), w = corner(f, (h % 3 + 1) % 3);
-  keys[h] = ((unsigned long long)min(u, w) << vbits) | (unsigned long long)max(u, w);
-  vals[h] = (uint32_t)h;
-}
-
-__global__ void edge_heads_kernel(int n, const unsigned long long* __restrict__ keys, uint32_t* __restrict__ heads) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  heads[i] = i == 0 || keys[i] != keys[i - 1];
-}
-
 // One thread per sorted half-edge: its edge id; the run's first thread writes the edge, its apexes and the locks.
 __global__ void edge_build_kernel(int n, const unsigned long long* __restrict__ keys, const uint32_t* __restrict__ vals,
                                   const uint32_t* __restrict__ scan, const int3* __restrict__ faces, int vbits,
@@ -441,16 +407,7 @@ struct Scratch {
 
 // The vertex -> face lists of the first F faces: vfaces[vrange[v].x, vrange[v].y) in face order.
 cudaError_t vertex_faces(Scratch& s, int F, int V, int vbits, cudaStream_t st) {
-  const int n = 3 * F;
-  incidence_kernel<<<ceil_div(n, kThreads), kThreads, 0, st>>>(n, s.faces, s.ikey_in, s.ival_in);
-  g_kernel_launches++;
-  cudaError_t e = cub::DeviceRadixSort::SortPairs(s.temp, s.temp_bytes, s.ikey_in, s.ikey, s.ival_in, s.vfaces, n, 0,
-                                                  vbits, st);
-  if (e != cudaSuccess) return e;
-  if ((e = cudaMemsetAsync(s.vrange, 0, (size_t)V * sizeof(uint2), st)) != cudaSuccess) return e;
-  ranges_kernel<<<ceil_div(n, kThreads), kThreads, 0, st>>>(n, s.ikey, s.vrange);
-  g_kernel_launches++;
-  return cudaGetLastError();
+  return vertex_faces(F, V, s.faces, vbits, s.ikey_in, s.ikey, s.ival_in, s.vfaces, s.vrange, s.temp, s.temp_bytes, st);
 }
 
 }  // namespace
@@ -534,13 +491,7 @@ int dgs_mesh_decimate(const float* vertices, long long num_vertices, const int* 
   int live = F, applied_rounds = 0;
   while (live > (long long)target_faces) {
     const int n = 3 * live, gn = ceil_div(n, kThreads), gv = ceil_div(V, kThreads);
-    halfedge_kernel<<<gn, kThreads, 0, st>>>(n, s.faces, vbits, s.hkey_in, s.hval_in);
-    DGS_POST_LAUNCH();
-    DGS_CUDA_OK(cub::DeviceRadixSort::SortPairs(s.temp, s.temp_bytes, s.hkey_in, s.hkey, s.hval_in, s.hval, n, 0,
-                                                2 * vbits, st));
-    edge_heads_kernel<<<gn, kThreads, 0, st>>>(n, s.hkey, s.heads);
-    DGS_POST_LAUNCH();
-    DGS_CUDA_OK(cub::DeviceScan::InclusiveSum(s.temp, s.temp_bytes, s.heads, s.heads, n, st));
+    DGS_CUDA_OK(sort_edges(n, s.faces, vbits, s.hkey_in, s.hkey, s.hval_in, s.hval, s.heads, s.temp, s.temp_bytes, st));
     edge_build_kernel<<<gn, kThreads, 0, st>>>(n, s.hkey, s.hval, s.heads, s.faces, vbits, s.edges, s.edge_of, s.lock,
                                                s.ctr);
     DGS_POST_LAUNCH();

@@ -221,6 +221,9 @@ def lib():
         L.dgs_mesh_decimate.argtypes = [vp, C.c_longlong, vp, C.c_longlong, C.c_longlong, ALLOC_FN, vp,
                                         C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_longlong),
                                         C.POINTER(C.c_longlong), C.POINTER(C.c_int), vp]
+        L.dgs_mesh_clean.argtypes = [vp, C.c_longlong, vp, C.c_longlong, C.c_double, C.c_longlong, C.c_double, C.c_int,
+                                     ALLOC_FN, vp, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_longlong),
+                                     C.POINTER(C.c_longlong), C.POINTER(C.c_int), C.POINTER(C.c_longlong), vp]
         _lib = L
     return _lib
 
@@ -310,5 +313,5 @@ EXPORTED = [  # every symbol include/dgs_b200.h declares (checked by tests/test_
     "dgs_dit_workspace_bytes_fp8", "dgs_dit_forward_fp8", "dgs_quantize_rows_e4m3", "dgs_ln_modulate_fp8", "dgs_gemm_fp8",
     "dgs_mesh_field", "dgs_marching_cubes",
     "dgs_dit_workspace_bytes_fp8_ex", "dgs_dit_forward_fp8_ex", "dgs_attention_quantize_e4m3", "dgs_attention_fwd_fp8",
-    "dgs_mesh_decimate", "dgs_render_frames",
+    "dgs_mesh_decimate", "dgs_render_frames", "dgs_mesh_clean",
 ]

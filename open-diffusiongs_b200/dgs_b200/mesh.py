@@ -1,11 +1,12 @@
-"""Mesh extraction on libdgs_b200.so (dgs_mesh_field / dgs_marching_cubes / dgs_mesh_decimate): the layer under
-`GaussianModel.extract_fields` / `extract_mesh`, and a command line that meshes a saved Gaussian PLY.
+"""Mesh extraction on libdgs_b200.so (dgs_mesh_field / dgs_marching_cubes / dgs_mesh_clean / dgs_mesh_decimate): the
+layer under `GaussianModel.extract_fields` / `extract_mesh`, and a command line that meshes a saved Gaussian PLY.
 
-    python -m dgs_b200.mesh in.ply out.obj [--resolution 256] [--density-thresh 0.005] [--decimate-target N]
+    python -m dgs_b200.mesh in.ply out.obj [--resolution 256] [--density-thresh 0.005] [--clean] [--decimate-target N]
 
 reads a PLY written by `GaussianModel.save_ply` (or the reference's), extracts the mesh exactly as
-`extract_mesh(density_thresh, resolution)` does and writes it as OBJ or binary PLY, chosen by the suffix; with
-`--decimate-target N` the mesh is first decimated to at most N faces (`decimate`, dgs_mesh_decimate).
+`extract_mesh(density_thresh, resolution)` does and writes it as OBJ or binary PLY, chosen by the suffix; with `--clean`
+the mesh is first cleaned (`clean`, dgs_mesh_clean), and with `--decimate-target N` then decimated to at most N faces
+(`decimate`, dgs_mesh_decimate).
 
 Marching cubes produces the same vertex set as PyMCubes (one vertex per sign-changing grid edge, at the linear
 interpolation of the iso value); on the ambiguous cases the triangulation may differ (a face with two diagonally
@@ -84,33 +85,30 @@ def marching_cubes(field, iso):
     return verts, faces
 
 
-def decimate(vertices, faces, target_faces):
-    """Quadric edge-collapse decimation to at most `target_faces` faces (dgs_mesh_decimate; the reference's
-    decimate_mesh with optimalplacement=True, boundary loops kept) -> (vertices, faces).  The signature of
-    extract_mesh's `postprocess`, so `extract_mesh(postprocess=decimate)` returns the reference's <= decimate_target
-    (1e5) face mesh.  numpy input (vertices float [V, 3], faces integer [F, 3]) runs on the current CUDA device and returns
-    numpy float32 [V', 3] / int64 [F', 3]; CUDA tensors return CUDA tensors of those dtypes on their device.  The
-    result has target_faces or target_faces - 1 faces unless no further edge can be collapsed; a mesh within the target
-    comes back unchanged."""
+def _mesh_check(name, vertices, faces):
+    """Checks the types, shapes and dtypes of a mesh argument pair -> whether it is numpy (else CUDA tensors)"""
     is_numpy = isinstance(vertices, np.ndarray) and isinstance(faces, np.ndarray)
     if not is_numpy and not (isinstance(vertices, torch.Tensor) and isinstance(faces, torch.Tensor)
                              and vertices.is_cuda and faces.is_cuda and vertices.device == faces.device):
-        raise TypeError("decimate: vertices and faces must both be numpy arrays or CUDA tensors on one device")
+        raise TypeError(f"{name}: vertices and faces must both be numpy arrays or CUDA tensors on one device")
     if vertices.ndim != 2 or vertices.shape[1] != 3 or faces.ndim != 2 or faces.shape[1] != 3:
-        raise ValueError(f"decimate: expected vertices [V, 3] and faces [F, 3], got {tuple(vertices.shape)} and "
+        raise ValueError(f"{name}: expected vertices [V, 3] and faces [F, 3], got {tuple(vertices.shape)} and "
                          f"{tuple(faces.shape)}")
     float_v = vertices.dtype.kind == "f" if is_numpy else vertices.dtype.is_floating_point
     int_f = faces.dtype.kind in "iu" if is_numpy else not (faces.dtype.is_floating_point or faces.dtype.is_complex
                                                              or faces.dtype == torch.bool)
     if not float_v or not int_f:
-        raise TypeError(f"decimate: vertices must be floating point and faces integer (got {vertices.dtype}, "
+        raise TypeError(f"{name}: vertices must be floating point and faces integer (got {vertices.dtype}, "
                         f"{faces.dtype})")
-    target = float(target_faces)
-    if not np.isfinite(target) or target < 0:
-        raise ValueError(f"decimate: target_faces must be a finite number >= 0 (got {target_faces!r})")
+    return is_numpy
+
+
+def _mesh_in(name, is_numpy, vertices, faces):
+    """A checked mesh argument pair -> (device, vertices fp32 [V, 3], faces int32 [F, 3]) as contiguous CUDA tensors;
+    numpy input goes to the current CUDA device."""
     i32 = np.iinfo(np.int32)
     if len(faces) and (int(faces.min()) < i32.min or int(faces.max()) > i32.max):
-        raise ValueError("decimate: face indices do not fit int32")
+        raise ValueError(f"{name}: face indices do not fit int32")
     if is_numpy:
         dev = torch.device("cuda", torch.cuda.current_device())
         v = torch.from_numpy(np.ascontiguousarray(vertices, np.float32)).to(dev)
@@ -119,6 +117,32 @@ def decimate(vertices, faces, target_faces):
         dev = vertices.device
         v = vertices.detach().to(torch.float32).contiguous()
         f = faces.detach().to(torch.int32).contiguous()
+    return dev, v, f
+
+
+def _mesh_out(is_numpy, dev, alloc, V, F):
+    """The output buffers a mesh call allocated after its scratch -> (vertices fp32 [V, 3], faces int64 [F, 3])"""
+    ov = alloc.tensors[1][:V * 12].view(torch.float32).view(V, 3) if V else torch.zeros(0, 3, device=dev)
+    of = alloc.tensors[2][:F * 12].view(torch.int32).view(F, 3).long() if F else torch.zeros(0, 3, dtype=torch.int64,
+                                                                                              device=dev)
+    if is_numpy:
+        return ov.cpu().numpy(), of.cpu().numpy()
+    return ov, of
+
+
+def decimate(vertices, faces, target_faces):
+    """Quadric edge-collapse decimation to at most `target_faces` faces (dgs_mesh_decimate; the reference's
+    decimate_mesh with optimalplacement=True, boundary loops kept) -> (vertices, faces).  The signature of
+    extract_mesh's `postprocess`, so `extract_mesh(postprocess=decimate)` returns the reference's <= decimate_target
+    (1e5) face mesh.  numpy input (vertices float [V, 3], faces integer [F, 3]) runs on the current CUDA device and returns
+    numpy float32 [V', 3] / int64 [F', 3]; CUDA tensors return CUDA tensors of those dtypes on their device.  The
+    result has target_faces or target_faces - 1 faces unless no further edge can be collapsed; a mesh within the target
+    comes back unchanged."""
+    is_numpy = _mesh_check("decimate", vertices, faces)
+    target = float(target_faces)
+    if not np.isfinite(target) or target < 0:
+        raise ValueError(f"decimate: target_faces must be a finite number >= 0 (got {target_faces!r})")
+    dev, v, f = _mesh_in("decimate", is_numpy, vertices, faces)
     alloc = Alloc(dev, _SCRATCH, (str(dev), "decimate"), cached=1)
     vp, fp = C.c_void_p(), C.c_void_p()
     nv, nf, rounds = C.c_longlong(0), C.c_longlong(0), C.c_int(0)
@@ -126,13 +150,44 @@ def decimate(vertices, faces, target_faces):
         check(_lib.lib().dgs_mesh_decimate(v.data_ptr(), len(v), f.data_ptr(), len(f), int(target), alloc.cb, None,
                                            C.byref(vp), C.byref(fp), C.byref(nv), C.byref(nf), C.byref(rounds),
                                            stream(dev)))
-    V, F = nv.value, nf.value
-    ov = alloc.tensors[1][:V * 12].view(torch.float32).view(V, 3) if V else torch.zeros(0, 3, device=dev)
-    of = alloc.tensors[2][:F * 12].view(torch.int32).view(F, 3).long() if F else torch.zeros(0, 3, dtype=torch.int64,
-                                                                                              device=dev)
-    if is_numpy:
-        return ov.cpu().numpy(), of.cpu().numpy()
-    return ov, of
+    return _mesh_out(is_numpy, dev, alloc, nv.value, nf.value)
+
+
+def clean(vertices, faces, v_pct=1, min_f=64, min_d=20, repair=True, stats=None):
+    """The reference's clean_mesh with remesh=False (dgs_mesh_clean) -> (vertices, faces): drop unreferenced
+    vertices, merge vertices closer than v_pct % of the bounding-box diagonal (v_pct <= 0: no merge), drop duplicate
+    and zero-area faces, edge-connected components with a diagonal under min_d % of the mesh's (min_d <= 0: kept) or
+    fewer than min_f faces (min_f <= 0: kept), and with `repair` the non-manifold edges' smallest faces and the
+    non-manifold vertices (split: one copy per extra fan).  Input and output types as `decimate`; the output positions
+    are copies of input positions, and the result is the same bits on every run.  `stats`, a dict, receives
+    "merge_rounds" and "stage_faces" (the face count after each of the nine stages of include/dgs_b200.h)."""
+    is_numpy = _mesh_check("clean", vertices, faces)
+    v_pct, min_d = float(v_pct), float(min_d)
+    if not (np.isfinite(v_pct) and np.isfinite(min_d)):
+        raise ValueError(f"clean: v_pct and min_d must be finite (got {v_pct!r}, {min_d!r})")
+    dev, v, f = _mesh_in("clean", is_numpy, vertices, faces)
+    alloc = Alloc(dev, _SCRATCH, (str(dev), "clean"), cached=1)
+    vp, fp = C.c_void_p(), C.c_void_p()
+    nv, nf, rounds = C.c_longlong(0), C.c_longlong(0), C.c_int(0)
+    counts = (C.c_longlong * 9)()
+    with torch.cuda.device(dev):
+        check(_lib.lib().dgs_mesh_clean(v.data_ptr(), len(v), f.data_ptr(), len(f), v_pct, int(min_f), min_d,
+                                        int(bool(repair)), alloc.cb, None, C.byref(vp), C.byref(fp), C.byref(nv),
+                                        C.byref(nf), C.byref(rounds), counts, stream(dev)))
+    if stats is not None:
+        stats["merge_rounds"] = rounds.value
+        stats["stage_faces"] = list(counts)
+    return _mesh_out(is_numpy, dev, alloc, nv.value, nf.value)
+
+
+def clean_then_decimate(vertices, faces, decimate_target):
+    """The reference's extract_mesh post-processing without its remeshing (gs_core.py:862-863): `clean` with its
+    defaults, then `decimate` to decimate_target faces when more are left.  The signature of extract_mesh's
+    `postprocess`: `extract_mesh(postprocess=clean_then_decimate)`."""
+    v, f = clean(vertices, faces)
+    if len(f) > decimate_target:
+        v, f = decimate(v, f, decimate_target)
+    return v, f
 
 
 class Mesh:
@@ -186,7 +241,21 @@ def parser():
     ap.add_argument("--density-thresh", type=float, default=0.005, help="iso value of the opacity field (default 0.005)")
     ap.add_argument("--decimate-target", type=int, default=None, metavar="N",
                     help="decimate to at most N faces (quadric edge collapse; default: the raw marching-cubes mesh)")
+    ap.add_argument("--clean", action="store_true",
+                    help="clean first (merge close vertices, drop duplicate / null faces and small components, repair "
+                         "non-manifold parts), as the reference's clean_mesh without remeshing")
     return ap
+
+
+def _postprocess(args):
+    """-> extract_mesh keyword arguments for the --clean / --decimate-target flags"""
+    if args.clean and args.decimate_target is not None:
+        return dict(postprocess=clean_then_decimate, decimate_target=args.decimate_target)
+    if args.clean:
+        return dict(postprocess=lambda v, f, _target: clean(v, f))
+    if args.decimate_target is not None:
+        return dict(postprocess=decimate, decimate_target=args.decimate_target)
+    return {}
 
 
 def main(argv=None):
@@ -194,8 +263,8 @@ def main(argv=None):
     from .renderer import GaussianModel
     gm = GaussianModel(0)
     gm.load_ply(args.ply)
-    kw = {} if args.decimate_target is None else dict(postprocess=decimate, decimate_target=args.decimate_target)
-    mesh = gm.to("cuda").extract_mesh(density_thresh=args.density_thresh, resolution=args.resolution, **kw)
+    mesh = gm.to("cuda").extract_mesh(density_thresh=args.density_thresh, resolution=args.resolution,
+                                      **_postprocess(args))
     mesh.export(args.out)
     print(f"{args.out}: {len(mesh.vertices)} vertices, {len(mesh.faces)} faces")
 

@@ -276,10 +276,10 @@ class GaussianModel:
         """gs_core.py:855-869: extract_fields(resolution, num_blocks=64), marching cubes at density_thresh on the GPU,
         vertices mapped by v / (resolution - 1) * 2 - 1 (in the normalised frame: not mapped back by mesh_center /
         mesh_scale, as in the reference) -> dgs_b200.mesh.Mesh (vertices float32 [V, 3], faces int64 [F, 3]).
-        The reference then cleans, remeshes and decimates with pymeshlab; that is not done here: without `postprocess`
-        the raw marching-cubes mesh is returned and `decimate_target` is unused.  `postprocess(vertices, faces,
-        decimate_target) -> (vertices, faces)` runs on the numpy arrays, e.g. a wrapper of the reference's clean_mesh /
-        decimate_mesh."""
+        The reference then cleans, remeshes and decimates with pymeshlab; without `postprocess` the raw marching-cubes
+        mesh is returned and `decimate_target` is unused.  `postprocess(vertices, faces, decimate_target) -> (vertices,
+        faces)` runs on the numpy arrays: `dgs_b200.mesh.clean_then_decimate` is the reference's chain without its
+        remeshing (clean, then decimate to decimate_target faces), `dgs_b200.mesh.decimate` decimates only."""
         from . import mesh as _mesh
         occ = self.extract_fields(resolution, num_blocks=64)
         return _mesh.extract_mesh(occ, density_thresh, resolution, postprocess, decimate_target)
