@@ -695,6 +695,64 @@ int dgs_mesh_clean(const float* vertices, long long num_vertices, const int* fac
                    long long min_f, double min_d, int repair, dgs_alloc_fn alloc, void* alloc_user,
                    float** out_vertices, int** out_faces, long long* out_num_vertices, long long* out_num_faces,
                    int* merge_rounds, long long* stage_faces, void* stream);
+/* Isotropic remeshing: the step the reference's clean_mesh(remesh=True) runs with pymeshlab's
+ * meshing_isotropic_explicit_remeshing(iterations, targetlen) (VCG's IsotropicRemeshing), as an exact contract that
+ * oracle/mesh_remesh.py restates serially.  vertices (device fp32 [V, 3]) and faces (device int32 [F, 3], every index in
+ * [0, V), none repeated within a face; checked on the device, a bad face is DGS_ERR_INVALID_ARGUMENT naming it).  Every
+ * decision and new position is fp64 from the fp32 positions (each product and sum rounded, sums left to right and over a
+ * vertex's faces in face order, correctly rounded sqrt and division); positions are stored as fp32 after each stage.
+ * L = target_len (finite, > 0), lo = 4 L / 5, hi = 4 L / 3; S = the input mesh, fixed for the call; max_surf_dist < 0
+ * means diag / 100 with diag = |max - min| of the referenced input vertices; cos_t = cos(feature_deg * pi / 180).
+ * Normals are (p1 - p0) x (p2 - p0) in stored corner order.  An edge is blocked when it does not have exactly two faces
+ * running it in opposite directions (boundary, non-manifold) or when it is a feature edge: n0 . n1 < cos_t |n0| |n1|.
+ * Each of `iterations` (>= 0) iterations:
+ *   0. lock the ends of every blocked edge (the locks hold for the iteration);
+ *   1. split every edge longer than hi at its fp32 midpoint, all at once: new vertices V, V + 1, ... in edge (min, max)
+ *      order, locked iff the edge is blocked (an unblocked edge between two locked ends gives a free midpoint, which
+ *      smoothing may move along the surface).  A face with split edge (a, b) opposite c becomes (a, m, c), (m, b, c);
+ *      with (c, a) the only unsplit edge, (m_ab, b, m_bc) and the quad (a, m_ab, m_bc, c) cut along (m_ab, c) if
+ *      strictly shorter than (a, m_bc), else along (a, m_bc), the diagonal from the lower index (m_ab >= V > a); with
+ *      three, (v0, m0, m2), (m0, v1, m1), (m2, m1, v2), (m0, m1, m2).  The first face replaces its parent, the others
+ *      are appended in parent order;
+ *   2. collapse rounds.  Candidates: not blocked, shorter than lo, not locked at both ends.  The new position is the
+ *      locked end's, else the fp32 midpoint.  Rejected when the link condition fails (as dgs_mesh_decimate), a face
+ *      around either end not containing both would flip or degenerate (new normal . old normal <= 0; faces of zero area
+ *      before are exempt), a neighbour of either end would be farther than hi from the new position, or the new position
+ *      is farther than max_surf_dist from S.  Key = fp32 bits of the length << 32 | edge; an edge is taken iff its key
+ *      is the smallest within two hops of both ends (dgs_mesh_decimate's selection).  The lower index survives, takes
+ *      the new position and the other end's lock; the two faces of the edge go.  Until a round takes none;
+ *   3. flip rounds.  Valence targets: 4 on a vertex of a one-face edge, else 6.  Edge (a, b) with faces (u, w, c),
+ *      (w, u, d) (h0's face first) becomes (c, u, d), (d, w, c) in place when it is not blocked, c != d, (c, d) is not an
+ *      edge, both new normals have a positive dot product with both old ones, the fp64 midpoint of c, d is within
+ *      max_surf_dist of S and gain = the drop of sum (valence - target)^2 over a, b, c, d is > 0.  A round takes every
+ *      candidate whose key (2^31 - 1 - gain) << 32 | edge is the smallest at all four of its vertices, so the energy
+ *      drops every round.  Until a round takes none;
+ *   4. one Jacobi pass of tangential smoothing of every unlocked vertex with faces: c = the mean of the other two
+ *      corners of each of its faces, n = the normalised sum of its face normals, p + (d - (d . n) n) with d = c - p;
+ *   5. every vertex with faces moves to its closest point on S: the smallest (squared distance, face) over S's faces
+ *      by Ericson's ClosestPtPointTriangle (found through a uniform grid of S's triangle boxes, built once per call).
+ * Collapse and flip stop after 256 rounds each (never an error).  The output keeps the referenced vertices in index
+ * order and the faces in face order, winding kept; iterations = 0 returns the input bit for bit (unreferenced vertices
+ * included).  Departures from VCG: no CollapseCrosses, a Jacobi uniform tangential Laplacian for its planar one, midpoint
+ * collapses everywhere.  The result is the same bits on every run.  stats (NULL or host [iterations][4]) receives per
+ * iteration the faces after the split, the collapse rounds, the flip rounds and 1 if a stage stopped at 256 rounds.
+ * alloc is called for scratch (about 450 B per face plus 80 B per vertex of the largest mesh; with iterations = 0 only
+ * for a few counters), for the grid, and again for scratch whenever a split outgrows it; then, after the last host sync, for *out_vertices (fp32 [V', 3]) and
+ * *out_faces (int32 [F', 3]) when F' > 0 (these are the last two requests); an empty result is V' = F' = 0 with NULL
+ * outputs.  The stream is synchronised to check the indices, to size the grid, once per split and once per round. */
+int dgs_mesh_remesh(const float* vertices, long long num_vertices, const int* faces, long long num_faces,
+                    double target_len, int iterations, double feature_deg, double max_surf_dist, dgs_alloc_fn alloc,
+                    void* alloc_user, float** out_vertices, int** out_faces, long long* out_num_vertices,
+                    long long* out_num_faces, long long* stats, void* stream);
+/* The closest point of a surface to each query: vertices (device fp32 [V, 3]) and faces (device int32 [F, 3], F > 0,
+ * checked as for dgs_mesh_remesh) form the surface; queries device fp64 [Q, 3].  Per query, out_points (device fp64
+ * [Q, 3]) receives the point, out_d2 (device fp64 [Q]) its squared distance and out_faces (device int32 [Q]) its face:
+ * the smallest (squared distance, face) over every face by Ericson's ClosestPtPointTriangle in fp64, the query
+ * dgs_mesh_remesh reprojects with, through the same grid.  alloc is called for scratch (about 16 B per face) and for the
+ * grid; the stream is synchronised to check the indices and to size the grid. */
+int dgs_mesh_closest_points(const float* vertices, long long num_vertices, const int* faces, long long num_faces,
+                            const double* queries, long long num_queries, double* out_points, double* out_d2,
+                            int* out_faces, dgs_alloc_fn alloc, void* alloc_user, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * B3. The elementwise callers either side of the path.

@@ -224,6 +224,11 @@ def lib():
         L.dgs_mesh_clean.argtypes = [vp, C.c_longlong, vp, C.c_longlong, C.c_double, C.c_longlong, C.c_double, C.c_int,
                                      ALLOC_FN, vp, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_longlong),
                                      C.POINTER(C.c_longlong), C.POINTER(C.c_int), C.POINTER(C.c_longlong), vp]
+        L.dgs_mesh_remesh.argtypes = [vp, C.c_longlong, vp, C.c_longlong, C.c_double, C.c_int, C.c_double, C.c_double,
+                                      ALLOC_FN, vp, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                      C.POINTER(C.c_longlong), C.POINTER(C.c_longlong), C.POINTER(C.c_longlong), vp]
+        L.dgs_mesh_closest_points.argtypes = [vp, C.c_longlong, vp, C.c_longlong, vp, C.c_longlong, vp, vp, vp, ALLOC_FN,
+                                              vp, vp]
         _lib = L
     return _lib
 
@@ -313,5 +318,6 @@ EXPORTED = [  # every symbol include/dgs_b200.h declares (checked by tests/test_
     "dgs_dit_workspace_bytes_fp8", "dgs_dit_forward_fp8", "dgs_quantize_rows_e4m3", "dgs_ln_modulate_fp8", "dgs_gemm_fp8",
     "dgs_mesh_field", "dgs_marching_cubes",
     "dgs_dit_workspace_bytes_fp8_ex", "dgs_dit_forward_fp8_ex", "dgs_attention_quantize_e4m3", "dgs_attention_fwd_fp8",
-    "dgs_mesh_decimate", "dgs_render_frames", "dgs_mesh_clean",
+    "dgs_mesh_decimate", "dgs_render_frames", "dgs_mesh_clean", "dgs_mesh_remesh",
+    "dgs_mesh_closest_points",
 ]

@@ -1,12 +1,15 @@
-"""Mesh extraction on libdgs_b200.so (dgs_mesh_field / dgs_marching_cubes / dgs_mesh_clean / dgs_mesh_decimate): the
-layer under `GaussianModel.extract_fields` / `extract_mesh`, and a command line that meshes a saved Gaussian PLY.
+"""Mesh extraction on libdgs_b200.so (dgs_mesh_field / dgs_marching_cubes / dgs_mesh_clean / dgs_mesh_remesh /
+dgs_mesh_decimate): the layer under `GaussianModel.extract_fields` / `extract_mesh`, and a command line that meshes a
+saved Gaussian PLY.
 
-    python -m dgs_b200.mesh in.ply out.obj [--resolution 256] [--density-thresh 0.005] [--clean] [--decimate-target N]
+    python -m dgs_b200.mesh in.ply out.obj [--resolution 256] [--density-thresh 0.005] [--clean] [--remesh [LEN]]
+                                           [--decimate-target N]
 
 reads a PLY written by `GaussianModel.save_ply` (or the reference's), extracts the mesh exactly as
 `extract_mesh(density_thresh, resolution)` does and writes it as OBJ or binary PLY, chosen by the suffix; with `--clean`
-the mesh is first cleaned (`clean`, dgs_mesh_clean), and with `--decimate-target N` then decimated to at most N faces
-(`decimate`, dgs_mesh_decimate).
+the mesh is first cleaned (`clean`, dgs_mesh_clean), with `--remesh [LEN]` then remeshed to edges of about LEN (default
+0.015; `remesh`, dgs_mesh_remesh), and with `--decimate-target N` then decimated to at most N faces (`decimate`,
+dgs_mesh_decimate).
 
 Marching cubes produces the same vertex set as PyMCubes (one vertex per sign-changing grid edge, at the linear
 interpolation of the iso value); on the ambiguous cases the triangulation may differ (a face with two diagonally
@@ -121,9 +124,10 @@ def _mesh_in(name, is_numpy, vertices, faces):
 
 
 def _mesh_out(is_numpy, dev, alloc, V, F):
-    """The output buffers a mesh call allocated after its scratch -> (vertices fp32 [V, 3], faces int64 [F, 3])"""
-    ov = alloc.tensors[1][:V * 12].view(torch.float32).view(V, 3) if V else torch.zeros(0, 3, device=dev)
-    of = alloc.tensors[2][:F * 12].view(torch.int32).view(F, 3).long() if F else torch.zeros(0, 3, dtype=torch.int64,
+    """The output buffers a mesh call allocated last, after its scratch -> (vertices fp32 [V, 3], faces int64 [F, 3])"""
+    out = alloc.tensors[len(alloc.tensors) - bool(V) - bool(F):]  # an empty output is not allocated
+    ov = out[0][:V * 12].view(torch.float32).view(V, 3) if V else torch.zeros(0, 3, device=dev)
+    of = out[-1][:F * 12].view(torch.int32).view(F, 3).long() if F else torch.zeros(0, 3, dtype=torch.int64,
                                                                                               device=dev)
     if is_numpy:
         return ov.cpu().numpy(), of.cpu().numpy()
@@ -190,6 +194,79 @@ def clean_then_decimate(vertices, faces, decimate_target):
     return v, f
 
 
+def remesh(vertices, faces, target_len=0.015, iterations=3, feature_deg=30, max_surf_dist=None, stats=None):
+    """Isotropic remeshing towards edges of target_len (dgs_mesh_remesh; the reference's clean_mesh remeshing step,
+    pymeshlab's meshing_isotropic_explicit_remeshing) -> (vertices, faces): per iteration, split edges longer than
+    4/3 target_len, collapse edges shorter than 4/5 target_len, flip edges towards valence 6, smooth tangentially and
+    project back onto the input surface.  Boundary, non-manifold and feature edges (dihedral angle above feature_deg)
+    are kept; no vertex moves farther than max_surf_dist (default: 1 % of the bounding-box diagonal) from the input by a
+    collapse or flip.  Input and output types as `decimate`; iterations=0 returns the input unchanged, and the result
+    is the same bits on every run.  `stats`, a dict, receives "iterations": per iteration [faces after the split,
+    collapse rounds, flip rounds, 1 if a stage stopped at its 256-round cap]."""
+    is_numpy = _mesh_check("remesh", vertices, faces)
+    L, deg = float(target_len), float(feature_deg)
+    if not (np.isfinite(L) and L > 0):
+        raise ValueError(f"remesh: target_len must be a finite number > 0 (got {target_len!r})")
+    if int(iterations) != iterations or iterations < 0:
+        raise ValueError(f"remesh: iterations must be an integer >= 0 (got {iterations!r})")
+    msd = -1.0 if max_surf_dist is None else float(max_surf_dist)
+    if not (np.isfinite(deg) and np.isfinite(msd)) or (max_surf_dist is not None and msd < 0):
+        raise ValueError(f"remesh: feature_deg and max_surf_dist must be finite, max_surf_dist >= 0 (got "
+                         f"{feature_deg!r}, {max_surf_dist!r})")
+    dev, v, f = _mesh_in("remesh", is_numpy, vertices, faces)
+    alloc = Alloc(dev, _SCRATCH, (str(dev), "remesh"), cached=1)  # only the first scratch: later requests differ
+    vp, fp = C.c_void_p(), C.c_void_p()
+    nv, nf = C.c_longlong(0), C.c_longlong(0)
+    it = int(iterations)
+    st = (C.c_longlong * max(4 * it, 1))()
+    with torch.cuda.device(dev):
+        check(_lib.lib().dgs_mesh_remesh(v.data_ptr(), len(v), f.data_ptr(), len(f), L, it, deg, msd, alloc.cb, None,
+                                         C.byref(vp), C.byref(fp), C.byref(nv), C.byref(nf), st, stream(dev)))
+    if stats is not None:
+        stats["iterations"] = [list(st[4 * i:4 * i + 4]) for i in range(it)]
+    return _mesh_out(is_numpy, dev, alloc, nv.value, nf.value)
+
+
+def closest_points(vertices, faces, queries):
+    """The closest point of the surface (vertices, faces) to each query (dgs_mesh_closest_points, the query `remesh`
+    reprojects with) -> (points float64 [Q, 3], squared distances float64 [Q], faces int64 [Q]): the smallest (squared
+    distance, face index) over all faces, in fp64.  numpy input (queries float [Q, 3]) returns numpy; CUDA tensors
+    return CUDA tensors on their device."""
+    is_numpy = _mesh_check("closest_points", vertices, faces)
+    if len(faces) == 0:
+        raise ValueError("closest_points: the surface has no faces")
+    if queries.ndim != 2 or queries.shape[1] != 3:
+        raise ValueError(f"closest_points: expected queries [Q, 3], got {tuple(queries.shape)}")
+    dev, v, f = _mesh_in("closest_points", is_numpy, vertices, faces)
+    if is_numpy:
+        q = torch.from_numpy(np.ascontiguousarray(queries, np.float64)).to(dev)
+    else:
+        q = queries.detach().to(device=dev, dtype=torch.float64).contiguous()
+    Q = len(q)
+    pts = torch.empty(Q, 3, dtype=torch.float64, device=dev)
+    d2 = torch.empty(Q, dtype=torch.float64, device=dev)
+    fi = torch.empty(Q, dtype=torch.int32, device=dev)
+    alloc = Alloc(dev, _SCRATCH, (str(dev), "closest"), cached=2)  # scratch and grid; the outputs are the caller's
+    with torch.cuda.device(dev):
+        check(_lib.lib().dgs_mesh_closest_points(v.data_ptr(), len(v), f.data_ptr(), len(f), q.data_ptr(), Q,
+                                                 pts.data_ptr(), d2.data_ptr(), fi.data_ptr(), alloc.cb, None,
+                                                 stream(dev)))
+    if is_numpy:
+        return pts.cpu().numpy(), d2.cpu().numpy(), fi.long().cpu().numpy()
+    return pts, d2, fi.long()
+
+
+def clean_remesh_then_decimate(vertices, faces, decimate_target):
+    """The reference's whole extract_mesh post-processing (gs_core.py:862-863): `clean` with its defaults, `remesh` to
+    edges of 0.015 in 3 iterations, then `decimate` to decimate_target faces when more are left.  The signature of
+    extract_mesh's `postprocess`: `extract_mesh(postprocess=clean_remesh_then_decimate)`."""
+    v, f = clean(vertices, faces)
+    v, f = remesh(v, f, 0.015, 3)
+    if len(f) > decimate_target:
+        v, f = decimate(v, f, decimate_target)
+    return v, f
+
+
 class Mesh:
     """The triangle mesh extract_mesh returns: `vertices` float32 [V, 3] and `faces` int64 [F, 3] numpy arrays (the
     attribute names of trimesh.Trimesh)."""
@@ -244,11 +321,22 @@ def parser():
     ap.add_argument("--clean", action="store_true",
                     help="clean first (merge close vertices, drop duplicate / null faces and small components, repair "
                          "non-manifold parts), as the reference's clean_mesh without remeshing")
+    ap.add_argument("--remesh", type=float, nargs="?", const=0.015, default=None, metavar="LEN",
+                    help="remesh isotropically to edges of about LEN (default 0.015), after --clean when both are given")
     return ap
 
 
 def _postprocess(args):
-    """-> extract_mesh keyword arguments for the --clean / --decimate-target flags"""
+    """-> extract_mesh keyword arguments for the --clean / --remesh / --decimate-target flags"""
+    if args.remesh is not None:
+        def chain(v, f, target):
+            if args.clean:
+                v, f = clean(v, f)
+            v, f = remesh(v, f, args.remesh)
+            if target is not None and len(f) > target:
+                v, f = decimate(v, f, target)
+            return v, f
+        return dict(postprocess=chain, decimate_target=args.decimate_target)
     if args.clean and args.decimate_target is not None:
         return dict(postprocess=clean_then_decimate, decimate_target=args.decimate_target)
     if args.clean:

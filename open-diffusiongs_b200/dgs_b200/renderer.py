@@ -278,8 +278,9 @@ class GaussianModel:
         mesh_scale, as in the reference) -> dgs_b200.mesh.Mesh (vertices float32 [V, 3], faces int64 [F, 3]).
         The reference then cleans, remeshes and decimates with pymeshlab; without `postprocess` the raw marching-cubes
         mesh is returned and `decimate_target` is unused.  `postprocess(vertices, faces, decimate_target) -> (vertices,
-        faces)` runs on the numpy arrays: `dgs_b200.mesh.clean_then_decimate` is the reference's chain without its
-        remeshing (clean, then decimate to decimate_target faces), `dgs_b200.mesh.decimate` decimates only."""
+        faces)` runs on the numpy arrays: `dgs_b200.mesh.clean_remesh_then_decimate` is the reference's whole chain
+        (clean, isotropic remeshing to edges of 0.015, then decimate to decimate_target faces),
+        `dgs_b200.mesh.clean_then_decimate` the chain without its remeshing, `dgs_b200.mesh.decimate` decimates only."""
         from . import mesh as _mesh
         occ = self.extract_fields(resolution, num_blocks=64)
         return _mesh.extract_mesh(occ, density_thresh, resolution, postprocess, decimate_target)
