@@ -465,7 +465,9 @@ int dgs_cast_transpose_f32(const float* in, long long in_batch_stride, int batch
 
 /* Building blocks, exported for the unit parity tests (same kernels dgs_dit_forward launches).
  * epi: 0 = bias -> bf16, 1 = bias + GELU(tanh) -> bf16, 2 = out(fp32) += gate[row / rows_per_sample] * (acc + bias),
- *      3 = (acc + bias) -> fp32.   A [M,K], W [N,K] bf16 row-major. */
+ *      3 = (acc + bias) -> fp32, 5 = max(acc + bias, 0) -> bf16 (the LPIPS convolutions).   A [M,K], W [N,K] bf16
+ *      row-major, bias optional (NULL = 0).  N % 32 == 0; A and W 16-byte aligned.  out is [M, ldc] with ldc >= N and
+ *      even; the columns [N, ldc) are left untouched.  Anything else is DGS_ERR_INVALID_ARGUMENT, naming the argument. */
 int dgs_gemm_bf16(const void* A, const void* W, const float* bias, const float* gate, void* out, int M, int N,
                   int K, int epi, int ldc, int gate_stride, int rows_per_sample, void* stream);
 /* qkv [B,N,3,heads,64] bf16 -> out [B,N,heads*64] bf16 = softmax(q k^T / 8) v */
@@ -477,13 +479,16 @@ int dgs_attention_fwd(const void* qkv, void* out, int B, int N, int heads, void*
 int dgs_attention_fwd_train(const void* qkv, void* out, float* lse2, int B, int N, int heads, void* stream);
 int dgs_attention_bwd(const void* qkv, const void* out, const void* dout, float* lse2, float* dsum, void* dqkv, int B,
                       int N, int heads, void* stream);
-/* extended GEMM entry (training epilogues): epi 4 = out(bf16) = acc * gelu'(aux);  aux (bf16 [M,ldc]): epi 1/2 also
- * store acc + bias there;  resid: residual source of epi 2 (NULL = in place);  lda/ldb: operand row strides (0 = K) */
+/* extended GEMM entry (training epilogues): epi 4 = out(bf16) = (acc + bias) * gelu'(aux);  aux (bf16 [M,ldc]): epi 1/2
+ * also store acc + bias there;  resid: residual source of epi 2 ([M,ldc], NULL = in place);  lda/ldb: operand row
+ * strides (0 = K), multiples of 8 and >= K;  ldc as for dgs_gemm_bf16 */
 int dgs_gemm_bf16_ex(const void* A, const void* W, const float* bias, const float* gate, void* out, void* aux,
                      const float* resid, int M, int N, int K, int lda, int ldb, int epi, int ldc, int gate_stride,
                      int rows_per_sample, void* stream);
 /* out[M,N] (fp32, row stride ldc) = A^T W for A [K,M], W [K,N] bf16 row-major with row strides lda / ldb (0 = M / N):
- * the weight-gradient GEMM (K = tokens) on MN-major wgmma operands -- no transposed copies */
+ * the weight-gradient GEMM (K = tokens) on MN-major wgmma operands -- no transposed copies.  N % 32 == 0; lda >= M,
+ * ldb >= N, multiples of 8; ldc (0 = N) >= N; the columns [N, ldc) are left untouched.  Anything else is
+ * DGS_ERR_INVALID_ARGUMENT, naming the argument. */
 int dgs_gemm_bf16_tn(const void* A, const void* W, float* out, int M, int N, int K, int lda, int ldb, int ldc, void* stream);
 /* backward of dgs_ln_modulate: dx (+)= ..., dshift/dscale [B, mod_stride] += ..., dln_w += ... (NULL where absent);
  * stats = scratch of 2*B*rows floats (per-row mean / rstd handed from the row kernel to the column kernel) */

@@ -531,6 +531,10 @@ int gemm_bf16(const void* A, const void* W, int M, int N, int K, int epi, const 
   DGS_REQUIRE(((uintptr_t)A % 16) == 0 && ((uintptr_t)W % 16) == 0, "gemm: operands must be 16-byte aligned");
   // every thread stores column pairs (n, n + 1) of a row, n even: the pairs of every row are aligned when ldc is even
   DGS_REQUIRE(ep.ldc % 2 == 0, "gemm: the output row stride must be even (got ldc=%d)", ep.ldc);
+  // a row stride below the row length would make rows overlap (and the last row run past an M x ldc buffer)
+  DGS_REQUIRE(ep.ldc >= N, "gemm: ldc=%d must be >= N=%d", ep.ldc, N);
+  DGS_REQUIRE(ep.lda == 0 || ep.lda >= K, "gemm: lda=%d must be >= K=%d (or 0)", ep.lda, K);
+  DGS_REQUIRE(ep.ldb == 0 || ep.ldb >= K, "gemm: ldb=%d must be >= K=%d (or 0)", ep.ldb, K);
   const int sms = num_sms();
   DGS_REQUIRE(sms > 0, "gemm: cannot query the device's SM count");
   // The epilogue stages the tile in shared memory for a TMA store (or, in place, a TMA reduce-add) when the output rows
@@ -578,6 +582,9 @@ int gemm_bf16_tn(const void* A, const void* W, int M, int N, int K, const GemmEp
   const int lda = ep.lda ? ep.lda : M, ldb = ep.ldb ? ep.ldb : N, ldc = ep.ldc ? ep.ldc : N;
   DGS_REQUIRE(N % 32 == 0 && lda % 8 == 0 && ldb % 8 == 0, "gemm_tn: need N %% 32 == 0 and row strides %% 8 == 0");
   DGS_REQUIRE(((uintptr_t)A % 16) == 0 && ((uintptr_t)W % 16) == 0, "gemm_tn: operands must be 16-byte aligned");
+  DGS_REQUIRE(lda >= M, "gemm_tn: lda=%d must be >= M=%d (or 0)", lda, M);
+  DGS_REQUIRE(ldb >= N, "gemm_tn: ldb=%d must be >= N=%d (or 0)", ldb, N);
+  DGS_REQUIRE(ldc >= N, "gemm_tn: ldc=%d must be >= N=%d (or 0)", ldc, N);
   const int sms = num_sms();
   const bool wide = (N % 256 == 0) && (ceil_div(M, BM) * (N / 256) >= sms);
   const int BN = wide ? 256 : 128;

@@ -44,52 +44,6 @@ def test_transpose_bf16(M, Cc, f32):
     assert rel(cs, xb.float().sum(0)) < 1e-5
 
 
-@pytest.mark.parametrize("M,N,K", [(4098, 4096, 1024), (300, 256, 128)])
-def test_gemm_training_epilogues(M, N, K):
-    """aux stores of the fc1 / gate epilogues, separate residual source, gelu' epilogue, padded operand strides."""
-    from dgs_b200 import _lib
-    L = _lib.lib()
-    g = torch.Generator(DEV).manual_seed(3)
-    A = torch.randn(M, K, device=DEV, generator=g).to(torch.bfloat16)
-    W = (torch.randn(N, K, device=DEV, generator=g) * 0.03).to(torch.bfloat16)
-    bias = torch.randn(N, device=DEV, generator=g) * 0.1
-    acc = A.float() @ W.float().t() + bias
-    # (1) fc1: out = gelu(acc), aux = acc
-    out = torch.empty(M, N, dtype=torch.bfloat16, device=DEV)
-    aux = torch.empty_like(out)
-    _lib.check(L.dgs_gemm_bf16_ex(ptr(A), ptr(W), ptr(bias), None, ptr(out), ptr(aux), None, M, N, K, 0, 0, 1, N, 0, 1, stream()))
-    assert rel(aux.float(), acc) < 2.5e-3
-    assert rel(out.float(), torch.nn.functional.gelu(acc, approximate="tanh")) < 2.5e-3
-    # (2) gelu' epilogue: out = (A W^T) * gelu'(u)
-    u = (torch.randn(M, N, device=DEV, generator=g) * 1.5).to(torch.bfloat16)
-    uf = u.float().requires_grad_(True)
-    torch.nn.functional.gelu(uf, approximate="tanh").sum().backward()
-    ref = (acc - bias) * uf.grad
-    _lib.check(L.dgs_gemm_bf16_ex(ptr(A), ptr(W), None, None, ptr(out), ptr(u), None, M, N, K, 0, 0, 4, N, 0, 1, stream()))
-    e = rel(out.float(), ref)
-    print(f"dgelu epilogue {M}x{N}x{K}: rel={e:.2e}")
-    assert e < 3e-3  # bf16 output rounding + tanh.approx
-    # (3) gate + residual from another buffer, pre-gate aux
-    rows = M // 2 + 1
-    gate = torch.randn(2, N, device=DEV, generator=g)
-    resid = torch.randn(M, N, device=DEV, generator=g)
-    xo = torch.zeros(M, N, device=DEV)
-    _lib.check(L.dgs_gemm_bf16_ex(ptr(A), ptr(W), ptr(bias), ptr(gate), ptr(xo), ptr(aux), ptr(resid), M, N, K, 0, 0, 2, N,
-                                  N, rows, stream()))
-    gfull = gate[(torch.arange(M, device=DEV) // rows)]
-    assert rel(xo, resid + gfull * acc) < 2e-5
-    assert rel(aux.float(), acc) < 2.5e-3
-    # (4) K-padded operands (row stride > K), fp32 out
-    Kp = K + 64
-    Ap = torch.zeros(M, Kp, dtype=torch.bfloat16, device=DEV)
-    Wp = torch.zeros(N, Kp, dtype=torch.bfloat16, device=DEV)
-    Ap[:, :K - 8], Wp[:, :K - 8] = A[:, :K - 8], W[:, :K - 8]
-    Ap[:, K - 8:] = 9.0  # garbage beyond the logical K: must not be read
-    o32 = torch.empty(M, N, device=DEV)
-    _lib.check(L.dgs_gemm_bf16_ex(ptr(Ap), ptr(Wp), None, None, ptr(o32), None, None, M, N, K - 8, Kp, Kp, 3, N, 0, 1, stream()))
-    assert rel(o32, A[:, :K - 8].float() @ W[:, :K - 8].float().t()) < 2e-5
-
-
 @pytest.mark.parametrize("B,N,H", [(1, 4098, 16), (2, 1026, 16), (1, 128, 2), (2, 200, 2), (1, 77, 4), (1, 64, 2), (1, 130, 1),
                                    (1, 16386, 1)])
 def test_attention_backward_vs_autograd(B, N, H):
@@ -297,20 +251,3 @@ def test_train_steps_reduce_loss_and_track_oracle():
     print("train steps: ours", losses, "oracle", ref_losses)
     assert losses[2] < losses[1] < losses[0]
     assert all(abs(a - b) <= 5e-3 * abs(b) for a, b in zip(losses, ref_losses))
-
-
-@pytest.mark.parametrize("M,N,K", [(128, 128, 64), (1024, 1024, 4098), (896, 1024, 4096), (3072, 1024, 16392),
-                                   (1024, 576, 4096), (200, 160, 104), (4096, 1024, 4098), (1024, 4096, 8196),
-                                   (4096, 4096, 520)])  # the last: enough 128 x 256 tiles for the 256-wide MN-major kernel
-def test_gemm_tn_mn_major_operands(M, N, K):
-    """dW = dY^T X on MN-major wgmma operands (no transposed copies): fp32 accumulation of exact bf16 products."""
-    from dgs_b200 import _lib
-    g = torch.Generator(DEV).manual_seed(M + N + K)
-    A = torch.randn(K, M, device=DEV, generator=g).to(torch.bfloat16)        # dY [tokens, n_out]
-    W = (torch.randn(K, N, device=DEV, generator=g) * 0.1).to(torch.bfloat16)  # X  [tokens, n_in]
-    out = torch.full((M, N), float("nan"), device=DEV)
-    _lib.check(_lib.lib().dgs_gemm_bf16_tn(ptr(A), ptr(W), ptr(out), M, N, K, 0, 0, N, stream()))
-    ref = A.float().t() @ W.float()
-    e = rel(out, ref)
-    print(f"gemm_tn {M}x{N}x{K}: rel={e:.2e}")
-    assert e < 4e-5  # fp32 accumulation-order error grows ~ sqrt(K) (K up to 16392 tokens)

@@ -1,5 +1,4 @@
-"""GPU tests of the DiT kernels at token counts with ragged tails: the in-place gate/residual GEMM epilogue on
-128 x 256 tiles (staged two column blocks at a time, the rows past M clipped by the TMA reduce-add), and the attention
+"""GPU tests of the DiT kernels at token counts with ragged tails (the GEMM's are in test_gemm_gpu.py): the attention
 forward with last key blocks of 1 to 98 valid keys and last query blocks that leave warpgroup 1 without a valid row."""
 import ctypes as C
 
@@ -17,34 +16,6 @@ def rel(a, b):
 
 def stream():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-# 4098 / 8196: 1 and 2 samples of obj-256 (one or two 128 x 256 tiles per CTA); 1, 130, 257: rows tails of 1, 2, 1
-@pytest.mark.parametrize("M", [4098, 8196, 1, 130, 257])
-@pytest.mark.parametrize("K", [1024, 4096])
-def test_gate_residual_tails(M, K):
-    from dgs_b200 import _lib
-    N = 1024
-    g = torch.Generator(DEV).manual_seed(M + K)
-    A = torch.randn(M, K, device=DEV, generator=g).to(torch.bfloat16)
-    W = (torch.randn(N, K, device=DEV, generator=g) * 0.03).to(torch.bfloat16)
-    bias = torch.randn(N, device=DEV, generator=g) * 0.1
-    rows = 4098 if M > 4098 else M  # 8196: two samples, each with its own gate row
-    x = torch.randn(M, N, device=DEV, generator=g)
-    mod = torch.randn((M + rows - 1) // rows, 6 * N, device=DEV, generator=g)
-    gate = mod[:, 2 * N:]
-    ref = x.double() + gate[:, :N].double().repeat_interleave(rows, 0)[:M] * (A.double() @ W.double().t() + bias.double())
-    # guard rows after the output: the clipped tile rows past M must not be written
-    buf = torch.cat([x, torch.full((130, N), 7.0, device=DEV)])
-    _lib.check(_lib.lib().dgs_gemm_bf16(A.data_ptr(), W.data_ptr(), bias.data_ptr(), gate.data_ptr(), buf.data_ptr(), M, N,
-                                        K, 2, N, mod.stride(0), rows, stream()))
-    torch.cuda.synchronize()
-    out = buf[:M]
-    e = rel(out, ref)
-    print(f"gate/residual M={M} K={K}: rel={e:.2e}")
-    assert e < 2e-5
-    assert rel(out[-(M % 128 or 128):], ref[-(M % 128 or 128):]) < 2e-5
-    assert bool((buf[M:] == 7.0).all())
 
 
 # the last key block holds 2, 1, 15, 64, 1, 2 and 98 valid keys; the last query block has as many rows, so its
