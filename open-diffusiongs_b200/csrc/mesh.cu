@@ -13,6 +13,7 @@
 
 #include "dgs_internal.h"
 #include "mc_tables.h"
+#include "sorted_ranges.cuh"
 
 namespace dgs {
 namespace {
@@ -127,14 +128,6 @@ __global__ void __launch_bounds__(kPrepThreads) field_fill_kernel(int P, int nc,
         keys[o] = (uint32_t)((bx * nc + by) * nc + bz);
         vals[o] = (uint32_t)g;
       }
-}
-
-__global__ void field_ranges_kernel(int n, const uint32_t* __restrict__ keys, uint2* __restrict__ ranges) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const uint32_t k = keys[i];
-  if (i == 0 || keys[i - 1] != k) ranges[k].x = i;
-  if (i == n - 1 || keys[i + 1] != k) ranges[k].y = i + 1;
 }
 
 // One warp per grid block, eight blocks per CTA.  At the default 4^3 points per block a warp holds the block's 64
@@ -358,7 +351,7 @@ int dgs_mesh_field(int P, const float* xyz, const float* scaling, const float* r
     DGS_POST_LAUNCH();
     DGS_CUDA_OK(cub::DeviceRadixSort::SortPairs(ps.temp, ps.temp_bytes, ps.keys_in, ps.keys, ps.vals_in, ps.vals, n, 0,
                                                 end_bit, st));
-    field_ranges_kernel<<<ceil_div(n, 256), 256, 0, st>>>(n, ps.keys, fs.ranges);
+    ranges_kernel<<<ceil_div(n, 256), 256, 0, st>>>(n, ps.keys, fs.ranges);
     DGS_POST_LAUNCH();
     field_eval_kernel<<<(unsigned)((nblocks + kEvalWarps - 1) / kEvalWarps), 32 * kEvalWarps, 0, st>>>(
         grid, fs.ranges, ps.vals, fs.rec, occ, block_counts);

@@ -14,47 +14,22 @@
 // Components (stages 5, 6) and fans (stage 8) are lock-free union-find over the sorted half-edges; a root is the
 // smallest member, i.e. the component's lowest face / the fan's corner in its lowest face.  Stage 7 walks its sorted
 // candidates in one thread.
-#include <cub/cub.cuh>
-
-#include <algorithm>
 #include <cmath>
-#include <cstring>
 
-#include "dgs_internal.h"
-#include "mesh_edges.cuh"
+#include "mesh_common.cuh"
 
 namespace dgs {
 namespace {
 
-constexpr unsigned long long kNoKey = ~0ull;
-constexpr unsigned kFull = 0xffffffffu;
 constexpr int kCellBits = 21;
 
 struct Counters {
-  unsigned long long bad_face;  // smallest face with an index outside [0, V); kNoKey if none
+  FaceCheck chk;                // stage 1's, then its box is stage 4's (the box of what is left)
   int selected;                 // faces kept by the last compaction
   int undecided;                // vertices left undecided by the last merge round
   int counted;                  // faces left by the stage before a combined compaction (3 before 4, 5 before 6)
   int candidates;               // stage 7's faces with an edge of more than two faces
-  unsigned box[6];              // order-preserving keys of the bounding box: min x y z, max x y z
 };
-
-// Order-preserving uint key of a float, and back (the host reads boxes too).
-__host__ __device__ __forceinline__ unsigned fkey(float x) {
-  unsigned u;
-  memcpy(&u, &x, sizeof(u));
-  return (u & 0x80000000u) ? ~u : u | 0x80000000u;
-}
-__host__ __device__ __forceinline__ float fval(unsigned k) {
-  const unsigned u = (k & 0x80000000u) ? k & 0x7fffffffu : ~k;
-  float x;
-  memcpy(&x, &u, sizeof(x));
-  return x;
-}
-
-__device__ __forceinline__ double3 load(const float* __restrict__ pos, int v) {
-  return make_double3(pos[3 * v], pos[3 * v + 1], pos[3 * v + 2]);
-}
 
 // |(b - a) x (c - a)| (fp64, no contraction)
 __device__ double doubled_area(const float* __restrict__ pos, int3 f) {
@@ -70,17 +45,6 @@ __host__ __device__ __forceinline__ double box_diag(const unsigned* b) {
                dz = (double)fval(b[5]) - (double)fval(b[2]);
   return sqrt(dx * dx + dy * dy + dz * dz);
 }
-
-struct Box {
-  unsigned lo[3] = {kFull, kFull, kFull}, hi[3] = {0u, 0u, 0u};
-  __device__ void add(const float* __restrict__ pos, int v) {
-    for (int k = 0; k < 3; k++) {
-      const unsigned q = fkey(pos[3 * v + k]);
-      lo[k] = min(lo[k], q);
-      hi[k] = max(hi[k], q);
-    }
-  }
-};
 
 // Merges the lane's box (and one to *size) into boxes[6 key] for key >= 0.  Every lane of the warp calls it; when the
 // warp's valid lanes share one key (the common case: neighbouring faces in one component) the warp reduces first.
@@ -156,25 +120,6 @@ __global__ void box_init_kernel(int n, unsigned* __restrict__ boxes) {
   if (i < 6 * n) boxes[i] = i % 6 < 3 ? kFull : 0u;
 }
 
-// ----------------------------------------------------------------------------------------- stage 1: check, box
-// The smallest bad face, and the box of the vertices the valid faces reference.
-__global__ void validate_kernel(int F, int V, const int3* __restrict__ faces, const float* __restrict__ pos,
-                                Counters* __restrict__ ctr, uint32_t* __restrict__ used) {
-  const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  Box b;
-  bool ok = false;
-  if (f < F) {
-    const int3 t = faces[f];
-    ok = t.x >= 0 && t.x < V && t.y >= 0 && t.y < V && t.z >= 0 && t.z < V;
-    if (!ok) atomicMin(&ctr->bad_face, (unsigned long long)f);
-    else {
-      b.add(pos, t.x); b.add(pos, t.y); b.add(pos, t.z);
-      used[t.x] = used[t.y] = used[t.z] = 1;
-    }
-  }
-  flush(ctr->box, nullptr, ok ? 0 : -1, b);
-}
-
 // ----------------------------------------------------------------------------------------- stage 2: merge
 struct Grid {
   double mn[3], cell, r;
@@ -239,16 +184,6 @@ __global__ void merge_round_kernel(int V, const float* __restrict__ pos, Grid g,
   if (out < 0) atomicAdd(&ctr->undecided, 1);
 }
 
-// Faces re-indexed onto their seeds; a face that now repeats a vertex goes.
-__global__ void remap_kernel(int F, int3* __restrict__ faces, const int* __restrict__ rep, uint8_t* __restrict__ keep) {
-  const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  if (f >= F) return;
-  int3 t = faces[f];
-  t = make_int3(rep[t.x], rep[t.y], rep[t.z]);
-  faces[f] = t;
-  keep[f] = t.x != t.y && t.y != t.z && t.x != t.z;
-}
-
 // ----------------------------------------------------------------------------------------- stages 3, 4
 // LSD sort of the sorted triples (a <= b <= c): by c, then stably by (a, b); ties stay in face order.
 __global__ void dup_key_c_kernel(int F, const int3* __restrict__ faces, uint32_t* __restrict__ keys,
@@ -295,7 +230,7 @@ __global__ void null_kernel(int F, const int3* __restrict__ faces, const float* 
     if (ok) { b.add(pos, t.x); b.add(pos, t.y); b.add(pos, t.z); }
   }
   warp_count(&ctr->counted, nondup);
-  flush(ctr->box, nullptr, ok ? 0 : -1, b);
+  flush(ctr->chk.box, nullptr, ok ? 0 : -1, b);
 }
 
 // ----------------------------------------------------------------------------------------- stages 5, 6
@@ -418,45 +353,19 @@ __global__ void reindex_kernel(int n, int* __restrict__ fv, const int* __restric
   if (id >= 0) fv[c] = id;
 }
 
-// ----------------------------------------------------------------------------------------- stage 9
-__global__ void used_kernel(int n, const int* __restrict__ fv, uint32_t* __restrict__ used) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c < n) used[fv[c]] = 1;
-}
-__global__ void emit_kernel(int V, int NV, int F, const float* __restrict__ pos, const int* __restrict__ src,
-                            const int3* __restrict__ faces, const uint32_t* __restrict__ used,
-                            const uint32_t* __restrict__ vscan, float* __restrict__ out_v, int3* __restrict__ out_f) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < NV && used[i]) {
-    const uint32_t o = vscan[i] - 1;
-    const int s = i < V ? i : src[i - V];
-    out_v[3 * o] = pos[3 * s];
-    out_v[3 * o + 1] = pos[3 * s + 1];
-    out_v[3 * o + 2] = pos[3 * s + 2];
-  }
-  if (i < F) {
-    const int3 t = faces[i];
-    out_f[i] = make_int3((int)vscan[t.x] - 1, (int)vscan[t.y] - 1, (int)vscan[t.z] - 1);
-  }
-}
-
 // All scratch, sized once from V and F (n = 3F half-edges / corners; at most n vertex copies).
-struct Scratch {
+struct Scratch : MeshScratch {
   Counters* ctr;
   int *rep_a, *rep_b, *parent, *copy_id, *src, *live, *csize;
-  uint32_t *used, *vscan, *cval_in, *cval, *hval_in, *hval, *heads, *ikey_in, *ikey, *ival_in, *vfaces, *edge_of;
-  unsigned long long *ckey_in, *ckey, *hkey_in, *hkey;
+  uint32_t *cval_in, *cval;
+  unsigned long long *ckey_in, *ckey;
   unsigned* cbox;
-  uint2* vrange;
-  int3 *faces, *faces_alt;
-  uint8_t* keep;
-  void* temp;
-  size_t temp_bytes;
 
-  size_t carve(void* base, int V, int F, int vbits) {
-    const int n = 3 * F, NV = V + n;
+  size_t carve(void* base, int V, int F) {
+    const int n = 3 * F;
     Carver cv(base);
     ctr = cv.take<Counters>(1);
+    carve_mesh(cv, V, F, V + n);
     rep_a = cv.take<int>(V);
     rep_b = cv.take<int>(V);
     parent = cv.take<int>(n);
@@ -464,40 +373,17 @@ struct Scratch {
     src = cv.take<int>(n);
     live = cv.take<int>(n);
     csize = cv.take<int>(F);
-    used = cv.take<uint32_t>(NV);
-    vscan = cv.take<uint32_t>(NV);
     cval_in = cv.take<uint32_t>(V);
     cval = cv.take<uint32_t>(V);
-    hval_in = cv.take<uint32_t>(n);
-    hval = cv.take<uint32_t>(n);
-    heads = cv.take<uint32_t>(n);
-    ikey_in = cv.take<uint32_t>(n);
-    ikey = cv.take<uint32_t>(n);
-    ival_in = cv.take<uint32_t>(n);
-    vfaces = cv.take<uint32_t>(n);
-    edge_of = cv.take<uint32_t>(n);
     ckey_in = cv.take<unsigned long long>(V);
     ckey = cv.take<unsigned long long>(V);
-    hkey_in = cv.take<unsigned long long>(n);
-    hkey = cv.take<unsigned long long>(n);
     cbox = cv.take<unsigned>(6 * (size_t)F);
-    vrange = cv.take<uint2>(V);
-    faces = cv.take<int3>(F);
-    faces_alt = cv.take<int3>(F);
-    keep = cv.take<uint8_t>(F);
     size_t t = 0;
-    temp_bytes = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, t, ckey_in, ckey, cval_in, cval, V, 0, 3 * kCellBits);
-    temp_bytes = std::max(temp_bytes, t);
+    need(t);
     cub::DeviceRadixSort::SortPairs(nullptr, t, hkey_in, hkey, hval_in, hval, n, 0, 64);
-    temp_bytes = std::max(temp_bytes, t);
-    cub::DeviceRadixSort::SortPairs(nullptr, t, ikey_in, ikey, ival_in, vfaces, n, 0, vbits);
-    temp_bytes = std::max(temp_bytes, t);
-    cub::DeviceScan::InclusiveSum(nullptr, t, heads, heads, std::max(n, NV));
-    temp_bytes = std::max(temp_bytes, t);
-    cub::DeviceSelect::Flagged(nullptr, t, faces, keep, faces_alt, static_cast<int*>(nullptr), F);
-    temp_bytes = std::max(temp_bytes, t);
-    temp = cv.take<char>(temp_bytes);
+    need(t);
+    carve_temp(cv);
     return cv.bytes();
   }
 };
@@ -507,15 +393,13 @@ struct Scratch {
 
 using namespace dgs;
 
-// Keeps the faces flagged in s.keep (face order), reads their number back and makes them s.faces.
-#define CLEAN_COMPACT(F)                                                                                            \
-  do {                                                                                                              \
-    DGS_CUDA_OK(cub::DeviceSelect::Flagged(s.temp, s.temp_bytes, s.faces, s.keep, s.faces_alt, &s.ctr->selected, F, \
-                                           st));                                                                    \
-    DGS_CUDA_OK(cudaMemcpyAsync(&h, s.ctr, sizeof(h), cudaMemcpyDeviceToHost, st));                                 \
-    DGS_CUDA_OK(cudaStreamSynchronize(st));                                                                         \
-    std::swap(s.faces, s.faces_alt);                                                                                \
-    F = h.selected;                                                                                                 \
+// Keeps the faces flagged in s.keep (face order) as s.faces and reads their number back.
+#define CLEAN_COMPACT(F)                                                          \
+  do {                                                                            \
+    DGS_CUDA_OK(s.compact(F, &s.ctr->selected, st));                              \
+    DGS_CUDA_OK(cudaMemcpyAsync(&h, s.ctr, sizeof(h), cudaMemcpyDeviceToHost, st)); \
+    DGS_CUDA_OK(cudaStreamSynchronize(st));                                       \
+    F = h.selected;                                                               \
   } while (0)
 
 extern "C" {
@@ -524,75 +408,55 @@ int dgs_mesh_clean(const float* vertices, long long num_vertices, const int* fac
                    long long min_f, double min_d, int repair, dgs_alloc_fn alloc, void* alloc_user,
                    float** out_vertices, int** out_faces, long long* out_num_vertices, long long* out_num_faces,
                    int* merge_rounds, long long* stage_faces, void* stream) {
-  DGS_REQUIRE(alloc && out_vertices && out_faces && out_num_vertices && out_num_faces,
-              "mesh clean: alloc and the four outputs must not be NULL");
-  DGS_REQUIRE(num_vertices >= 0 && num_faces >= 0, "mesh clean: negative size (%lld vertices, %lld faces)", num_vertices,
-              num_faces);
-  DGS_REQUIRE(num_vertices + 3 * num_faces <= 0x7fffffffLL,
-              "mesh clean: %lld vertices / %lld faces is too many (V + 3F must be at most 2^31 - 1)", num_vertices,
-              num_faces);
-  DGS_REQUIRE((num_vertices == 0 || vertices) && (num_faces == 0 || faces),
-              "mesh clean: vertices and faces must not be NULL");
+  const char* name = "mesh clean";
+  const MeshOut out{alloc, alloc_user, out_vertices, out_faces, out_num_vertices, out_num_faces};
+  const int rc = check_mesh_args(name, vertices, num_vertices, faces, num_faces,
+                                 num_vertices + 3 * num_faces <= 0x7fffffffLL, "V + 3F must be at most 2^31 - 1", out);
+  if (rc != DGS_OK) return rc;
   DGS_REQUIRE(std::isfinite(v_pct) && std::isfinite(min_d), "mesh clean: v_pct and min_d must be finite");
-  *out_vertices = nullptr;
-  *out_faces = nullptr;
-  *out_num_vertices = *out_num_faces = 0;
+  out.set(nullptr, nullptr, 0, 0);
   if (merge_rounds) *merge_rounds = 0;
   if (stage_faces)
     for (int k = 0; k < 9; k++) stage_faces[k] = 0;
   if (num_faces == 0) return DGS_OK;  // nothing is referenced: the result is empty
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const int V = (int)num_vertices;
+  const int V = (int)num_vertices, vbits = bits_for(V);
   int F = (int)num_faces;
-  int vbits = 1;
-  while (vbits < 31 && (1LL << vbits) < num_vertices) vbits++;
   Scratch s;
-  const size_t bytes = s.carve(nullptr, V, F, vbits);
-  void* buf = alloc(bytes, alloc_user);
-  if (!buf) { set_error("mesh clean: scratch allocation failed (%zu bytes)", bytes); return DGS_ERR_ALLOC; }
-  s.carve(buf, V, F, vbits);
+  void* buf = out.scratch(name, s.carve(nullptr, V, F));
+  if (!buf) return DGS_ERR_ALLOC;
+  s.carve(buf, V, F);
   const int3* in_faces = reinterpret_cast<const int3*>(faces);
   long long counts[9];
   Counters h;
   const int T = kThreads;
 
   // 1. check the indices; the box of the referenced vertices
-  DGS_CUDA_OK(cudaMemsetAsync(s.ctr, 0, sizeof(Counters), st));
-  DGS_CUDA_OK(cudaMemsetAsync(&s.ctr->bad_face, 0xff, sizeof(unsigned long long), st));
-  box_init_kernel<<<1, 32, 0, st>>>(1, s.ctr->box);
-  DGS_POST_LAUNCH();
-  DGS_CUDA_OK(cudaMemsetAsync(s.used, 0, (size_t)V * sizeof(uint32_t), st));
-  validate_kernel<<<ceil_div(F, T), T, 0, st>>>(F, V, in_faces, vertices, s.ctr, s.used);
-  DGS_POST_LAUNCH();
   DGS_CUDA_OK(cudaMemcpyAsync(s.faces, in_faces, (size_t)F * sizeof(int3), cudaMemcpyDeviceToDevice, st));
-  DGS_CUDA_OK(cudaMemcpyAsync(&h, s.ctr, sizeof(h), cudaMemcpyDeviceToHost, st));
-  DGS_CUDA_OK(cudaStreamSynchronize(st));  // indices must be valid before any kernel follows them
-  if (h.bad_face != kNoKey) {
-    int t[3] = {0, 0, 0};
-    DGS_CUDA_OK(cudaMemcpyAsync(t, in_faces + h.bad_face, sizeof(t), cudaMemcpyDeviceToHost, st));
-    DGS_CUDA_OK(cudaStreamSynchronize(st));
-    set_error("mesh clean: face %llu = (%d, %d, %d) has an index outside [0, %d)", h.bad_face, t[0], t[1], t[2], V);
-    return DGS_ERR_INVALID_ARGUMENT;
+  {
+    const int rc = check_faces(name, vertices, V, in_faces, F, false, s.used, &s.ctr->chk, h.chk, st);
+    if (rc != DGS_OK) return rc;
   }
   counts[0] = F;
 
   // 2. merge close vertices
   int rounds = 0;
   if (v_pct > 0) {
-    const double r = (v_pct / 100.0) * box_diag(h.box);
+    const double r = (v_pct / 100.0) * box_diag(h.chk.box);
     const int gv = ceil_div(V, T);
     if (r > 0) {
       Grid g;
       double ext = 0.0;
       for (int k = 0; k < 3; k++) {
-        g.mn[k] = (double)fval(h.box[k]);
-        ext = std::max(ext, (double)fval(h.box[3 + k]) - g.mn[k]);
+        g.mn[k] = (double)fval(h.chk.box[k]);
+        ext = std::max(ext, (double)fval(h.chk.box[3 + k]) - g.mn[k]);
       }
       // a margin over r keeps every pair closer than r within adjacent cells; at most 2^21 - 1 cells per axis
       g.cell = std::max(r * (1.0 + 0x1p-20), ext / ((1 << kCellBits) - 2));
       g.r = r;
       for (int k = 0; k < 3; k++)
-        g.n[k] = std::min((int)std::floor(((double)fval(h.box[3 + k]) - g.mn[k]) / g.cell) + 1, (1 << kCellBits) - 1);
+        g.n[k] =
+            std::min((int)std::floor(((double)fval(h.chk.box[3 + k]) - g.mn[k]) / g.cell) + 1, (1 << kCellBits) - 1);
       cell_key_kernel<<<gv, T, 0, st>>>(V, vertices, s.used, g, s.ckey_in, s.cval_in);
       DGS_POST_LAUNCH();
       DGS_CUDA_OK(cub::DeviceRadixSort::SortPairs(s.temp, s.temp_bytes, s.ckey_in, s.ckey, s.cval_in, s.cval, V, 0, 64,
@@ -632,7 +496,7 @@ int dgs_mesh_clean(const float* vertices, long long num_vertices, const int* fac
     dup_flag_kernel<<<g, T, 0, st>>>(F, s.faces, s.hkey, s.hval, s.keep);
     DGS_POST_LAUNCH();
     DGS_CUDA_OK(cudaMemsetAsync(&s.ctr->counted, 0, sizeof(int), st));
-    box_init_kernel<<<1, 32, 0, st>>>(1, s.ctr->box);
+    box_init_kernel<<<1, 32, 0, st>>>(1, s.ctr->chk.box);
     DGS_POST_LAUNCH();
     null_kernel<<<g, T, 0, st>>>(F, s.faces, vertices, s.keep, s.ctr);
     DGS_POST_LAUNCH();
@@ -647,7 +511,7 @@ int dgs_mesh_clean(const float* vertices, long long num_vertices, const int* fac
   counts[4] = F;
   if (F > 0 && (min_d > 0 || min_f > 0)) {
     const int n = 3 * F, g = ceil_div(F, T);
-    DGS_CUDA_OK(sort_edges(n, s.faces, vbits, s.hkey_in, s.hkey, s.hval_in, s.hval, s.heads, s.temp, s.temp_bytes, st));
+    DGS_CUDA_OK(s.sort_edges(F, V, st));
     iota_kernel<<<g, T, 0, st>>>(F, s.parent);
     DGS_POST_LAUNCH();
     face_union_kernel<<<ceil_div(n, T), T, 0, st>>>(n, s.hkey, s.hval, s.parent);
@@ -659,7 +523,7 @@ int dgs_mesh_clean(const float* vertices, long long num_vertices, const int* fac
     DGS_CUDA_OK(cudaMemsetAsync(s.csize, 0, (size_t)F * sizeof(int), st));
     comp_stats_kernel<<<g, T, 0, st>>>(F, s.faces, vertices, s.parent, s.cbox, s.csize);
     DGS_POST_LAUNCH();
-    const double min_diag = min_d > 0 ? (min_d / 100.0) * box_diag(h.box) : -1.0;
+    const double min_diag = min_d > 0 ? (min_d / 100.0) * box_diag(h.chk.box) : -1.0;
     DGS_CUDA_OK(cudaMemsetAsync(&s.ctr->counted, 0, sizeof(int), st));
     comp_flag_kernel<<<g, T, 0, st>>>(F, s.parent, s.cbox, s.csize, min_diag, min_f > 0 ? min_f : 0, s.keep, s.ctr);
     DGS_POST_LAUNCH();
@@ -671,7 +535,7 @@ int dgs_mesh_clean(const float* vertices, long long num_vertices, const int* fac
   // 7. non-manifold edges
   if (repair && F > 0) {
     const int n = 3 * F, g = ceil_div(F, T);
-    DGS_CUDA_OK(sort_edges(n, s.faces, vbits, s.hkey_in, s.hkey, s.hval_in, s.hval, s.heads, s.temp, s.temp_bytes, st));
+    DGS_CUDA_OK(s.sort_edges(F, V, st));
     edge_count_kernel<<<ceil_div(n, T), T, 0, st>>>(n, s.hkey, s.hval, s.heads, s.edge_of, s.live);
     DGS_POST_LAUNCH();
     DGS_CUDA_OK(cudaMemsetAsync(&s.ctr->candidates, 0, sizeof(int), st));
@@ -691,15 +555,14 @@ int dgs_mesh_clean(const float* vertices, long long num_vertices, const int* fac
   if (repair && F > 0) {
     const int n = 3 * F, gn = ceil_div(n, T);
     int* fv = reinterpret_cast<int*>(s.faces);
-    DGS_CUDA_OK(sort_edges(n, s.faces, vbits, s.hkey_in, s.hkey, s.hval_in, s.hval, s.heads, s.temp, s.temp_bytes, st));
+    DGS_CUDA_OK(s.sort_edges(F, V, st));
     iota_kernel<<<gn, T, 0, st>>>(n, s.parent);
     DGS_POST_LAUNCH();
     fan_union_kernel<<<gn, T, 0, st>>>(n, s.hkey, s.hval, fv, s.parent);
     DGS_POST_LAUNCH();
     flatten_kernel<<<gn, T, 0, st>>>(n, s.parent);
     DGS_POST_LAUNCH();
-    DGS_CUDA_OK(vertex_faces(F, V, s.faces, vbits, s.ikey_in, s.ikey, s.ival_in, s.vfaces, s.vrange, s.temp,
-                             s.temp_bytes, st));
+    DGS_CUDA_OK(s.vertex_faces(F, V, st));
     copy_flag_kernel<<<gn, T, 0, st>>>(n, s.ikey, s.vfaces, s.vrange, s.faces, s.parent, s.heads);
     DGS_POST_LAUNCH();
     DGS_CUDA_OK(cub::DeviceScan::InclusiveSum(s.temp, s.temp_bytes, s.heads, s.vscan, n, st));
@@ -718,31 +581,10 @@ int dgs_mesh_clean(const float* vertices, long long num_vertices, const int* fac
   counts[7] = counts[8] = F;
 
   // 9. compact: referenced vertices (copies last) in index order, faces remapped
-  const int NV = V + copies;
-  DGS_CUDA_OK(cudaMemsetAsync(s.used, 0, (size_t)NV * sizeof(uint32_t), st));
-  if (F > 0) {
-    used_kernel<<<ceil_div(3 * F, T), T, 0, st>>>(3 * F, reinterpret_cast<const int*>(s.faces), s.used);
-    DGS_POST_LAUNCH();
-  }
-  DGS_CUDA_OK(cub::DeviceScan::InclusiveSum(s.temp, s.temp_bytes, s.used, s.vscan, NV, st));
-  uint32_t nv = 0;
-  DGS_CUDA_OK(cudaMemcpyAsync(&nv, s.vscan + NV - 1, sizeof(nv), cudaMemcpyDeviceToHost, st));
-  DGS_CUDA_OK(cudaStreamSynchronize(st));  // the vertex count sizes the output
   if (merge_rounds) *merge_rounds = rounds;
   if (stage_faces)
     for (int k = 0; k < 9; k++) stage_faces[k] = counts[k];
-  if (F == 0) return DGS_OK;
-  float* v = reinterpret_cast<float*>(alloc((size_t)nv * 3 * sizeof(float), alloc_user));
-  int* f = reinterpret_cast<int*>(alloc((size_t)F * 3 * sizeof(int), alloc_user));
-  if (!v || !f) { set_error("mesh clean: output allocation failed"); return DGS_ERR_ALLOC; }
-  emit_kernel<<<ceil_div(std::max(NV, F), T), T, 0, st>>>(V, NV, F, vertices, s.src, s.faces, s.used, s.vscan, v,
-                                                          reinterpret_cast<int3*>(f));
-  DGS_POST_LAUNCH();
-  *out_vertices = v;
-  *out_faces = f;
-  *out_num_vertices = nv;
-  *out_num_faces = F;
-  return DGS_OK;
+  return emit_mesh(name, s, V, V + copies, F, vertices, s.src, nullptr, out, st);
 }
 
 }  // extern "C"

@@ -1,31 +1,16 @@
-// mesh_collapse.cuh -- what mesh_decimate.cu and mesh_remesh.cu share to collapse edges in parallel rounds: the fp64
-// vector helpers, the link condition, the fold-over test, and the two-hop minimum (m1, m2) that selects independent
-// edges.  Both files are compiled with the same helpers, so a collapse test means the same thing in each.
+// mesh_collapse.cuh -- what mesh_decimate.cu and mesh_remesh.cu share to collapse edges in parallel rounds: the link
+// condition, the fold-over test, and the two-hop minimum (m1, m2) that selects independent edges.  Both files are
+// compiled with the same helpers, so a collapse test means the same thing in each.
 #pragma once
-#include "mesh_edges.cuh"
+#include "mesh_common.cuh"
 
 namespace dgs {
 namespace {
-
-constexpr unsigned long long kNoKey = ~0ull;
 
 struct Edge {
   int a, b;  // a < b
   int c, d;  // the apexes of its two faces; -1 unless it has exactly two
 };
-
-__device__ __forceinline__ double3 sub(double3 u, double3 v) { return make_double3(u.x - v.x, u.y - v.y, u.z - v.z); }
-__device__ __forceinline__ double dot(double3 u, double3 v) { return u.x * v.x + u.y * v.y + u.z * v.z; }
-__device__ __forceinline__ double3 cross(double3 u, double3 v) {
-  return make_double3(u.y * v.z - u.z * v.y, u.z * v.x - u.x * v.z, u.x * v.y - u.y * v.x);
-}
-__device__ __forceinline__ double3 load(const float* __restrict__ pos, int v) {
-  return make_double3(pos[3 * v], pos[3 * v + 1], pos[3 * v + 2]);
-}
-__device__ __forceinline__ double3 round_f32(double3 v) {
-  return make_double3((double)(float)v.x, (double)(float)v.y, (double)(float)v.z);
-}
-__device__ __forceinline__ bool has(int3 f, int x) { return f.x == x || f.y == x || f.z == x; }
 
 // Moving v to p keeps the orientation of every face around v that does not contain `other` (those die): its normal
 // after the move has a positive dot product with its normal before.  Faces with zero area before are exempt.

@@ -25,11 +25,6 @@
 // are kept.  Apply: the lower index survives at the new position with Q_a += Q_b, b becomes a in every face (winding
 // kept), the two faces with both die and the faces are compacted in order.  Rounds stop at F <= target or when no
 // edge can be taken.  Finish: referenced vertices are compacted in index order and the faces remapped.
-#include <cub/cub.cuh>
-
-#include <algorithm>
-
-#include "dgs_internal.h"
 #include "mesh_collapse.cuh"
 
 namespace dgs {
@@ -42,7 +37,7 @@ struct Quadric {
 };
 
 struct Counters {
-  unsigned long long bad_face;  // smallest face with an index out of range or repeated; kNoKey if none
+  FaceCheck chk;
   int num_edges, num_selected, num_faces;
 };
 
@@ -97,15 +92,6 @@ __device__ double3 placement(const double* q, double3 pa, double3 pb, double& co
 }
 
 // ---------------------------------------------------------------------------------------------------------- setup
-__global__ void validate_kernel(int F, int V, const int3* __restrict__ faces, Counters* __restrict__ ctr) {
-  const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  if (f >= F) return;
-  const int3 t = faces[f];
-  const bool ok = t.x >= 0 && t.x < V && t.y >= 0 && t.y < V && t.z >= 0 && t.z < V && t.x != t.y && t.y != t.z &&
-                  t.x != t.z;
-  if (!ok) atomicMin(&ctr->bad_face, (unsigned long long)f);
-}
-
 __global__ void vertex_quadric_kernel(int V, const float* __restrict__ pos, const int3* __restrict__ faces,
                                       const uint2* __restrict__ vrange, const uint32_t* __restrict__ vfaces,
                                       Quadric* __restrict__ Q) {
@@ -211,111 +197,40 @@ __global__ void apply_kernel(const Counters* __restrict__ ctr, const Edge* __res
   to[e.b] = e.a;
 }
 
-__global__ void remap_kernel(int F, int3* __restrict__ faces, const int* __restrict__ to, uint8_t* __restrict__ alive) {
-  const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  if (f >= F) return;
-  int3 t = faces[f];
-  if (to[t.x] >= 0) t.x = to[t.x];
-  if (to[t.y] >= 0) t.y = to[t.y];
-  if (to[t.z] >= 0) t.z = to[t.z];
-  faces[f] = t;
-  alive[f] = t.x != t.y && t.y != t.z && t.x != t.z;
-}
-
-// ---------------------------------------------------------------------------------------------------------- finish
-__global__ void used_kernel(int n, const int3* __restrict__ faces, uint32_t* __restrict__ used) {
-  const int h = blockIdx.x * blockDim.x + threadIdx.x;
-  if (h >= n) return;
-  used[corner(faces[h / 3], h % 3)] = 1;
-}
-
-__global__ void emit_kernel(int V, int F, const float* __restrict__ pos, const int3* __restrict__ faces,
-                            const uint32_t* __restrict__ used, const uint32_t* __restrict__ vscan,
-                            float* __restrict__ out_v, int3* __restrict__ out_f) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < V && used[i]) {
-    const uint32_t o = vscan[i] - 1;
-    out_v[3 * o] = pos[3 * i];
-    out_v[3 * o + 1] = pos[3 * i + 1];
-    out_v[3 * o + 2] = pos[3 * i + 2];
-  }
-  if (i < F) {
-    const int3 t = faces[i];
-    out_f[i] = make_int3((int)vscan[t.x] - 1, (int)vscan[t.y] - 1, (int)vscan[t.z] - 1);
-  }
-}
-
 // All scratch, sized once from V and F (n = 3F half-edges, at most n edges).
-struct Scratch {
+struct Scratch : MeshScratch {
   Counters* ctr;
   float* pos;
   Quadric* Q;
   uint8_t* lock;
   int* to;
-  unsigned long long *m1, *m2;
-  uint32_t *used, *vscan;
-  uint2* vrange;
-  int3 *faces, *faces_alt;
-  uint8_t* alive;
-  unsigned long long *hkey_in, *hkey, *skey, *skey_sorted, *ekey;
-  uint32_t *hval_in, *hval, *ikey_in, *ikey, *ival_in, *vfaces, *heads, *edge_of;
+  unsigned long long *m1, *m2, *skey, *skey_sorted, *ekey;
   Edge* edges;
   float3* eplace;
-  void* temp;
-  size_t temp_bytes;
 
-  size_t carve(void* base, int V, int F, int vbits) {
+  size_t carve(void* base, int V, int F) {
     const int n = 3 * F;
     Carver cv(base);
     ctr = cv.take<Counters>(1);
+    carve_mesh(cv, V, F, V);
     pos = cv.take<float>(3 * (size_t)V);
     Q = cv.take<Quadric>(V);
     lock = cv.take<uint8_t>(V);
     to = cv.take<int>(V);
     m1 = cv.take<unsigned long long>(V);
     m2 = cv.take<unsigned long long>(V);
-    used = cv.take<uint32_t>(V);
-    vscan = cv.take<uint32_t>(V);
-    vrange = cv.take<uint2>(V);
-    faces = cv.take<int3>(F);
-    faces_alt = cv.take<int3>(F);
-    alive = cv.take<uint8_t>(F);
-    hkey_in = cv.take<unsigned long long>(n);
-    hkey = cv.take<unsigned long long>(n);
     skey = cv.take<unsigned long long>(n);
     skey_sorted = cv.take<unsigned long long>(n);
     ekey = cv.take<unsigned long long>(n);
-    hval_in = cv.take<uint32_t>(n);
-    hval = cv.take<uint32_t>(n);
-    ikey_in = cv.take<uint32_t>(n);
-    ikey = cv.take<uint32_t>(n);
-    ival_in = cv.take<uint32_t>(n);
-    vfaces = cv.take<uint32_t>(n);
-    heads = cv.take<uint32_t>(n);
-    edge_of = cv.take<uint32_t>(n);
     edges = cv.take<Edge>(n);
     eplace = cv.take<float3>(n);
     size_t t = 0;
-    temp_bytes = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, t, hkey_in, hkey, hval_in, hval, n, 0, 2 * vbits);
-    temp_bytes = std::max(temp_bytes, t);
-    cub::DeviceRadixSort::SortPairs(nullptr, t, ikey_in, ikey, ival_in, vfaces, n, 0, vbits);
-    temp_bytes = std::max(temp_bytes, t);
     cub::DeviceRadixSort::SortKeys(nullptr, t, skey, skey_sorted, n);
-    temp_bytes = std::max(temp_bytes, t);
-    cub::DeviceScan::InclusiveSum(nullptr, t, heads, heads, std::max(n, V));
-    temp_bytes = std::max(temp_bytes, t);
-    cub::DeviceSelect::Flagged(nullptr, t, faces, alive, faces_alt, static_cast<int*>(nullptr), F);
-    temp_bytes = std::max(temp_bytes, t);
-    temp = cv.take<char>(temp_bytes);
+    need(t);
+    carve_temp(cv);
     return cv.bytes();
   }
 };
-
-// The vertex -> face lists of the first F faces: vfaces[vrange[v].x, vrange[v].y) in face order.
-cudaError_t vertex_faces(Scratch& s, int F, int V, int vbits, cudaStream_t st) {
-  return vertex_faces(F, V, s.faces, vbits, s.ikey_in, s.ikey, s.ival_in, s.vfaces, s.vrange, s.temp, s.temp_bytes, st);
-}
 
 }  // namespace
 }  // namespace dgs
@@ -328,69 +243,33 @@ int dgs_mesh_decimate(const float* vertices, long long num_vertices, const int* 
                       long long target_faces, dgs_alloc_fn alloc, void* alloc_user, float** out_vertices,
                       int** out_faces, long long* out_num_vertices, long long* out_num_faces, int* rounds,
                       void* stream) {
-  DGS_REQUIRE(alloc && out_vertices && out_faces && out_num_vertices && out_num_faces,
-              "mesh decimate: alloc and the four outputs must not be NULL");
-  DGS_REQUIRE(num_vertices >= 0 && num_faces >= 0, "mesh decimate: negative size (%lld vertices, %lld faces)",
-              num_vertices, num_faces);
+  const char* name = "mesh decimate";
+  const MeshOut out{alloc, alloc_user, out_vertices, out_faces, out_num_vertices, out_num_faces};
+  const int rc = check_mesh_args(name, vertices, num_vertices, faces, num_faces,
+                                 num_vertices <= 0x7fffffffLL && 3 * num_faces <= 0x7fffffffLL,
+                                 "at most 2^31 - 1 vertices and half-edges", out);
+  if (rc != DGS_OK) return rc;
   DGS_REQUIRE(target_faces >= 0, "mesh decimate: target_faces must be >= 0 (got %lld)", target_faces);
-  DGS_REQUIRE(num_vertices <= 0x7fffffffLL && 3 * num_faces <= 0x7fffffffLL,
-              "mesh decimate: %lld vertices / %lld faces is too many (at most 2^31 - 1 vertices and half-edges)",
-              num_vertices, num_faces);
-  DGS_REQUIRE((num_vertices == 0 || vertices) && (num_faces == 0 || faces),
-              "mesh decimate: vertices and faces must not be NULL");
-  *out_vertices = nullptr;
-  *out_faces = nullptr;
-  *out_num_vertices = *out_num_faces = 0;
+  out.set(nullptr, nullptr, 0, 0);
   if (rounds) *rounds = 0;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const int V = (int)num_vertices, F = (int)num_faces;
-  int vbits = 1;
-  while (vbits < 31 && (1LL << vbits) < num_vertices) vbits++;
-  const bool decimate = num_faces > target_faces;
+  const int V = (int)num_vertices, F = (int)num_faces, vbits = bits_for(V);
+  if (num_faces <= target_faces) return copy_unchanged(name, vertices, V, faces, F, out, st);
   Scratch s;
-  // the input is returned as it is when it is within the target: only the counters are needed to check it
-  const size_t bytes = decimate ? s.carve(nullptr, V, F, vbits) : sizeof(Counters);
-  void* buf = alloc(bytes, alloc_user);
-  if (!buf) { set_error("mesh decimate: scratch allocation failed (%zu bytes)", bytes); return DGS_ERR_ALLOC; }
-  if (decimate) s.carve(buf, V, F, vbits);
-  else s.ctr = reinterpret_cast<Counters*>(buf);
+  void* buf = out.scratch(name, s.carve(nullptr, V, F));
+  if (!buf) return DGS_ERR_ALLOC;
+  s.carve(buf, V, F);
   const int3* in_faces = reinterpret_cast<const int3*>(faces);
+  DGS_CUDA_OK(cudaMemcpyAsync(s.pos, vertices, 3 * (size_t)V * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  DGS_CUDA_OK(cudaMemcpyAsync(s.faces, in_faces, (size_t)F * sizeof(int3), cudaMemcpyDeviceToDevice, st));
   Counters h;
-  DGS_CUDA_OK(cudaMemsetAsync(s.ctr, 0xff, sizeof(Counters), st));
-  if (F > 0) {
-    validate_kernel<<<ceil_div(F, kThreads), kThreads, 0, st>>>(F, V, in_faces, s.ctr);
-    DGS_POST_LAUNCH();
-  }
-  if (decimate) {
-    DGS_CUDA_OK(cudaMemcpyAsync(s.pos, vertices, 3 * (size_t)V * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    DGS_CUDA_OK(cudaMemcpyAsync(s.faces, in_faces, (size_t)F * sizeof(int3), cudaMemcpyDeviceToDevice, st));
-  }
-  DGS_CUDA_OK(cudaMemcpyAsync(&h, s.ctr, sizeof(h), cudaMemcpyDeviceToHost, st));
-  DGS_CUDA_OK(cudaStreamSynchronize(st));  // indices must be valid before any kernel follows them
-  if (h.bad_face != kNoKey) {
-    const int3* bad = in_faces + h.bad_face;
-    int t[3] = {0, 0, 0};
-    DGS_CUDA_OK(cudaMemcpyAsync(t, bad, sizeof(t), cudaMemcpyDeviceToHost, st));
-    DGS_CUDA_OK(cudaStreamSynchronize(st));
-    set_error("mesh decimate: face %llu = (%d, %d, %d) has an index outside [0, %d) or a repeated index", h.bad_face,
-              t[0], t[1], t[2], V);
-    return DGS_ERR_INVALID_ARGUMENT;
-  }
-  if (!decimate) {
-    float* v = V ? reinterpret_cast<float*>(alloc(3 * (size_t)V * sizeof(float), alloc_user)) : nullptr;
-    int* f = F ? reinterpret_cast<int*>(alloc(3 * (size_t)F * sizeof(int), alloc_user)) : nullptr;
-    if ((V && !v) || (F && !f)) { set_error("mesh decimate: output allocation failed"); return DGS_ERR_ALLOC; }
-    if (V) DGS_CUDA_OK(cudaMemcpyAsync(v, vertices, 3 * (size_t)V * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    if (F) DGS_CUDA_OK(cudaMemcpyAsync(f, faces, 3 * (size_t)F * sizeof(int), cudaMemcpyDeviceToDevice, st));
-    *out_vertices = v;
-    *out_faces = f;
-    *out_num_vertices = V;
-    *out_num_faces = F;
-    return DGS_OK;
+  {
+    const int rc = check_faces(name, vertices, V, in_faces, F, true, nullptr, &s.ctr->chk, h.chk, st);
+    if (rc != DGS_OK) return rc;
   }
 
   // setup: vertex quadrics over the vertex -> face lists (face order), no locks yet
-  DGS_CUDA_OK(vertex_faces(s, F, V, vbits, st));
+  DGS_CUDA_OK(s.vertex_faces(F, V, st));
   vertex_quadric_kernel<<<ceil_div(V, kThreads), kThreads, 0, st>>>(V, s.pos, s.faces, s.vrange, s.vfaces, s.Q);
   DGS_POST_LAUNCH();
   DGS_CUDA_OK(cudaMemsetAsync(s.lock, 0, (size_t)V, st));
@@ -398,11 +277,11 @@ int dgs_mesh_decimate(const float* vertices, long long num_vertices, const int* 
   int live = F, applied_rounds = 0;
   while (live > (long long)target_faces) {
     const int n = 3 * live, gn = ceil_div(n, kThreads), gv = ceil_div(V, kThreads);
-    DGS_CUDA_OK(sort_edges(n, s.faces, vbits, s.hkey_in, s.hkey, s.hval_in, s.hval, s.heads, s.temp, s.temp_bytes, st));
+    DGS_CUDA_OK(s.sort_edges(live, V, st));
     edge_build_kernel<<<gn, kThreads, 0, st>>>(n, s.hkey, s.hval, s.heads, s.faces, vbits, s.edges, s.edge_of, s.lock,
                                                s.ctr);
     DGS_POST_LAUNCH();
-    if (applied_rounds > 0) DGS_CUDA_OK(vertex_faces(s, live, V, vbits, st));  // setup built the first round's
+    if (applied_rounds > 0) DGS_CUDA_OK(s.vertex_faces(live, V, st));  // setup built the first round's
     cost_kernel<<<gn, kThreads, 0, st>>>(s.ctr, s.edges, s.pos, s.Q, s.lock, s.faces, s.vrange, s.vfaces, s.ekey,
                                          s.eplace);
     DGS_POST_LAUNCH();
@@ -430,43 +309,16 @@ int dgs_mesh_decimate(const float* vertices, long long num_vertices, const int* 
     DGS_CUDA_OK(cudaMemsetAsync(s.to, 0xff, (size_t)V * sizeof(int), st));
     apply_kernel<<<gn, kThreads, 0, st>>>(s.ctr, s.edges, s.skey, thr, s.eplace, s.pos, s.Q, s.to);
     DGS_POST_LAUNCH();
-    remap_kernel<<<ceil_div(live, kThreads), kThreads, 0, st>>>(live, s.faces, s.to, s.alive);
+    remap_kernel<<<ceil_div(live, kThreads), kThreads, 0, st>>>(live, s.faces, s.to, s.keep);
     DGS_POST_LAUNCH();
-    DGS_CUDA_OK(cub::DeviceSelect::Flagged(s.temp, s.temp_bytes, s.faces, s.alive, s.faces_alt, &s.ctr->num_faces, live,
-                                           st));
-    std::swap(s.faces, s.faces_alt);
+    DGS_CUDA_OK(s.compact(live, &s.ctr->num_faces, st));
     live -= 2 * take;
     applied_rounds++;
   }
 
   // finish: referenced vertices in index order, faces remapped
-  DGS_CUDA_OK(cudaMemsetAsync(s.used, 0, (size_t)V * sizeof(uint32_t), st));
-  if (live > 0) {
-    used_kernel<<<ceil_div(3 * live, kThreads), kThreads, 0, st>>>(3 * live, s.faces, s.used);
-    DGS_POST_LAUNCH();
-  }
-  DGS_CUDA_OK(cub::DeviceScan::InclusiveSum(s.temp, s.temp_bytes, s.used, s.vscan, V, st));
-  uint32_t nv = 0;
-  DGS_CUDA_OK(cudaMemcpyAsync(&nv, s.vscan + V - 1, sizeof(nv), cudaMemcpyDeviceToHost, st));
-  DGS_CUDA_OK(cudaMemcpyAsync(&h, s.ctr, sizeof(h), cudaMemcpyDeviceToHost, st));
-  DGS_CUDA_OK(cudaStreamSynchronize(st));  // the vertex count sizes the output
-  if (applied_rounds > 0 && h.num_faces != live) {
-    set_error("mesh decimate: internal error, %d live faces where %d were expected", h.num_faces, live);
-    return DGS_ERR_CUDA;
-  }
   if (rounds) *rounds = applied_rounds;
-  if (nv == 0) return DGS_OK;
-  float* v = reinterpret_cast<float*>(alloc((size_t)nv * 3 * sizeof(float), alloc_user));
-  int* f = live ? reinterpret_cast<int*>(alloc((size_t)live * 3 * sizeof(int), alloc_user)) : nullptr;
-  if (!v || (live && !f)) { set_error("mesh decimate: output allocation failed"); return DGS_ERR_ALLOC; }
-  emit_kernel<<<ceil_div(std::max(V, live), kThreads), kThreads, 0, st>>>(V, live, s.pos, s.faces, s.used, s.vscan, v,
-                                                                           reinterpret_cast<int3*>(f));
-  DGS_POST_LAUNCH();
-  *out_vertices = v;
-  *out_faces = f;
-  *out_num_vertices = nv;
-  *out_num_faces = live;
-  return DGS_OK;
+  return emit_mesh(name, s, V, V, live, s.pos, nullptr, applied_rounds > 0 ? &s.ctr->num_faces : nullptr, out, st);
 }
 
 }  // extern "C"

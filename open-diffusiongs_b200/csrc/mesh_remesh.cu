@@ -6,19 +6,14 @@
 // The only atomics are integer ones whose result does not depend on their order (min of keys, counts, flags), so the
 // output is the same bits on every run.
 //
-// Per iteration: the edges (mesh_edges.cuh sort_edges) give the locks; split (one pass, one read-back for the counts;
+// Per iteration: the edges (mesh_common.cuh sort_edges) give the locks; split (one pass, one read-back for the counts;
 // scratch grows here when the mesh outgrows it); collapse rounds (the key / m1 / m2 selection of mesh_decimate.cu
 // through mesh_collapse.cuh, one read-back per round); flip rounds (each vertex keeps the smallest (-gain, edge) key of
 // the candidates that touch it, one read-back per round); one Jacobi pass of tangential smoothing; reprojection onto the
 // input surface through a uniform grid of its triangle boxes (cell -> triangle pairs radix-sorted once per call).
 // Collapse and flip stages stop after kRoundCap rounds each; that is reported in the stats, never an error.
-#include <cub/cub.cuh>
-
-#include <algorithm>
 #include <cmath>
-#include <cstring>
 
-#include "dgs_internal.h"
 #include "mesh_collapse.cuh"
 
 namespace dgs {
@@ -26,12 +21,10 @@ namespace {
 
 constexpr int kRoundCap = 256;        // rounds per collapse / flip stage and iteration
 constexpr int kMaxCells = 1024;       // grid cells per axis (10 bits of the cell key each)
-constexpr unsigned kFull = 0xffffffffu;
 
 struct Counters {
-  unsigned long long bad_face;  // smallest face with an index outside [0, V) or repeated; kNoKey if none
+  FaceCheck chk;
   int num_edges, selected, num_faces;
-  unsigned box[6];              // order-preserving keys of the referenced vertices' box: min x y z, max x y z
 };
 
 // An undirected edge (a < b) of the current faces; h0 < h1 are its first two half-edges (3 f + k runs from corner k
@@ -51,18 +44,6 @@ struct Surface {
   double mn[3], h;
   int n[3];
 };
-
-__host__ __device__ __forceinline__ unsigned fkey(float x) {
-  unsigned u;
-  memcpy(&u, &x, sizeof(u));
-  return (u & 0x80000000u) ? ~u : u | 0x80000000u;
-}
-__host__ __device__ __forceinline__ float fval(unsigned k) {
-  const unsigned u = (k & 0x80000000u) ? k & 0x7fffffffu : ~k;
-  float x;
-  memcpy(&x, &u, sizeof(x));
-  return x;
-}
 
 __device__ __forceinline__ double3 add(double3 u, double3 v) { return make_double3(u.x + v.x, u.y + v.y, u.z + v.z); }
 __device__ __forceinline__ double3 scale(double s, double3 v) { return make_double3(s * v.x, s * v.y, s * v.z); }
@@ -162,37 +143,6 @@ __device__ __forceinline__ bool near_surface(const Surface& S, double3 p, double
 }
 
 // ---------------------------------------------------------------------------------------------------------- setup
-// The smallest bad face, and the box of the vertices the faces reference (warp-reduced key atomics).
-__global__ void validate_kernel(int F, int V, const int3* __restrict__ faces, const float* __restrict__ pos,
-                                Counters* __restrict__ ctr) {
-  const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  unsigned lo[3] = {kFull, kFull, kFull}, hi[3] = {0u, 0u, 0u};
-  if (f < F) {
-    const int3 t = faces[f];
-    const bool ok = t.x >= 0 && t.x < V && t.y >= 0 && t.y < V && t.z >= 0 && t.z < V && t.x != t.y &&
-                    t.y != t.z && t.x != t.z;
-    if (!ok) atomicMin(&ctr->bad_face, (unsigned long long)f);
-    else
-      for (int j = 0; j < 3; j++) {
-        const int v = corner(t, j);
-        for (int k = 0; k < 3; k++) {
-          const unsigned q = fkey(pos[3 * v + k]);
-          lo[k] = min(lo[k], q);
-          hi[k] = max(hi[k], q);
-        }
-      }
-  }
-  for (int k = 0; k < 3; k++) {
-    lo[k] = __reduce_min_sync(kFull, lo[k]);
-    hi[k] = __reduce_max_sync(kFull, hi[k]);
-  }
-  if ((threadIdx.x & 31) == 0)
-    for (int k = 0; k < 3; k++) {
-      atomicMin(&ctr->box[k], lo[k]);
-      atomicMax(&ctr->box[3 + k], hi[k]);
-    }
-}
-
 __device__ __forceinline__ void cell_range(const Surface& S, const float* __restrict__ pos, int3 f, int* lo, int* hi) {
   for (int k = 0; k < 3; k++) {
     const double x0 = pos[3 * f.x + k], x1 = pos[3 * f.y + k], x2 = pos[3 * f.z + k];
@@ -391,17 +341,6 @@ __global__ void collapse_apply_kernel(Counters* __restrict__ ctr, const REdge* _
   atomicAdd(&ctr->selected, 1);
 }
 
-__global__ void remap_kernel(int F, int3* __restrict__ faces, const int* __restrict__ to, uint8_t* __restrict__ alive) {
-  const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  if (f >= F) return;
-  int3 t = faces[f];
-  if (to[t.x] >= 0) t.x = to[t.x];
-  if (to[t.y] >= 0) t.y = to[t.y];
-  if (to[t.z] >= 0) t.z = to[t.z];
-  faces[f] = t;
-  alive[f] = t.x != t.y && t.y != t.z && t.x != t.z;
-}
-
 // ---------------------------------------------------------------------------------------------------------- flip
 __global__ void valence_kernel(const Counters* __restrict__ ctr, const REdge* __restrict__ edges, int* __restrict__ val,
                                uint8_t* __restrict__ bnd) {
@@ -512,44 +451,18 @@ __global__ void reproject_kernel(int V, float* __restrict__ pos, const uint2* __
   store(pos, v, closest(S, load(pos, v), &d2));
 }
 
-// ---------------------------------------------------------------------------------------------------------- finish
-__global__ void used_kernel(int n, const int3* __restrict__ faces, uint32_t* __restrict__ used) {
-  const int h = blockIdx.x * blockDim.x + threadIdx.x;
-  if (h < n) used[corner(faces[h / 3], h % 3)] = 1;
-}
-__global__ void emit_kernel(int V, int F, const float* __restrict__ pos, const int3* __restrict__ faces,
-                            const uint32_t* __restrict__ used, const uint32_t* __restrict__ vscan,
-                            float* __restrict__ out_v, int3* __restrict__ out_f) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < V && used[i]) {
-    const uint32_t o = vscan[i] - 1;
-    out_v[3 * o] = pos[3 * i];
-    out_v[3 * o + 1] = pos[3 * i + 1];
-    out_v[3 * o + 2] = pos[3 * i + 2];
-  }
-  if (i < F) {
-    const int3 t = faces[i];
-    out_f[i] = make_int3((int)vscan[t.x] - 1, (int)vscan[t.y] - 1, (int)vscan[t.z] - 1);
-  }
-}
-
 // The mesh being remeshed and the per-round scratch, sized for Vc vertices and Fc faces (n = 3 Fc half-edges, at
 // most n edges).  A split that outgrows it gets a new one; the mesh is copied over.
-struct Scratch {
+struct Scratch : MeshScratch {
   int Vc = 0, Fc = 0;
   Counters* ctr;
   float *pos, *pos_alt;
-  uint8_t *lock, *bnd, *alive;
+  uint8_t *lock, *bnd;
   int *to, *val;
-  unsigned long long *m1, *m2, *hkey_in, *hkey, *ekey;
-  uint32_t *used, *vscan, *xcnt, *xscan, *hval_in, *hval, *heads, *edge_of, *ikey_in, *ikey, *ival_in, *vfaces,
-      *eflag, *erank;
-  uint2* vrange;
-  int3 *faces, *faces_alt;
+  unsigned long long *m1, *m2, *ekey;
+  uint32_t *xcnt, *xscan, *eflag, *erank;
   REdge* edges;
   float3* eplace;
-  void* temp;
-  size_t temp_bytes;
 
   size_t carve(void* base, int V, int F) {
     Vc = std::max(V, 1);
@@ -557,6 +470,7 @@ struct Scratch {
     const int n = 3 * Fc;
     Carver cv(base);
     ctr = cv.take<Counters>(1);
+    carve_mesh(cv, Vc, Fc, Vc);
     pos = cv.take<float>(3 * (size_t)Vc);
     pos_alt = cv.take<float>(3 * (size_t)Vc);
     lock = cv.take<uint8_t>(Vc);
@@ -565,91 +479,37 @@ struct Scratch {
     val = cv.take<int>(Vc);
     m1 = cv.take<unsigned long long>(Vc);
     m2 = cv.take<unsigned long long>(Vc);
-    used = cv.take<uint32_t>(Vc);
-    vscan = cv.take<uint32_t>(Vc);
-    vrange = cv.take<uint2>(Vc);
-    faces = cv.take<int3>(Fc);
-    faces_alt = cv.take<int3>(Fc);
-    alive = cv.take<uint8_t>(Fc);
+    ekey = cv.take<unsigned long long>(n);
     xcnt = cv.take<uint32_t>(Fc);
     xscan = cv.take<uint32_t>(Fc);
-    hkey_in = cv.take<unsigned long long>(n);
-    hkey = cv.take<unsigned long long>(n);
-    ekey = cv.take<unsigned long long>(n);
-    hval_in = cv.take<uint32_t>(n);
-    hval = cv.take<uint32_t>(n);
-    heads = cv.take<uint32_t>(n);
-    edge_of = cv.take<uint32_t>(n);
-    ikey_in = cv.take<uint32_t>(n);
-    ikey = cv.take<uint32_t>(n);
-    ival_in = cv.take<uint32_t>(n);
-    vfaces = cv.take<uint32_t>(n);
     eflag = cv.take<uint32_t>(n);
     erank = cv.take<uint32_t>(n);
     edges = cv.take<REdge>(n);
     eplace = cv.take<float3>(n);
     size_t t = 0;
-    temp_bytes = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, t, hkey_in, hkey, hval_in, hval, n, 0, 64);
-    temp_bytes = std::max(temp_bytes, t);
-    cub::DeviceRadixSort::SortPairs(nullptr, t, ikey_in, ikey, ival_in, vfaces, n, 0, 32);
-    temp_bytes = std::max(temp_bytes, t);
-    cub::DeviceScan::InclusiveSum(nullptr, t, heads, heads, std::max(n, Vc));
-    temp_bytes = std::max(temp_bytes, t);
-    cub::DeviceScan::InclusiveSum(nullptr, t, hkey_in, hkey, Fc);
-    temp_bytes = std::max(temp_bytes, t);
-    cub::DeviceSelect::Flagged(nullptr, t, faces, alive, faces_alt, static_cast<int*>(nullptr), Fc);
-    temp_bytes = std::max(temp_bytes, t);
-    temp = cv.take<char>(temp_bytes);
+    cub::DeviceScan::InclusiveSum(nullptr, t, hkey_in, hkey, Fc);  // build_surface's scan of the grid counts
+    need(t);
+    carve_temp(cv);
     return cv.bytes();
   }
 };
 
-int bits_for(int V) {
-  int b = 1;
-  while (b < 31 && (1LL << b) < V) b++;
-  return b;
-}
-
 // Edges of the first F faces (and, with lock, the iteration's locks); then the vertex -> face lists when vf is set.
 cudaError_t edge_pass(Scratch& s, int F, int V, double cos_t, uint8_t* lock, bool vf, cudaStream_t st) {
-  const int n = 3 * F, vbits = bits_for(V);
-  cudaError_t e = sort_edges(n, s.faces, vbits, s.hkey_in, s.hkey, s.hval_in, s.hval, s.heads, s.temp, s.temp_bytes, st);
+  const int n = 3 * F;
+  cudaError_t e = s.sort_edges(F, V, st);
   if (e != cudaSuccess) return e;
-  edge_kernel<<<ceil_div(n, kThreads), kThreads, 0, st>>>(n, s.hkey, s.hval, s.heads, s.faces, s.pos, vbits, cos_t,
-                                                           s.edges, s.edge_of, lock, s.ctr);
+  edge_kernel<<<ceil_div(n, kThreads), kThreads, 0, st>>>(n, s.hkey, s.hval, s.heads, s.faces, s.pos, bits_for(V),
+                                                           cos_t, s.edges, s.edge_of, lock, s.ctr);
   g_kernel_launches++;
   if ((e = cudaGetLastError()) != cudaSuccess || !vf) return e;
-  return vertex_faces(F, V, s.faces, vbits, s.ikey_in, s.ikey, s.ival_in, s.vfaces, s.vrange, s.temp, s.temp_bytes, st);
-}
-
-
-// Checks every face (indices in [0, V), none repeated) on the device and reads back the counters: the smallest bad
-// face and the box of the referenced vertices.  A bad face is DGS_ERR_INVALID_ARGUMENT naming it.
-int check_faces(const char* name, const float* vertices, int V, const int3* faces, int F, Counters* ctr, Counters& h,
-                cudaStream_t st) {
-  DGS_CUDA_OK(cudaMemsetAsync(ctr, 0, sizeof(Counters), st));
-  DGS_CUDA_OK(cudaMemsetAsync(&ctr->bad_face, 0xff, sizeof(unsigned long long), st));
-  DGS_CUDA_OK(cudaMemsetAsync(ctr->box, 0xff, 3 * sizeof(unsigned), st));
-  if (F > 0) {
-    validate_kernel<<<ceil_div(F, kThreads), kThreads, 0, st>>>(F, V, faces, vertices, ctr);
-    DGS_POST_LAUNCH();
-  }
-  DGS_CUDA_OK(cudaMemcpyAsync(&h, ctr, sizeof(h), cudaMemcpyDeviceToHost, st));
-  DGS_CUDA_OK(cudaStreamSynchronize(st));  // indices must be valid before any kernel follows them
-  if (h.bad_face == kNoKey) return DGS_OK;
-  int t[3] = {0, 0, 0};
-  DGS_CUDA_OK(cudaMemcpyAsync(t, faces + h.bad_face, sizeof(t), cudaMemcpyDeviceToHost, st));
-  DGS_CUDA_OK(cudaStreamSynchronize(st));
-  set_error("%s: face %llu = (%d, %d, %d) has an index outside [0, %d) or a repeated index", name, h.bad_face, t[0],
-            t[1], t[2], V);
-  return DGS_ERR_INVALID_ARGUMENT;
+  return s.vertex_faces(F, V, st);
 }
 
 // The grid of the surface (F > 0 checked faces, box in h): about sqrt(F) / 2 cells along the longest axis, so a
 // marching-cubes triangle touches a few cells.  cnt and scan are scratch of F entries, temp holds an InclusiveSum of F
 // of them; the (cell, triangle) pairs get an allocation of their own.
-int build_surface(const char* name, const float* vertices, const int3* faces, int F, const Counters& h,
+int build_surface(const char* name, const float* vertices, const int3* faces, int F, const FaceCheck& h,
                   unsigned long long* cnt, unsigned long long* scan, void* temp, size_t temp_bytes, dgs_alloc_fn alloc,
                   void* alloc_user, cudaStream_t st, Surface& S) {
   double ext[3], ext_max = 0.0;
@@ -725,55 +585,34 @@ int dgs_mesh_remesh(const float* vertices, long long num_vertices, const int* fa
                     double target_len, int iterations, double feature_deg, double max_surf_dist, dgs_alloc_fn alloc,
                     void* alloc_user, float** out_vertices, int** out_faces, long long* out_num_vertices,
                     long long* out_num_faces, long long* stats, void* stream) {
-  DGS_REQUIRE(alloc && out_vertices && out_faces && out_num_vertices && out_num_faces,
-              "mesh remesh: alloc and the four outputs must not be NULL");
-  DGS_REQUIRE(num_vertices >= 0 && num_faces >= 0, "mesh remesh: negative size (%lld vertices, %lld faces)",
-              num_vertices, num_faces);
-  DGS_REQUIRE(num_vertices <= 0x7fffffffLL && 3 * num_faces <= 0x7fffffffLL,
-              "mesh remesh: %lld vertices / %lld faces is too many (at most 2^31 - 1 vertices and half-edges)",
-              num_vertices, num_faces);
-  DGS_REQUIRE((num_vertices == 0 || vertices) && (num_faces == 0 || faces),
-              "mesh remesh: vertices and faces must not be NULL");
+  const char* name = "mesh remesh";
+  const MeshOut out{alloc, alloc_user, out_vertices, out_faces, out_num_vertices, out_num_faces};
+  const int rc = check_mesh_args(name, vertices, num_vertices, faces, num_faces,
+                                 num_vertices <= 0x7fffffffLL && 3 * num_faces <= 0x7fffffffLL,
+                                 "at most 2^31 - 1 vertices and half-edges", out);
+  if (rc != DGS_OK) return rc;
   DGS_REQUIRE(std::isfinite(target_len) && target_len > 0, "mesh remesh: target_len must be finite and > 0 (got %g)",
               target_len);
   DGS_REQUIRE(iterations >= 0, "mesh remesh: iterations must be >= 0 (got %d)", iterations);
   DGS_REQUIRE(std::isfinite(feature_deg) && std::isfinite(max_surf_dist),
               "mesh remesh: feature_deg and max_surf_dist must be finite");
-  *out_vertices = nullptr;
-  *out_faces = nullptr;
-  *out_num_vertices = *out_num_faces = 0;
+  out.set(nullptr, nullptr, 0, 0);
   if (stats)
     for (long long k = 0; k < 4LL * iterations; k++) stats[k] = 0;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   int V = (int)num_vertices, F = (int)num_faces;
   const int T = kThreads;
+  if (iterations == 0) return copy_unchanged(name, vertices, V, faces, F, out, st);  // the input, bit for bit
   const int3* in_faces = reinterpret_cast<const int3*>(faces);
-  Counters h;
-  if (iterations == 0) {  // the input, bit for bit: only the counters are needed to check it
-    Counters* ctr = reinterpret_cast<Counters*>(alloc(sizeof(Counters), alloc_user));
-    if (!ctr) { set_error("mesh remesh: scratch allocation failed"); return DGS_ERR_ALLOC; }
-    const int rc = check_faces("mesh remesh", vertices, V, in_faces, F, ctr, h, st);
-    if (rc != DGS_OK) return rc;
-    float* v = V ? reinterpret_cast<float*>(alloc(3 * (size_t)V * sizeof(float), alloc_user)) : nullptr;
-    int* f = F ? reinterpret_cast<int*>(alloc(3 * (size_t)F * sizeof(int), alloc_user)) : nullptr;
-    if ((V && !v) || (F && !f)) { set_error("mesh remesh: output allocation failed"); return DGS_ERR_ALLOC; }
-    if (V) DGS_CUDA_OK(cudaMemcpyAsync(v, vertices, 3 * (size_t)V * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    if (F) DGS_CUDA_OK(cudaMemcpyAsync(f, faces, 3 * (size_t)F * sizeof(int), cudaMemcpyDeviceToDevice, st));
-    *out_vertices = v;
-    *out_faces = f;
-    *out_num_vertices = V;
-    *out_num_faces = F;
-    return DGS_OK;
-  }
   Scratch s;
   {
-    const size_t bytes = s.carve(nullptr, V, F);
-    void* buf = alloc(bytes, alloc_user);
-    if (!buf) { set_error("mesh remesh: scratch allocation failed (%zu bytes)", bytes); return DGS_ERR_ALLOC; }
+    void* buf = out.scratch(name, s.carve(nullptr, V, F));
+    if (!buf) return DGS_ERR_ALLOC;
     s.carve(buf, V, F);
   }
+  Counters h;
   {
-    const int rc = check_faces("mesh remesh", vertices, V, in_faces, F, s.ctr, h, st);
+    const int rc = check_faces(name, vertices, V, in_faces, F, true, nullptr, &s.ctr->chk, h.chk, st);
     if (rc != DGS_OK) return rc;
   }
   if (F == 0) return DGS_OK;  // nothing is referenced: the result is empty
@@ -783,14 +622,14 @@ int dgs_mesh_remesh(const float* vertices, long long num_vertices, const int* fa
   if (max_surf_dist < 0) {
     double d2 = 0.0;
     for (int k = 0; k < 3; k++) {
-      const double e = (double)fval(h.box[3 + k]) - (double)fval(h.box[k]);
+      const double e = (double)fval(h.chk.box[3 + k]) - (double)fval(h.chk.box[k]);
       d2 += e * e;
     }
     max_surf_dist = std::sqrt(d2) / 100.0;
   }
   Surface S;
   {
-    const int rc = build_surface("mesh remesh", vertices, in_faces, F, h, s.hkey_in, s.hkey, s.temp, s.temp_bytes, alloc,
+    const int rc = build_surface(name, vertices, in_faces, F, h.chk, s.hkey_in, s.hkey, s.temp, s.temp_bytes, alloc,
                                  alloc_user, st, S);
     if (rc != DGS_OK) return rc;
   }
@@ -823,9 +662,8 @@ int dgs_mesh_remesh(const float* vertices, long long num_vertices, const int* fa
       if (V2 > s.Vc || F2 > s.Fc) {
         const int vc = (int)std::min(V2 + V2 / 2, 0x7fffffffLL), fc = (int)std::min(F2 + F2 / 2, 0x7fffffffLL / 3);
         Scratch g;
-        const size_t bytes = g.carve(nullptr, vc, fc);
-        void* buf = alloc(bytes, alloc_user);
-        if (!buf) { set_error("mesh remesh: scratch allocation failed (%zu bytes)", bytes); return DGS_ERR_ALLOC; }
+        void* buf = out.scratch(name, g.carve(nullptr, vc, fc));
+        if (!buf) return DGS_ERR_ALLOC;
         g.carve(buf, vc, fc);
         DGS_CUDA_OK(cudaMemcpyAsync(g.pos, s.pos, 3 * (size_t)V * sizeof(float), cudaMemcpyDeviceToDevice, st));
         DGS_CUDA_OK(cudaMemcpyAsync(g.lock, s.lock, (size_t)V, cudaMemcpyDeviceToDevice, st));
@@ -865,11 +703,9 @@ int dgs_mesh_remesh(const float* vertices, long long num_vertices, const int* fa
         return DGS_ERR_CUDA;
       }
       if (h.selected == 0) break;
-      remap_kernel<<<ceil_div(F, T), T, 0, st>>>(F, s.faces, s.to, s.alive);
+      remap_kernel<<<ceil_div(F, T), T, 0, st>>>(F, s.faces, s.to, s.keep);
       DGS_POST_LAUNCH();
-      DGS_CUDA_OK(cub::DeviceSelect::Flagged(s.temp, s.temp_bytes, s.faces, s.alive, s.faces_alt, &s.ctr->num_faces, F,
-                                             st));
-      std::swap(s.faces, s.faces_alt);
+      DGS_CUDA_OK(s.compact(F, &s.ctr->num_faces, st));
       F -= 2 * h.selected;  // the link condition leaves exactly the two faces of each collapsed edge degenerate
       collapsed = true;
       if (row) row[1]++;
@@ -904,8 +740,7 @@ int dgs_mesh_remesh(const float* vertices, long long num_vertices, const int* fa
     if (F == 0) break;
     // tangential smoothing, then reprojection of the referenced vertices onto S
     const int gv = ceil_div(V, T);
-    DGS_CUDA_OK(vertex_faces(F, V, s.faces, bits_for(V), s.ikey_in, s.ikey, s.ival_in, s.vfaces, s.vrange, s.temp,
-                             s.temp_bytes, st));
+    DGS_CUDA_OK(s.vertex_faces(F, V, st));
     smooth_kernel<<<gv, T, 0, st>>>(V, s.pos, s.faces, s.vrange, s.vfaces, s.lock, s.pos_alt);
     DGS_POST_LAUNCH();
     std::swap(s.pos, s.pos_alt);
@@ -914,27 +749,7 @@ int dgs_mesh_remesh(const float* vertices, long long num_vertices, const int* fa
   }
 
   // finish: referenced vertices in index order, faces remapped
-  DGS_CUDA_OK(cudaMemsetAsync(s.used, 0, (size_t)V * sizeof(uint32_t), st));
-  if (F > 0) {
-    used_kernel<<<ceil_div(3 * F, T), T, 0, st>>>(3 * F, s.faces, s.used);
-    DGS_POST_LAUNCH();
-  }
-  DGS_CUDA_OK(cub::DeviceScan::InclusiveSum(s.temp, s.temp_bytes, s.used, s.vscan, V, st));
-  uint32_t nv = 0;
-  DGS_CUDA_OK(cudaMemcpyAsync(&nv, s.vscan + V - 1, sizeof(nv), cudaMemcpyDeviceToHost, st));
-  DGS_CUDA_OK(cudaStreamSynchronize(st));  // the vertex count sizes the output
-  if (F == 0 || nv == 0) return DGS_OK;
-  float* v = reinterpret_cast<float*>(alloc((size_t)nv * 3 * sizeof(float), alloc_user));
-  int* f = reinterpret_cast<int*>(alloc((size_t)F * 3 * sizeof(int), alloc_user));
-  if (!v || !f) { set_error("mesh remesh: output allocation failed"); return DGS_ERR_ALLOC; }
-  emit_kernel<<<ceil_div(std::max(V, F), T), T, 0, st>>>(V, F, s.pos, s.faces, s.used, s.vscan, v,
-                                                         reinterpret_cast<int3*>(f));
-  DGS_POST_LAUNCH();
-  *out_vertices = v;
-  *out_faces = f;
-  *out_num_vertices = nv;
-  *out_num_faces = F;
-  return DGS_OK;
+  return emit_mesh(name, s, V, V, F, s.pos, nullptr, nullptr, out, st);
 }
 
 int dgs_mesh_closest_points(const float* vertices, long long num_vertices, const int* faces, long long num_faces,
@@ -956,19 +771,19 @@ int dgs_mesh_closest_points(const float* vertices, long long num_vertices, const
   cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, static_cast<unsigned long long*>(nullptr),
                                 static_cast<unsigned long long*>(nullptr), F);
   Carver probe(nullptr);
-  probe.take<Counters>(1);
+  probe.take<FaceCheck>(1);
   probe.take<unsigned long long>(F);
   probe.take<unsigned long long>(F);
   probe.take<char>(scan_bytes);
   void* buf = alloc(probe.bytes(), alloc_user);
   if (!buf) { set_error("mesh closest points: scratch allocation failed (%zu bytes)", probe.bytes()); return DGS_ERR_ALLOC; }
   Carver cv(buf);
-  Counters* ctr = cv.take<Counters>(1);
+  FaceCheck* chk = cv.take<FaceCheck>(1);
   unsigned long long* cnt = cv.take<unsigned long long>(F);
   unsigned long long* scan = cv.take<unsigned long long>(F);
   void* temp = cv.take<char>(scan_bytes);
-  Counters h;
-  int rc = check_faces("mesh closest points", vertices, V, in_faces, F, ctr, h, st);
+  FaceCheck h;
+  int rc = check_faces("mesh closest points", vertices, V, in_faces, F, true, nullptr, chk, h, st);
   if (rc != DGS_OK) return rc;
   Surface S;
   rc = build_surface("mesh closest points", vertices, in_faces, F, h, cnt, scan, temp, scan_bytes, alloc, alloc_user, st,

@@ -134,6 +134,32 @@ def _mesh_out(is_numpy, dev, alloc, V, F):
     return ov, of
 
 
+def _run_mesh(name, is_numpy, vertices, faces, args, stats=()):
+    """Runs dgs_mesh_<name>(vertices, V, faces, F, *args, alloc, NULL, the four outputs, *stats, stream) on a checked
+    mesh argument pair -> (vertices, faces) as `_mesh_out`"""
+    dev, v, f = _mesh_in(name, is_numpy, vertices, faces)
+    alloc = Alloc(dev, _SCRATCH, (str(dev), name), cached=1)  # only the first scratch: remesh's later requests differ
+    vp, fp = C.c_void_p(), C.c_void_p()
+    nv, nf = C.c_longlong(0), C.c_longlong(0)
+    with torch.cuda.device(dev):
+        check(getattr(_lib.lib(), f"dgs_mesh_{name}")(v.data_ptr(), len(v), f.data_ptr(), len(f), *args, alloc.cb, None,
+                                                       C.byref(vp), C.byref(fp), C.byref(nv), C.byref(nf), *stats,
+                                                       stream(dev)))
+    return _mesh_out(is_numpy, dev, alloc, nv.value, nf.value)
+
+
+def _chain(vertices, faces, clean_first, remesh_len, decimate_target):
+    """`clean` with its defaults when clean_first, `remesh` to edges of remesh_len when it is given, then `decimate` to
+    decimate_target faces when it is given and more are left"""
+    if clean_first:
+        vertices, faces = clean(vertices, faces)
+    if remesh_len is not None:
+        vertices, faces = remesh(vertices, faces, remesh_len)
+    if decimate_target is not None and len(faces) > decimate_target:
+        vertices, faces = decimate(vertices, faces, decimate_target)
+    return vertices, faces
+
+
 def decimate(vertices, faces, target_faces):
     """Quadric edge-collapse decimation to at most `target_faces` faces (dgs_mesh_decimate; the reference's
     decimate_mesh with optimalplacement=True, boundary loops kept) -> (vertices, faces).  The signature of
@@ -146,15 +172,7 @@ def decimate(vertices, faces, target_faces):
     target = float(target_faces)
     if not np.isfinite(target) or target < 0:
         raise ValueError(f"decimate: target_faces must be a finite number >= 0 (got {target_faces!r})")
-    dev, v, f = _mesh_in("decimate", is_numpy, vertices, faces)
-    alloc = Alloc(dev, _SCRATCH, (str(dev), "decimate"), cached=1)
-    vp, fp = C.c_void_p(), C.c_void_p()
-    nv, nf, rounds = C.c_longlong(0), C.c_longlong(0), C.c_int(0)
-    with torch.cuda.device(dev):
-        check(_lib.lib().dgs_mesh_decimate(v.data_ptr(), len(v), f.data_ptr(), len(f), int(target), alloc.cb, None,
-                                           C.byref(vp), C.byref(fp), C.byref(nv), C.byref(nf), C.byref(rounds),
-                                           stream(dev)))
-    return _mesh_out(is_numpy, dev, alloc, nv.value, nf.value)
+    return _run_mesh("decimate", is_numpy, vertices, faces, (int(target),), (C.byref(C.c_int(0)),))
 
 
 def clean(vertices, faces, v_pct=1, min_f=64, min_d=20, repair=True, stats=None):
@@ -169,29 +187,20 @@ def clean(vertices, faces, v_pct=1, min_f=64, min_d=20, repair=True, stats=None)
     v_pct, min_d = float(v_pct), float(min_d)
     if not (np.isfinite(v_pct) and np.isfinite(min_d)):
         raise ValueError(f"clean: v_pct and min_d must be finite (got {v_pct!r}, {min_d!r})")
-    dev, v, f = _mesh_in("clean", is_numpy, vertices, faces)
-    alloc = Alloc(dev, _SCRATCH, (str(dev), "clean"), cached=1)
-    vp, fp = C.c_void_p(), C.c_void_p()
-    nv, nf, rounds = C.c_longlong(0), C.c_longlong(0), C.c_int(0)
-    counts = (C.c_longlong * 9)()
-    with torch.cuda.device(dev):
-        check(_lib.lib().dgs_mesh_clean(v.data_ptr(), len(v), f.data_ptr(), len(f), v_pct, int(min_f), min_d,
-                                        int(bool(repair)), alloc.cb, None, C.byref(vp), C.byref(fp), C.byref(nv),
-                                        C.byref(nf), C.byref(rounds), counts, stream(dev)))
+    rounds, counts = C.c_int(0), (C.c_longlong * 9)()
+    out = _run_mesh("clean", is_numpy, vertices, faces, (v_pct, int(min_f), min_d, int(bool(repair))),
+                    (C.byref(rounds), counts))
     if stats is not None:
         stats["merge_rounds"] = rounds.value
         stats["stage_faces"] = list(counts)
-    return _mesh_out(is_numpy, dev, alloc, nv.value, nf.value)
+    return out
 
 
 def clean_then_decimate(vertices, faces, decimate_target):
     """The reference's extract_mesh post-processing without its remeshing (gs_core.py:862-863): `clean` with its
     defaults, then `decimate` to decimate_target faces when more are left.  The signature of extract_mesh's
     `postprocess`: `extract_mesh(postprocess=clean_then_decimate)`."""
-    v, f = clean(vertices, faces)
-    if len(f) > decimate_target:
-        v, f = decimate(v, f, decimate_target)
-    return v, f
+    return _chain(vertices, faces, True, None, decimate_target)
 
 
 def remesh(vertices, faces, target_len=0.015, iterations=3, feature_deg=30, max_surf_dist=None, stats=None):
@@ -213,18 +222,12 @@ def remesh(vertices, faces, target_len=0.015, iterations=3, feature_deg=30, max_
     if not (np.isfinite(deg) and np.isfinite(msd)) or (max_surf_dist is not None and msd < 0):
         raise ValueError(f"remesh: feature_deg and max_surf_dist must be finite, max_surf_dist >= 0 (got "
                          f"{feature_deg!r}, {max_surf_dist!r})")
-    dev, v, f = _mesh_in("remesh", is_numpy, vertices, faces)
-    alloc = Alloc(dev, _SCRATCH, (str(dev), "remesh"), cached=1)  # only the first scratch: later requests differ
-    vp, fp = C.c_void_p(), C.c_void_p()
-    nv, nf = C.c_longlong(0), C.c_longlong(0)
     it = int(iterations)
     st = (C.c_longlong * max(4 * it, 1))()
-    with torch.cuda.device(dev):
-        check(_lib.lib().dgs_mesh_remesh(v.data_ptr(), len(v), f.data_ptr(), len(f), L, it, deg, msd, alloc.cb, None,
-                                         C.byref(vp), C.byref(fp), C.byref(nv), C.byref(nf), st, stream(dev)))
+    out = _run_mesh("remesh", is_numpy, vertices, faces, (L, it, deg, msd), (st,))
     if stats is not None:
         stats["iterations"] = [list(st[4 * i:4 * i + 4]) for i in range(it)]
-    return _mesh_out(is_numpy, dev, alloc, nv.value, nf.value)
+    return out
 
 
 def closest_points(vertices, faces, queries):
@@ -260,11 +263,7 @@ def clean_remesh_then_decimate(vertices, faces, decimate_target):
     """The reference's whole extract_mesh post-processing (gs_core.py:862-863): `clean` with its defaults, `remesh` to
     edges of 0.015 in 3 iterations, then `decimate` to decimate_target faces when more are left.  The signature of
     extract_mesh's `postprocess`: `extract_mesh(postprocess=clean_remesh_then_decimate)`."""
-    v, f = clean(vertices, faces)
-    v, f = remesh(v, f, 0.015, 3)
-    if len(f) > decimate_target:
-        v, f = decimate(v, f, decimate_target)
-    return v, f
+    return _chain(vertices, faces, True, 0.015, decimate_target)
 
 
 class Mesh:
@@ -329,14 +328,8 @@ def parser():
 def _postprocess(args):
     """-> extract_mesh keyword arguments for the --clean / --remesh / --decimate-target flags"""
     if args.remesh is not None:
-        def chain(v, f, target):
-            if args.clean:
-                v, f = clean(v, f)
-            v, f = remesh(v, f, args.remesh)
-            if target is not None and len(f) > target:
-                v, f = decimate(v, f, target)
-            return v, f
-        return dict(postprocess=chain, decimate_target=args.decimate_target)
+        return dict(postprocess=lambda v, f, target: _chain(v, f, args.clean, args.remesh, target),
+                    decimate_target=args.decimate_target)
     if args.clean and args.decimate_target is not None:
         return dict(postprocess=clean_then_decimate, decimate_target=args.decimate_target)
     if args.clean:

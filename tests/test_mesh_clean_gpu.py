@@ -7,6 +7,7 @@ import pytest
 import torch
 
 from mesh_clean_cases import cases
+from mesh_shapes import cuda_grid, directed, mc, shell_model
 from oracle import mesh_clean as oc
 
 pytestmark = pytest.mark.gpu
@@ -35,17 +36,6 @@ def test_hand_cases_equal_oracle(case):
     assert np.array_equal(ov, ev.reshape(-1, 3)) and np.array_equal(of, ef.reshape(-1, 3)) and st["stage_faces"] == counts
 
 
-def _mc(field):
-    from dgs_b200 import mesh
-    v, f = mesh.marching_cubes(field.contiguous(), 0.0)
-    return v.cpu().numpy(), f.cpu().numpy().astype(np.int64)
-
-
-def _grid(n):
-    x = torch.arange(n, device="cuda", dtype=torch.float32) - (n - 1) / 2
-    return torch.meshgrid(x, x, x, indexing="ij")
-
-
 def _blobs(X, Y, Z, centres, r):
     return torch.stack([r - torch.sqrt((X - a) ** 2 + (Y - b) ** 2 + (Z - c) ** 2) for a, b, c in centres]).amax(0)
 
@@ -55,38 +45,17 @@ def _blobs(X, Y, Z, centres, r):
                          ids=["defaults", "v_pct0.3", "v_pct2", "no_repair"])
 def test_surfaces_with_blobs_equal_oracle(shape, kw):
     n = 96
-    X, Y, Z = _grid(n)
+    X, Y, Z = cuda_grid(n)
     if shape == "sphere":
         body = 30 - torch.sqrt(X * X + Y * Y + Z * Z)
     else:
         body = 9 - torch.sqrt((torch.sqrt(X * X + Y * Y) - 26) ** 2 + Z * Z)
     blobs = _blobs(X, Y, Z, [(40, 40, 40), (-40, 38, -36), (36, -40, 30)], 2.5)
-    v, f = _mc(torch.maximum(body, blobs))
+    v, f = mc(torch.maximum(body, blobs))
     ov, of, st = _same_as_oracle(v, f, **kw)
     print(f"{shape} {kw}: {len(v)} -> {len(ov)} vertices, stage faces {st['stage_faces']}, "
           f"{st['merge_rounds']} merge rounds")
     assert st["stage_faces"][5] < st["stage_faces"][3]  # the blobs go
-
-
-def _model(P, seed, floaters=True):
-    from dgs_b200 import synth
-    from dgs_b200.renderer import GaussianModel
-    g = synth.make_shell_gaussians(P, seed, "fine")
-    if floaters:
-        rng = np.random.default_rng(seed)
-        k = 400
-        for c in [(0.8, 0.7, 0.0), (-0.7, -0.75, 0.6), (0.1, -0.8, -0.7)]:
-            extra = {key: g[key][:k].copy() for key in g}
-            extra["xyz"] = (np.asarray(c) + rng.normal(0, 0.01, (k, 3))).astype(np.float32)
-            g = {key: np.concatenate([g[key], extra[key]]) for key in g}
-    m = GaussianModel(0)
-    m._xyz, m._scaling, m._rotation, m._opacity = (torch.tensor(g[k], device="cuda") for k in
-                                                   ("xyz", "scaling", "rotation", "opacity"))
-    return m
-
-
-def _directed(f):
-    return np.concatenate([f[:, [0, 1]], f[:, [1, 2]], f[:, [2, 0]]])
 
 
 def _check_clean(v, f, min_f=64, min_d=20):
@@ -95,7 +64,7 @@ def _check_clean(v, f, min_f=64, min_d=20):
     assert (f[:, 0] != f[:, 1]).all() and (f[:, 1] != f[:, 2]).all() and (f[:, 0] != f[:, 2]).all()
     assert len(np.unique(np.sort(f, axis=1), axis=0)) == len(f), "a duplicate face"
     assert (oc.doubled_area(v, f) > 0).all(), "a null face"
-    e = np.sort(_directed(f), axis=1)
+    e = np.sort(directed(f), axis=1)
     _, cnt = np.unique(e, axis=0, return_counts=True)
     assert cnt.max() <= 2, "an edge of more than 2 faces"
     # one fan per vertex: corners of a vertex joined through its edges form a single component
@@ -136,7 +105,7 @@ def _check_clean(v, f, min_f=64, min_d=20):
 def test_obj256_pipeline_equals_oracle():
     import time
     from dgs_b200 import mesh
-    m = _model(262146, 11)
+    m = shell_model(262146, 11)
     raw = m.extract_mesh()
     v, f = raw.vertices, raw.faces
     ov, of, st = _native(v, f)
@@ -162,7 +131,7 @@ def test_obj256_pipeline_equals_oracle():
 
 def test_clean_then_decimate_postprocess():
     from dgs_b200 import mesh
-    m = _model(262146, 11)
+    m = shell_model(262146, 11)
     out = m.extract_mesh(postprocess=mesh.clean_then_decimate)
     raw = m.extract_mesh()
     cv, cf = mesh.clean(raw.vertices, raw.faces)
@@ -182,8 +151,8 @@ def test_clean_then_decimate_postprocess():
 
 def test_edge_cases():
     from dgs_b200 import _lib, mesh
-    X, Y, Z = _grid(24)
-    v, f = _mc(8 - torch.sqrt(X * X + Y * Y + Z * Z))
+    X, Y, Z = cuda_grid(24)
+    v, f = mc(8 - torch.sqrt(X * X + Y * Y + Z * Z))
     bad = f.copy()
     bad[7, 1] = len(v)
     with pytest.raises(_lib.DgsError, match="face 7 .* outside"):

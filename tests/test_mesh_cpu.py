@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 import torch
 
+from mesh_shapes import closed_and_oriented, euler, grid, volume
 from oracle import mesh as om
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -58,23 +59,6 @@ def test_table_uses_exactly_the_sign_changing_edges():
             assert not any(a in f and b in f for f in faces), (case, a, b)
 
 
-def _closed_and_oriented(faces):
-    d = np.concatenate([faces[:, [0, 1]], faces[:, [1, 2]], faces[:, [2, 0]]])
-    fwd = {tuple(e) for e in d.tolist()}
-    assert len(fwd) == len(d), "a directed edge is used twice (inconsistent orientation)"
-    assert all((b, a) in fwd for a, b in fwd), "an edge without its opposite (open surface)"
-
-
-def _euler(verts, faces):
-    e = np.sort(np.concatenate([faces[:, [0, 1]], faces[:, [1, 2]], faces[:, [2, 0]]]), axis=1)
-    return len(np.unique(faces)) - len(np.unique(e, axis=0)) + len(faces)
-
-
-def _volume(verts, faces):
-    a, b, c = verts[faces[:, 0]], verts[faces[:, 1]], verts[faces[:, 2]]
-    return float(np.einsum("ij,ij->i", a, np.cross(b, c)).sum() / 6.0)
-
-
 @pytest.mark.parametrize("seed", range(4))
 def test_numpy_marching_cubes_random_fields_closed(seed):
     rng = np.random.default_rng(seed)
@@ -82,27 +66,22 @@ def test_numpy_marching_cubes_random_fields_closed(seed):
     f[0], f[-1], f[:, 0], f[:, -1], f[:, :, 0], f[:, :, -1] = 0, 0, 0, 0, 0, 0  # surface stays inside the grid
     v, t = om.marching_cubes(f, 0.5)
     assert len(t) > 0
-    _closed_and_oriented(t)
-
-
-def _grid(n):
-    x = np.arange(n, dtype=np.float64) - (n - 1) / 2
-    return np.meshgrid(x, x, x, indexing="ij")
+    closed_and_oriented(t)
 
 
 def test_numpy_marching_cubes_sphere_and_torus():
-    X, Y, Z = _grid(40)
+    X, Y, Z = grid(40)
     r = 12.0
     v, t = om.marching_cubes(r - np.sqrt(X ** 2 + Y ** 2 + Z ** 2), 0.0)  # high inside
-    _closed_and_oriented(t)
-    assert _euler(v, t) == 2
-    vol = _volume(v, t)
+    closed_and_oriented(t)
+    assert euler(t) == 2
+    vol = volume(v, t, f64=False)
     assert abs(vol / (4 / 3 * np.pi * r ** 3) - 1) < 0.02  # positive: normals point outwards
     R0, r0 = 11.0, 4.5
     torus = r0 - np.sqrt((np.sqrt(X ** 2 + Y ** 2) - R0) ** 2 + Z ** 2)
     v, t = om.marching_cubes(torus, 0.0)
-    _closed_and_oriented(t)
-    assert _euler(v, t) == 0
+    closed_and_oriented(t)
+    assert euler(t) == 0
 
 
 def test_ply_roundtrip(tmp_path):
@@ -136,7 +115,7 @@ def test_get_covariance_matches_oracle():
 
 def test_mesh_export_ply_and_obj(tmp_path):
     from dgs_b200.mesh import Mesh
-    X, Y, Z = _grid(12)
+    X, Y, Z = grid(12)
     v, t = om.marching_cubes(4.0 - np.sqrt(X ** 2 + Y ** 2 + Z ** 2), 0.0)
     m = Mesh(v, t)
     assert m.vertices.dtype == np.float32 and m.faces.dtype == np.int64

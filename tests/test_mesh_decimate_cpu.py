@@ -6,35 +6,14 @@ import ctypes
 import numpy as np
 import pytest
 
+from mesh_shapes import closed_and_oriented, euler, grid, volume
 from oracle import mesh as om
 from oracle import mesh_decimate as od
 
 
-def _grid(n):
-    x = np.arange(n, dtype=np.float64) - (n - 1) / 2
-    return np.meshgrid(x, x, x, indexing="ij")
-
-
-def _closed_and_oriented(faces):
-    d = np.concatenate([faces[:, [0, 1]], faces[:, [1, 2]], faces[:, [2, 0]]])
-    fwd = {tuple(e) for e in d.tolist()}
-    assert len(fwd) == len(d), "a directed edge is used twice (inconsistent orientation)"
-    assert all((b, a) in fwd for a, b in fwd), "an edge without its opposite (open surface)"
-
-
-def _euler(faces):
-    e = np.sort(np.concatenate([faces[:, [0, 1]], faces[:, [1, 2]], faces[:, [2, 0]]]), axis=1)
-    return len(np.unique(faces)) - len(np.unique(e, axis=0)) + len(faces)
-
-
-def _volume(v, f):
-    v = v.astype(np.float64)
-    return float(np.einsum("ij,ij->i", v[f[:, 0]], np.cross(v[f[:, 1]], v[f[:, 2]])).sum() / 6.0)
-
-
 @pytest.mark.parametrize("shape", ["sphere", "torus"])
 def test_oracle_decimates_closed_surfaces(shape):
-    X, Y, Z = _grid(28)
+    X, Y, Z = grid(28)
     if shape == "sphere":
         r = 9.0
         field, chi = r - np.sqrt(X ** 2 + Y ** 2 + Z ** 2), 2
@@ -48,19 +27,19 @@ def test_oracle_decimates_closed_surfaces(shape):
     ov, of, n = od.decimate(v, f, target)
     c = (np.array(field.shape) - 1) / 2
     d = dist(ov.astype(np.float64) - c)
-    vol0, vol1 = _volume(v, f), _volume(ov, of)
+    vol0, vol1 = volume(v, f), volume(ov, of)
     print(f"{shape}: {len(f)} -> {len(of)} faces ({n} collapses), distance mean {d.mean():.3f} max {d.max():.3f}, "
           f"volume {vol1 / vol0:.4f} of the raw mesh's")
     assert len(of) in (target - 1, target) and n == (len(f) - len(of)) // 2
     assert ov.dtype == np.float32 and of.dtype == np.int64 and len(np.unique(of)) == len(ov)
     assert (of[:, 0] != of[:, 1]).all() and (of[:, 1] != of[:, 2]).all() and (of[:, 0] != of[:, 2]).all()
-    _closed_and_oriented(of)
-    assert _euler(of) == chi
+    closed_and_oriented(of)
+    assert euler(of) == chi
     assert d.max() < 0.5 and abs(vol1 / vol0 - 1) < 0.03
 
 
 def test_oracle_keeps_small_meshes():
-    X, Y, Z = _grid(12)
+    X, Y, Z = grid(12)
     v, f = om.marching_cubes(4.0 - np.sqrt(X ** 2 + Y ** 2 + Z ** 2), 0.0)
     ov, of, n = od.decimate(v, f, len(f))
     assert n == 0 and np.array_equal(ov, v.astype(np.float32)) and np.array_equal(of, f)

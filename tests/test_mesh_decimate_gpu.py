@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 import torch
 
+from mesh_shapes import closed_and_oriented, cuda_grid, directed, euler_per_component, mc, shell_model, volume
 from oracle import mesh_decimate as od
 
 pytestmark = pytest.mark.gpu
@@ -15,62 +16,19 @@ SPHERE_VOL = {5000: 0.002, 500: 0.02}  # |volume / raw volume - 1|: measured 0.0
 PIPELINE_DIST = 7e-3  # max distance of a decimated vertex to the raw surface (extract_mesh units): measured 3.6e-3
 
 
-def _directed(faces):
-    return np.concatenate([faces[:, [0, 1]], faces[:, [1, 2]], faces[:, [2, 0]]])
-
-
-def _closed_and_oriented(faces):
-    d = _directed(faces)
-    fwd = {tuple(e) for e in d.tolist()}
-    assert len(fwd) == len(d), "a directed edge is used twice (inconsistent orientation)"
-    assert all((b, a) in fwd for a, b in fwd), "an edge without its opposite (open surface)"
-
-
 def _clean(faces):
     assert (faces[:, 0] != faces[:, 1]).all() and (faces[:, 1] != faces[:, 2]).all() and (faces[:, 0] != faces[:, 2]).all()
     assert len(np.unique(np.sort(faces, axis=1), axis=0)) == len(faces), "a duplicate face"
 
 
-def _euler_per_component(faces):
-    """-> sorted Euler characteristics V - E + F of the edge-connected components"""
-    from scipy.sparse import coo_matrix
-    from scipy.sparse.csgraph import connected_components
-    n = int(faces.max()) + 1 if len(faces) else 0
-    d = _directed(faces)
-    _, lab = connected_components(coo_matrix((np.ones(len(d)), (d[:, 0], d[:, 1])), shape=(n, n)), directed=False)
-    out = []
-    for c in np.unique(lab[faces[:, 0]]):
-        f = faces[lab[faces[:, 0]] == c]
-        e = np.unique(np.sort(_directed(f), axis=1), axis=0)
-        out.append(len(np.unique(f)) - len(e) + len(f))
-    return sorted(out)
-
-
-def _volume(v, f):
-    v = v.astype(np.float64)
-    return float(np.einsum("ij,ij->i", v[f[:, 0]], np.cross(v[f[:, 1]], v[f[:, 2]])).sum() / 6.0)
-
-
-def _grid(n):
-    x = torch.arange(n, device="cuda", dtype=torch.float32) - (n - 1) / 2
-    return torch.meshgrid(x, x, x, indexing="ij")
-
-
-def _mc(field):
-    """GPU marching cubes at 0 -> numpy (vertices float32 [V, 3] in index coordinates, faces int64 [F, 3])"""
-    from dgs_b200 import mesh
-    v, f = mesh.marching_cubes(field.contiguous(), 0.0)
-    return v.cpu().numpy(), f.cpu().numpy().astype(np.int64)
-
-
 def _sphere(n, r):
-    X, Y, Z = _grid(n)
-    return _mc(r - torch.sqrt(X * X + Y * Y + Z * Z))
+    X, Y, Z = cuda_grid(n)
+    return mc(r - torch.sqrt(X * X + Y * Y + Z * Z))
 
 
 def _torus(n, R0, r0):
-    X, Y, Z = _grid(n)
-    return _mc(r0 - torch.sqrt((torch.sqrt(X * X + Y * Y) - R0) ** 2 + Z * Z))
+    X, Y, Z = cuda_grid(n)
+    return mc(r0 - torch.sqrt((torch.sqrt(X * X + Y * Y) - R0) ** 2 + Z * Z))
 
 
 def _sphere_dist(v, n, r):
@@ -93,14 +51,14 @@ def test_sphere(target):
     v, f = _sphere(n, r)
     ov, of = _decimate(v, f, target)
     d = _sphere_dist(ov, n, r)
-    vol = _volume(ov, of) / _volume(v, f)
+    vol = volume(ov, of) / volume(v, f)
     print(f"sphere r={r}: {len(f)} -> {len(of)} faces, {len(ov)} vertices, distance mean {d.mean():.4f} max "
           f"{d.max():.4f}, volume / raw {vol:.5f}")
     assert ov.dtype == np.float32 and of.dtype == np.int64
     assert len(of) in (target - 1, target)
     _clean(of)
-    _closed_and_oriented(of)
-    assert _euler_per_component(of) == [2]
+    closed_and_oriented(of)
+    assert euler_per_component(of) == [2]
     assert len(np.unique(of)) == len(ov)
     assert d.max() <= SPHERE_DIST[target] and abs(vol - 1) <= SPHERE_VOL[target]
 
@@ -109,28 +67,28 @@ def test_torus_and_two_spheres_keep_topology():
     v, f = _torus(128, 36.0, 14.0)
     ov, of = _decimate(v, f, 2000)
     print(f"torus: {len(f)} -> {len(of)} faces, distance max {_torus_dist(ov, 128, 36.0, 14.0).max():.4f}")
-    assert len(of) in (1999, 2000) and _euler_per_component(of) == [0]
+    assert len(of) in (1999, 2000) and euler_per_component(of) == [0]
     _clean(of)
-    _closed_and_oriented(of)
-    X, Y, Z = _grid(128)
+    closed_and_oriented(of)
+    X, Y, Z = cuda_grid(128)
     two = torch.maximum(20 - torch.sqrt((X - 30) ** 2 + Y * Y + Z * Z), 15 - torch.sqrt((X + 30) ** 2 + Y * Y + Z * Z))
-    v, f = _mc(two)
+    v, f = mc(two)
     ov, of = _decimate(v, f, 1000)
-    print(f"two spheres: {len(f)} -> {len(of)} faces, components {_euler_per_component(of)}")
-    assert len(of) in (999, 1000) and _euler_per_component(of) == [2, 2]
+    print(f"two spheres: {len(f)} -> {len(of)} faces, components {euler_per_component(of)}")
+    assert len(of) in (999, 1000) and euler_per_component(of) == [2, 2]
     _clean(of)
-    _closed_and_oriented(of)
+    closed_and_oriented(of)
 
 
 def test_open_surface_keeps_boundary_loops():
     g = torch.Generator("cuda").manual_seed(0)
     rnd = torch.rand(1, 1, 48, 44, 40, device="cuda", generator=g)
     field = torch.nn.functional.avg_pool3d(rnd, 5, 1, 2, count_include_pad=False)[0, 0]
-    v, f = _mc(field - field.mean())  # not zeroed at the grid's faces: the surface is cut open there
+    v, f = mc(field - field.mean())  # not zeroed at the grid's faces: the surface is cut open there
     ov, of = _decimate(v, f, len(f) // 3)
 
     def boundary(v, f):
-        d = _directed(f)
+        d = directed(f)
         fwd = {tuple(e) for e in d.tolist()}
         return {(tuple(v[a]), tuple(v[b])) for a, b in fwd if (b, a) not in fwd}
     b0, b1 = boundary(v, f), boundary(ov, of)
@@ -138,7 +96,7 @@ def test_open_surface_keeps_boundary_loops():
     assert len(b0) > 100 and b1 == b0  # the same directed edges between bit-identical positions
     assert len(of) < 0.5 * len(f)
     _clean(of)
-    d = _directed(of)
+    d = directed(of)
     assert len({tuple(e) for e in d.tolist()}) == len(d), "a directed edge is used twice"
 
 
@@ -159,32 +117,22 @@ def test_quality_against_serial_oracle(shape):
     print(f"{shape}: {len(f)} -> {len(gf)} (GPU) / {len(rf)} (oracle) faces; distance mean {dg.mean():.4f} / "
           f"{dr.mean():.4f}, max {dg.max():.4f} / {dr.max():.4f}")
     assert len(gf) in (target - 1, target) and len(rf) in (target - 1, target)
-    _closed_and_oriented(gf)
+    closed_and_oriented(gf)
     assert dg.mean() <= 2 * dr.mean() and dg.max() <= 2 * dr.max()
-
-
-def _model(P, seed, dist):
-    from dgs_b200 import synth
-    from dgs_b200.renderer import GaussianModel
-    g = synth.make_shell_gaussians(P, seed, dist)
-    m = GaussianModel(0)
-    m._xyz, m._scaling, m._rotation, m._opacity = (torch.tensor(g[k], device="cuda") for k in
-                                                   ("xyz", "scaling", "rotation", "opacity"))
-    return m
 
 
 def test_extract_mesh_pipeline():
     from scipy.spatial import cKDTree
     from dgs_b200 import mesh
-    m = _model(262146, 11, "fine")
+    m = shell_model(262146, 11, "fine", floaters=False)
     raw = m.extract_mesh()
     dec = m.extract_mesh(postprocess=mesh.decimate)
     again = m.extract_mesh(postprocess=mesh.decimate)
     F = len(dec.faces)
     assert F in (99999, 100000)
     _clean(dec.faces)
-    _closed_and_oriented(dec.faces)
-    chi_raw, chi_dec = _euler_per_component(raw.faces), _euler_per_component(dec.faces)
+    closed_and_oriented(dec.faces)
+    chi_raw, chi_dec = euler_per_component(raw.faces), euler_per_component(dec.faces)
     assert chi_dec == chi_raw
     assert np.array_equal(dec.vertices, again.vertices) and np.array_equal(dec.faces, again.faces)
     tv, tf = mesh.decimate(torch.from_numpy(raw.vertices).cuda(), torch.from_numpy(raw.faces).cuda(), 1e5)
@@ -213,8 +161,8 @@ def test_edge_cases():
     print(f"target 0: {len(f)} -> {len(of)} faces")
     assert 4 <= len(of) < len(f) // 10
     _clean(of)
-    _closed_and_oriented(of)
-    assert _euler_per_component(of) == [2]
+    closed_and_oriented(of)
+    assert euler_per_component(of) == [2]
     bad = f.copy()
     bad[7, 1] = len(v)
     with pytest.raises(_lib.DgsError, match="face 7 .* outside"):

@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 import torch
 
+from mesh_shapes import closed_and_oriented
 from oracle import mesh as om
 
 pytestmark = pytest.mark.gpu
@@ -113,13 +114,6 @@ def test_field_is_deterministic(full):
     assert torch.equal(occ, occ2) and torch.equal(counts, counts2)
 
 
-def _closed_and_oriented(faces):
-    d = np.concatenate([faces[:, [0, 1]], faces[:, [1, 2]], faces[:, [2, 0]]])
-    fwd = {tuple(e) for e in d.tolist()}
-    assert len(fwd) == len(d), "a directed edge is used twice (inconsistent orientation)"
-    assert all((b, a) in fwd for a, b in fwd), "an edge without its opposite (open surface)"
-
-
 def _check_mc(field, iso):
     from dgs_b200 import mesh
     v, f = mesh.marching_cubes(field, iso)
@@ -140,7 +134,7 @@ def test_marching_cubes_matches_oracle_on_fields():
     rnd = torch.rand(40, 33, 27, device="cuda", generator=g)
     rnd[0], rnd[-1], rnd[:, 0], rnd[:, -1], rnd[:, :, 0], rnd[:, :, -1] = 0, 0, 0, 0, 0, 0
     _, f = _check_mc(rnd, 0.5)
-    _closed_and_oriented(f)
+    closed_and_oriented(f)
 
 
 def test_marching_cubes_sphere_volume():
@@ -148,7 +142,7 @@ def test_marching_cubes_sphere_volume():
     x = torch.arange(n, device="cuda", dtype=torch.float32) - (n - 1) / 2
     X, Y, Z = torch.meshgrid(x, x, x, indexing="ij")
     v, f = _check_mc((r - torch.sqrt(X * X + Y * Y + Z * Z)).contiguous(), 0.0)
-    _closed_and_oriented(f)
+    closed_and_oriented(f)
     a, b, c = v[f[:, 0]], v[f[:, 1]], v[f[:, 2]]
     vol = float(np.einsum("ij,ij->i", a, np.cross(b, c)).sum() / 6.0)
     print(f"sphere r={r}: volume / analytic = {vol / (4 / 3 * np.pi * r ** 3):.5f}")
@@ -172,7 +166,7 @@ def test_extract_mesh_end_to_end():
     assert boundary <= 0.005
     assert len(mesh.faces) > 1000 and mesh.faces.dtype == np.int64 and mesh.vertices.dtype == np.float32
     assert (np.abs(mesh.vertices) <= 1).all()
-    _closed_and_oriented(mesh.faces)
+    closed_and_oriented(mesh.faces)
     calls = []
     m.extract_mesh(postprocess=lambda v, f, target: calls.append(target) or (v[:3], f[:1] * 0))
     assert calls == [1e5]

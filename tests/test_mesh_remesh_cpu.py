@@ -3,9 +3,8 @@ an open patch (orientation, topology, boundary loops, face validity, edge length
 brute force, the Python wrapper's argument checks and the command line's --remesh."""
 import numpy as np
 import pytest
-from scipy.sparse import coo_matrix
-from scipy.sparse.csgraph import connected_components
 
+from mesh_shapes import check_remeshed, edges, grid, patch
 from oracle import mesh as om
 from oracle import mesh_clean as oc
 from oracle import mesh_remesh as orr
@@ -17,75 +16,14 @@ def _mc(field):
     return v, f
 
 
-def _grid(n):
-    x = np.arange(n, dtype=np.float64) - (n - 1) / 2
-    return np.meshgrid(x, x, x, indexing="ij")
-
-
 def _sphere(n=28, r=10.0):
-    X, Y, Z = _grid(n)
+    X, Y, Z = grid(n)
     return _mc(r - np.sqrt(X * X + Y * Y + Z * Z))
 
 
 def _torus(n=36):
-    X, Y, Z = _grid(n)
+    X, Y, Z = grid(n)
     return _mc(4.5 - np.sqrt((np.sqrt(X * X + Y * Y) - 10) ** 2 + Z * Z))
-
-
-def _patch(n=14):
-    """An open, gently curved grid patch (a boundary loop of 4 (n - 1) vertices)"""
-    x = np.arange(n, dtype=np.float64)
-    X, Y = np.meshgrid(x, x, indexing="ij")
-    v = np.stack([X, Y, 0.02 * (X - n / 2) ** 2], -1).reshape(-1, 3).astype(np.float32)
-    i = np.arange(n - 1)
-    a = (i[:, None] * n + i[None, :]).reshape(-1)
-    f = np.concatenate([np.stack([a, a + n, a + 1], 1), np.stack([a + 1, a + n, a + n + 1], 1)])
-    return v, f
-
-
-def _edges(f):
-    e = np.sort(np.concatenate([f[:, [0, 1]], f[:, [1, 2]], f[:, [2, 0]]]), 1)
-    return np.unique(e, axis=0, return_counts=True)
-
-
-def _components(f):
-    """-> per edge-connected component: (Euler characteristic V - E + F, whether it has a boundary), sorted"""
-    d = np.concatenate([f[:, [0, 1]], f[:, [1, 2]], f[:, [2, 0]]])
-    key = np.sort(d, 1)
-    fid = np.tile(np.arange(len(f)), 3)
-    order = np.lexsort((fid, key[:, 1], key[:, 0]))
-    ks = key[order]
-    same = np.flatnonzero((ks[1:] == ks[:-1]).all(1)) + 1
-    _, lab = connected_components(coo_matrix((np.ones(len(same)), (fid[order][same], fid[order][same - 1])),
-                                             shape=(len(f), len(f))), directed=False)
-    out = []
-    for c in np.unique(lab):
-        fc = f[lab == c]
-        e, cnt = _edges(fc)
-        out.append((len(np.unique(fc)) - len(e) + len(fc), bool((cnt == 1).any())))
-    return sorted(out)
-
-
-def check_remeshed(v, f, ov, of, L, nondegenerate=True):
-    """The properties every remeshed closed or open surface keeps.  Reprojection may land two vertices of a face on
-    one point of the input (at creases of a coarse input), so large meshes skip the zero-area check."""
-    assert ov.dtype == np.float32 and of.dtype == np.int64 and np.isfinite(ov).all()
-    assert of.min() >= 0 and of.max() < len(ov) and len(np.unique(of)) == len(ov)
-    assert (of[:, 0] != of[:, 1]).all() and (of[:, 1] != of[:, 2]).all() and (of[:, 0] != of[:, 2]).all()
-    assert len(np.unique(np.sort(of, 1), axis=0)) == len(of), "a duplicate face"
-    assert not nondegenerate or (oc.doubled_area(ov, of) > 0).all(), "a zero-area face"
-    # oriented where the input is: no directed edge twice.  An input edge that two faces run in one direction is
-    # blocked: never collapsed or flipped, but each iteration's split may halve it into two such edges
-    def twice(t):
-        d = np.concatenate([t[:, [0, 1]], t[:, [1, 2]], t[:, [2, 0]]])
-        return len(d) - len(np.unique(d, axis=0))
-    assert twice(of) <= 8 * twice(f), f"{twice(of)} edges run twice in one direction (input: {twice(f)})"
-    assert _components(f) == _components(of), "topology changed"
-    e, _ = _edges(of)
-    ln = np.linalg.norm(ov[e[:, 0]].astype(np.float64) - ov[e[:, 1]], axis=1)
-    med = float(np.median(ln))
-    assert 4 * L / 5 <= med <= 4 * L / 3, f"median edge {med} outside [{4 * L / 5}, {4 * L / 3}]"
-    return ln
 
 
 @pytest.mark.parametrize("shape", ["sphere", "torus"])
@@ -94,7 +32,7 @@ def test_oracle_closed_surfaces(shape, L):
     v, f = _sphere() if shape == "sphere" else _torus()
     ov, of, stats = orr.remesh(v, f, L, 3)
     ln = check_remeshed(v, f, ov, of, L)
-    e, cnt = _edges(of)
+    e, cnt = edges(of)
     assert (cnt == 2).all(), "not closed"
     val = np.bincount(e.reshape(-1))
     print(f"{shape} L={L}: {len(f)} -> {len(of)} faces, in [lo, hi] {np.mean((ln >= 0.8 * L) & (ln <= 4 * L / 3)):.3f}, "
@@ -105,12 +43,12 @@ def test_oracle_closed_surfaces(shape, L):
 
 
 def test_oracle_open_patch_keeps_its_boundary():
-    v, f = _patch()
+    v, f = patch()
     ov, of, _ = orr.remesh(v, f, 0.7, 3)
     check_remeshed(v, f, ov, of, 0.7)
-    e, cnt = _edges(f)
+    e, cnt = edges(f)
     b_in = {tuple(v[x]) for x in np.unique(e[cnt == 1])}
-    oe, ocnt = _edges(of)
+    oe, ocnt = edges(of)
     b_out = {tuple(ov[x]) for x in np.unique(oe[ocnt == 1])}
     assert b_in <= b_out, "a boundary vertex moved or went"
     # the boundary is split, never collapsed: its new vertices are midpoints on the old boundary segments

@@ -8,9 +8,9 @@ import numpy as np
 import pytest
 import torch
 
+from mesh_shapes import check_remeshed, components, cuda_grid, edges, mc, patch, shell_model
 from oracle import mesh_clean as oc
 from oracle import mesh_remesh as orr
-from test_mesh_remesh_cpu import _components, _edges, _patch, check_remeshed
 
 pytestmark = pytest.mark.gpu
 
@@ -43,33 +43,21 @@ def _crease_strip():
 @pytest.mark.parametrize("case, L, it", [("tetra", 0.4, 3), ("tetra", 3.0, 2), ("crease_strip", 0.8, 3),
                                          ("crease_strip", 1.7, 2), ("patch", 0.7, 3), ("patch", 1.5, 3)])
 def test_hand_cases_equal_oracle(case, L, it):
-    v, f = {"tetra": _tetra, "crease_strip": _crease_strip, "patch": _patch}[case]()
+    v, f = {"tetra": _tetra, "crease_strip": _crease_strip, "patch": patch}[case]()
     ov, of, st = _same_as_oracle(v, f, L, it)
     print(f"{case} L={L}: {len(f)} -> {len(of)} faces, stats {st}")
-    assert _components(f) == _components(of)
-
-
-def _mc(field):
-    from dgs_b200 import mesh
-    v, f = mesh.marching_cubes(field.contiguous(), 0.0)
-    v, f = mesh.clean(v.cpu().numpy(), f.cpu().numpy().astype(np.int64), min_f=0, min_d=0)
-    return v, f
-
-
-def _grid(n):
-    x = torch.arange(n, device="cuda", dtype=torch.float32) - (n - 1) / 2
-    return torch.meshgrid(x, x, x, indexing="ij")
+    assert components(f) == components(of)
 
 
 def _surface(shape):
-    X, Y, Z = _grid(44)
+    X, Y, Z = cuda_grid(44)
     if shape == "sphere":
-        return _mc(16 - torch.sqrt(X * X + Y * Y + Z * Z))
+        return mc(16 - torch.sqrt(X * X + Y * Y + Z * Z), clean=True)
     if shape == "torus":
-        return _mc(6 - torch.sqrt((torch.sqrt(X * X + Y * Y) - 13) ** 2 + Z * Z))
+        return mc(6 - torch.sqrt((torch.sqrt(X * X + Y * Y) - 13) ** 2 + Z * Z), clean=True)
     a = 9 - torch.sqrt((X - 10) ** 2 + Y * Y + Z * Z)
     b = 8 - torch.sqrt((X + 10) ** 2 + Y * Y + Z * Z)
-    return _mc(torch.maximum(a, b))
+    return mc(torch.maximum(a, b), clean=True)
 
 
 @pytest.mark.parametrize("shape", ["sphere", "torus", "two_spheres"])
@@ -82,26 +70,9 @@ def test_surfaces_equal_oracle(shape, L, it):
         check_remeshed(v, f, ov, of, L)
 
 
-def _model(P, seed, floaters=True):
-    from dgs_b200 import synth
-    from dgs_b200.renderer import GaussianModel
-    g = synth.make_shell_gaussians(P, seed, "fine")
-    if floaters:
-        rng = np.random.default_rng(seed)
-        k = 400
-        for c in [(0.8, 0.7, 0.0), (-0.7, -0.75, 0.6), (0.1, -0.8, -0.7)]:
-            extra = {key: g[key][:k].copy() for key in g}
-            extra["xyz"] = (np.asarray(c) + rng.normal(0, 0.01, (k, 3))).astype(np.float32)
-            g = {key: np.concatenate([g[key], extra[key]]) for key in g}
-    m = GaussianModel(0)
-    m._xyz, m._scaling, m._rotation, m._opacity = (torch.tensor(g[k], device="cuda") for k in
-                                                   ("xyz", "scaling", "rotation", "opacity"))
-    return m
-
-
 def test_obj256_properties():
     from dgs_b200 import mesh
-    m = _model(262146, 11)
+    m = shell_model(262146, 11)
     raw = m.extract_mesh()
     v, f = mesh.clean(raw.vertices, raw.faces)
     L = 0.015
@@ -110,7 +81,7 @@ def test_obj256_properties():
     ln = check_remeshed(v, f, ov, of, L, nondegenerate=False)
     _, d2, _ = orr.closest_points(v, f, ov.astype(np.float64))
     share = float(np.mean((ln >= 0.8 * L) & (ln <= 4 * L / 3)))
-    e, _ = _edges(of)
+    e, _ = edges(of)
     dval = float(np.abs(np.bincount(e.reshape(-1)) - 6).mean())
     print(f"obj-256 cleaned: {len(f)} -> {len(of)} faces, stats {st['iterations']}, max distance to S "
           f"{np.sqrt(d2).max():.2e}, edges in [lo, hi] {share:.3f}, mean |valence - 6| {dval:.3f}, zero-area faces "
@@ -136,7 +107,7 @@ def _boundary_loops(f):
     """-> the number of connected pieces of the edges with one face"""
     from scipy.sparse import coo_matrix
     from scipy.sparse.csgraph import connected_components
-    e, cnt = _edges(f)
+    e, cnt = edges(f)
     b = e[cnt == 1]
     if not len(b):
         return 0
@@ -161,25 +132,25 @@ def test_clean_remesh_then_decimate_closed_sphere():
     field = _sphere_field(96, 0.6)
     raw = mesh.extract_mesh(field, 0.0, 96)
     cv, cf = mesh.clean(raw.vertices, raw.faces)
-    assert (_edges(cf)[1] == 2).all(), "the cleaned sphere is not closed"
+    assert (edges(cf)[1] == 2).all(), "the cleaned sphere is not closed"
     out = mesh.extract_mesh(field, 0.0, 96, postprocess=mesh.clean_remesh_then_decimate, decimate_target=20000)
-    _, cnt = _edges(out.faces)
+    _, cnt = edges(out.faces)
     print(f"sphere through clean_remesh_then_decimate: {len(cf)} cleaned -> {len(out.faces)} faces")
     assert 0 < len(out.faces) <= 20000 and (cnt == 2).all(), "not closed"
-    assert _components(out.faces) == [(2, False)]
+    assert components(out.faces) == [(2, False)]
     raw = mesh.extract_mesh(_sphere_field(128, 0.6), 0.0, 128)
     rv, rf = mesh.remesh(raw.vertices, raw.faces)
-    assert (_edges(rf)[1] == 2).all() and _components(rf) == [(2, False)]
+    assert (edges(rf)[1] == 2).all() and components(rf) == [(2, False)]
 
 
 def test_clean_remesh_then_decimate_postprocess():
     from dgs_b200 import mesh
-    m = _model(262146, 11)
+    m = shell_model(262146, 11)
     out = m.extract_mesh(postprocess=mesh.clean_remesh_then_decimate)
     raw = m.extract_mesh()
     cv, cf = mesh.clean(raw.vertices, raw.faces)
-    _, cnt = _edges(out.faces)
-    _, ccnt = _edges(cf)
+    _, cnt = edges(out.faces)
+    _, ccnt = edges(cf)
     print(f"clean_remesh_then_decimate: {len(out.faces)} faces, {int((cnt == 1).sum())} boundary edges in "
           f"{_boundary_loops(out.faces)} loops (the cleaned input {int((ccnt == 1).sum())} in {_boundary_loops(cf)})")
     assert len(out.faces) <= 1e5 and (cnt <= 2).all()
