@@ -424,18 +424,25 @@ def mod_table64(model, c):
     return torch.cat([F.linear(s, lin.weight.double(), lin.bias.double()) for lin in lins], dim=1)
 
 
-def gaussians_epilogue64(gs_tok, img_gs, ray_o, ray_d, depth_mode, near=0.0, far=500.0, defects=()):
-    """The raw head outputs -> the renderer-ready Gaussians (denoiser.py:103-120, 362-413; denoiser_scene.py:263,
-    406-410) in fp64.  gs_tok [B, G, 14], img_gs [B, T, p*p*14]; depth_mode 0: (2 sigmoid(m) - 1) * 1.8 + o.(-d)
+def head_channels(sh_degree):
+    """Channels per Gaussian of both heads: xyz 3 | features 3 (d+1)^2 | scaling 3 | rotation 4 | opacity 1."""
+    return 11 + 3 * (sh_degree + 1) ** 2
+
+
+def gaussians_epilogue(gs_tok, img_gs, ray_o, ray_d, depth_mode, near=0.0, far=500.0, defects=()):
+    """The raw head outputs -> the renderer-ready Gaussians (denoiser.py:94-98, 103-120, 145-149, 362-413;
+    denoiser_scene.py:263, 406-410) in the dtype of the inputs.  gs_tok [B, G, C], img_gs [B, T, p*p*C] with
+    C = head_channels(d) split [xyz 3 | features 3 (d+1)^2 | scaling 3 | rotation 4 | opacity 1]; the features reshape
+    coefficient-major, RGB-minor to [B, G + T*p*p, (d+1)^2, 3].  depth_mode 0: (2 sigmoid(m) - 1) * 1.8 + o.(-d)
     (object model, 'relative_plk'), 1: sigmoid(m) * (far - near) + near (scene model), 2: sigmoid(m) (object model,
     'plk').  -> {xyz, features, scaling, rotation, opacity, img_aligned_xyz, depth_m (the sigmoid argument m)}."""
-    ray_o, ray_d = ray_o.double(), ray_d.double()
     b, v, _, h, w = ray_o.shape
-    p = math.isqrt(img_gs.shape[-1] // 14)
-    img_g = img_gs.double().reshape(b, -1, 14)
-    allg = torch.cat((gs_tok.double(), img_g), dim=1)
-    xyz, features, scaling, rotation, opacity = allg.split([3, 3, 3, 4, 1], dim=2)
-    features = features.reshape(b, -1, 1, 3)
+    C = gs_tok.shape[-1]
+    p = math.isqrt(img_gs.shape[-1] // C)
+    img_g = img_gs.reshape(b, -1, C)
+    allg = torch.cat((gs_tok, img_g), dim=1)
+    xyz, features, scaling, rotation, opacity = allg.split([3, C - 11, 3, 4, 1], dim=2)
+    features = features.reshape(b, -1, (C - 11) // 3, 3)
     if "clamp_grad_everywhere" in defects:
         scaling = scaling - 2.3 + ((scaling - 2.3).clamp(max=-1.20) - (scaling - 2.3)).detach()
     else:
@@ -460,9 +467,15 @@ def gaussians_epilogue64(gs_tok, img_gs, ray_o, ray_d, depth_mode, near=0.0, far
                 depth_m=m)
 
 
+def gaussians_epilogue64(gs_tok, img_gs, ray_o, ray_d, depth_mode, near=0.0, far=500.0, defects=()):
+    """gaussians_epilogue in fp64."""
+    return gaussians_epilogue(gs_tok.double(), img_gs.double(), ray_o.double(), ray_d.double(), depth_mode, near, far,
+                              defects)
+
+
 def heads64(model, x, mod_heads, ray_o, ray_d, depth_mode, near=0.0, far=500.0, matched=False, defects=(), feed=None):
     """The two heads on the final residual stream x [B, G + T, w] with their modulation mod_heads [B, 4w] (the last
-    4w columns of mod_table64): {gs_tok [B, G, 14], img_gs [B, T, p*p*14], h_ups, h_dec} and every output of
+    4w columns of mod_table64): {gs_tok [B, G, C], img_gs [B, T, p*p*C], h_ups, h_dec} and every output of
     gaussians_epilogue64.  matched: the upsampler and decoder products split-bf16 as the kernels compute them; in the
     backward the decoder's output gradient d_img and both heads' dh rounded to bf16, dh of the decoder through hi(W),
     and its weight gradient through hi(h).  feed: {"gs_tok" / "img_gs": tensor} -- the epilogue runs on the given raw
@@ -495,7 +508,7 @@ def _init_linear(m):
 
 class DenoiserOracle(nn.Module):
     def __init__(self, width=1024, heads=16, layers=24, patch=8, n_gaussians=2, scene=False, near=0.0, far=500.0,
-                 ray_pe_type=None):
+                 ray_pe_type=None, sh_degree=0):
         super().__init__()
         self.width, self.patch, self.G, self.scene, self.near, self.far = width, patch, n_gaussians, scene, near, far
         # yaml defaults: object configs leave the class default 'relative_plk' (denoiser.py:186), scene configs set 'plk'
@@ -511,9 +524,10 @@ class DenoiserOracle(nn.Module):
         self.transformer_input_layernorm = nn.LayerNorm(width, bias=False)
         self.transformer = nn.ModuleList([DiTBlock(width, heads) for _ in range(layers)])
         self.transformer.apply(_init_linear)
-        self.upsampler = _Head(width, 14)
+        C = head_channels(sh_degree)
+        self.upsampler = _Head(width, C)
         self.upsampler.apply(_init_linear)
-        self.image_token_decoder = _Head(width, patch * patch * 14)
+        self.image_token_decoder = _Head(width, patch * patch * C)
         self.image_token_decoder.apply(_init_linear)
 
     def image_to_gaussians(self, images, ray_o, ray_d, t, return_tokens=False):
@@ -534,24 +548,10 @@ class DenoiserOracle(nn.Module):
             x = blk(x, temb)
         tokens = x
         g_tok, i_tok = x.split([self.G, x.shape[1] - self.G], dim=1)
-        gaussians = self.upsampler(g_tok, temb)
-        img_g = self.image_token_decoder(i_tok, temb).reshape(b, -1, 14)
-        allg = torch.cat((gaussians, img_g), dim=1)
-        xyz, features, scaling, rotation, opacity = allg.split([3, 3, 3, 4, 1], dim=2)
-        features = features.reshape(b, -1, 1, 3)
-        scaling = (scaling - 2.3).clamp(max=-1.20)
-        opacity = opacity - 2.0
-        n_img = img_g.shape[1]
-        ia = xyz[:, -n_img:, :].reshape(b, v, h // p, w // p, p, p, 3).permute(0, 1, 6, 2, 4, 3, 5).reshape(b, v, 3, h, w)
-        ia = ia.mean(dim=2, keepdim=True)
-        if self.scene:  # denoiser_scene.py:263,406-410 (range_func, whatever ray_pe_type is)
-            depth = torch.sigmoid(ia) * (self.far - self.near) + self.near
-        elif self.ray_pe_type == "relative_plk":  # denoiser.py:381-388
-            depth = (2.0 * torch.sigmoid(ia) - 1.0) * 1.8 + o_dot_d
-        else:
-            depth = torch.sigmoid(ia)
-        ia = ray_o + depth * ray_d
-        ia_flat = ia.reshape(b, v, 3, h // p, p, w // p, p).permute(0, 1, 3, 5, 4, 6, 2).reshape(b, -1, 3)
-        xyz = torch.cat((xyz[:, :-n_img, :], ia_flat), dim=1)
-        out = dict(xyz=xyz, features=features, scaling=scaling, rotation=rotation, opacity=opacity)
+        # the scene model's range_func whatever ray_pe_type is (denoiser_scene.py:263,406-410); denoiser.py:381-388
+        depth_mode = 1 if self.scene else (0 if self.ray_pe_type == "relative_plk" else 2)
+        g = gaussians_epilogue(self.upsampler(g_tok, temb), self.image_token_decoder(i_tok, temb), ray_o, ray_d,
+                               depth_mode, self.near, self.far)
+        out = {k: g[k] for k in ("xyz", "features", "scaling", "rotation", "opacity")}
+        ia = g["img_aligned_xyz"]
         return (out, ia, tokens) if return_tokens else (out, ia)

@@ -13,10 +13,14 @@ rescales a DGSDenoiser (or the oracle's DenoiserOracle: same module tree) in pla
   through 24 layers.
 
 tests/test_dit_block_power_cpu.py pins the resulting statistics on the oracle.
+
+Also the seeded DiT inputs of the GPU tests (`dit_inputs`) and the oracle of a product model (`oracle_like`).
 """
 import math
 
 import torch
+
+DEV = "cuda:0"
 
 ADALN_BIAS_STD = 0.2
 ADALN_DYNAMIC_RMS = 0.2
@@ -64,3 +68,26 @@ def apply_trained_scale(model, seed=0):
         _fill(head.adaLN_modulation[1].weight, g, adaln_w_std)
         _fill(head.adaLN_modulation[1].bias, g, ADALN_BIAS_STD)
     return model
+
+
+def oracle_like(model, **kw):
+    """A DenoiserOracle with the configuration of the product model `model` (DGSDenoiser[Scene]), its parameters
+    loaded strictly."""
+    from oracle.dit import DenoiserOracle
+    c = model.cfg
+    o = DenoiserOracle(width=c.width, heads=c.width // c.dim_heads, layers=c.num_layers, patch=c.patch_size,
+                       n_gaussians=c.n_gaussians, scene=model.SCENE, near=c.range_setting_near, far=c.range_setting_far,
+                       ray_pe_type=c.ray_pe_type, sh_degree=c.gaussians_sh_degree, **kw)
+    o.load_state_dict({k: v.detach() for k, v in model.state_dict().items()}, strict=True)
+    return o.to(model.device)
+
+
+def dit_inputs(B, V, H, W, seed=0):
+    """Seeded (images, ray_o, ray_d, t) on the device: view 0 in [0, 1), the other views N(0, 1)."""
+    g = torch.Generator(DEV).manual_seed(seed)
+    images = torch.rand(B, V, 3, H, W, device=DEV, generator=g)
+    images[:, 1:] = torch.randn(B, V - 1, 3, H, W, device=DEV, generator=g)
+    ray_o = torch.randn(B, V, 3, 1, 1, device=DEV, generator=g).expand(B, V, 3, H, W).contiguous() * 1.5
+    ray_d = torch.nn.functional.normalize(torch.randn(B, V, 3, H, W, device=DEV, generator=g), dim=2)
+    t = torch.randint(0, 1000, (B,), device=DEV, generator=g)
+    return images, ray_o, ray_d, t

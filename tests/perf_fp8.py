@@ -98,10 +98,10 @@ def gemms(L):
 
 def step_times():
     from dgs_b200.denoiser import DGSDenoiser
-    from test_dit_gpu import _inputs
+    from dit_regime import dit_inputs
     torch.manual_seed(0)
     model = DGSDenoiser(dict(patch_size=8, num_layers=24)).to(DEV).eval()
-    inputs = _inputs(1, 4, 256, 256, seed=0)
+    inputs = dit_inputs(1, 4, 256, 256, seed=0)
     scratch = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=DEV)
 
     def run(prec):

@@ -76,10 +76,10 @@ def kernels(N, windows, iters, H=16, B=1):
 
 def dit(res_hw, steps, layers=24):
     from dgs_b200.denoiser import DGSDenoiser
-    from test_dit_gpu import _inputs
+    from dit_regime import dit_inputs
     torch.manual_seed(0)
     model = DGSDenoiser(dict(patch_size=8, num_layers=layers)).to(DEV).eval()
-    inputs = _inputs(1, 4, res_hw, res_hw, seed=0)
+    inputs = dit_inputs(1, 4, res_hw, res_hw, seed=0)
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=DEV)  # > the 50 MB L2
     t = {"fp8": [], "fp8_attention": []}
     with torch.no_grad():

@@ -101,12 +101,12 @@ def bench_step(B, V, H, steps):
     from dgs_b200.denoiser import DGSDenoiser
     from dgs_b200.losses import LossComputer, fused_render_and_loss
     from dgs_b200.train import DitTrainer
-    from test_dit_gpu import _inputs
+    from dit_regime import dit_inputs
     torch.manual_seed(0)
     model = DGSDenoiser(dict(patch_size=8)).to(DEV)
     trainer = DitTrainer(model, recompute=True)
     model.train()
-    images, ray_o, ray_d, t = _inputs(B, V, H, H)
+    images, ray_o, ray_d, t = dit_inputs(B, V, H, H)
     c2w, fx = synth.orbit_cameras(V, H, H)
     c2w = torch.tensor(c2w[None], device=DEV).expand(B, -1, -1, -1).contiguous()
     fx = torch.tensor(fx[None], device=DEV).expand(B, -1, -1).contiguous()

@@ -25,7 +25,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "open-diffusiongs_b200"))
 from dgs_b200 import _lib, raster, synth  # noqa: E402
 from perf_dit_linears import card, load_lib  # noqa: E402
-from util import scene_c1  # noqa: E402
+from util import rel_l2 as rel, scene_c1  # noqa: E402
 
 DEV = "cuda:0"
 
@@ -156,10 +156,6 @@ def same(a, b):
     if isinstance(a, torch.Tensor):
         return bool(a.shape == b.shape and torch.equal(a, b))
     return a == b
-
-
-def rel(a, b):
-    return float((a.double() - b.double()).norm() / (b.double().norm() + 1e-30))
 
 
 def run(name, wl, libs):

@@ -13,7 +13,8 @@ import torch
 
 from oracle.attention import (ATTENTION_DEFECTS, C, attention_bwd_matched, attention_fwd_matched)
 from test_attention_gpu import (BWD_DK_REL, BWD_DQ_REL, BWD_DV_REL, FWD_DIFF_FRAC, FWD_LSE, FWD_OUT_REL, REGIMES,
-                                SHAPES, bits_stats, make_qkv, rel)
+                                SHAPES, bits_stats, make_qkv)
+from util import rel_l2 as rel
 
 CPU_SHAPES = [s for s in SHAPES if s[0] * s[1] * s[2] <= 2000]  # the GPU test's shapes small enough for the CPU
 

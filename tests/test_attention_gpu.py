@@ -12,10 +12,11 @@ fp32 accumulation order and ex2.approx.
 Every bound below was set from the errors measured on an H100 80GB HBM3 over seeds 0, 1, 2; the measured worst case
 is written next to it.
 """
-import ctypes as C
-
 import pytest
 import torch
+
+from dgs_b200 import _lib
+from util import rel_l2 as rel
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -49,25 +50,6 @@ SHAPES = [(1, 1, 1), (2, 64, 3), (3, 77, 2), (1, 129, 20), (2, 226, 1), (1, 256,
           (2, 383, 5), (1, 130, 64), (1, 4098, 16), (3, 4098, 16), (1, 16386, 2)]
 
 
-def lib():
-    from dgs_b200 import _lib
-    return _lib.lib()
-
-
-def check(rc):
-    from dgs_b200 import _lib
-    _lib.check(rc)
-
-
-def stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def rel(a, b):
-    a, b = a.double(), b.double()
-    return float((a - b).norm() / (b.norm() + 1e-30))
-
-
 def lse_stride(N):
     return (N + 127) // 128 * 128
 
@@ -91,10 +73,11 @@ def attention_fwd(qkv, train):
     B, N, _, H, _ = qkv.shape
     out = torch.empty(B, N, H * 64, dtype=torch.bfloat16, device=DEV)
     if not train:
-        check(lib().dgs_attention_fwd(qkv.data_ptr(), out.data_ptr(), B, N, H, stream()))
+        _lib.check(_lib.lib().dgs_attention_fwd(qkv.data_ptr(), out.data_ptr(), B, N, H, _lib.stream(None)))
         return out, None
     lse2 = torch.full((B, H, lse_stride(N)), float("nan"), device=DEV)
-    check(lib().dgs_attention_fwd_train(qkv.data_ptr(), out.data_ptr(), lse2.data_ptr(), B, N, H, stream()))
+    _lib.check(_lib.lib().dgs_attention_fwd_train(qkv.data_ptr(), out.data_ptr(), lse2.data_ptr(), B, N, H,
+                                                  _lib.stream(None)))
     return out, lse2
 
 
@@ -102,8 +85,8 @@ def attention_bwd(qkv, out, dout, lse2):
     B, N, _, H, _ = qkv.shape
     dsum = torch.full_like(lse2, float("nan"))
     dqkv = torch.empty_like(qkv)
-    check(lib().dgs_attention_bwd(qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse2.data_ptr(), dsum.data_ptr(),
-                                  dqkv.data_ptr(), B, N, H, stream()))
+    _lib.check(_lib.lib().dgs_attention_bwd(qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse2.data_ptr(),
+                                            dsum.data_ptr(), dqkv.data_ptr(), B, N, H, _lib.stream(None)))
     return dqkv, dsum
 
 
@@ -200,7 +183,7 @@ def _guards_intact(buf, sentinel, guard=4096):
 def test_guard_bands_and_pads(B, N, H):
     """Nothing outside out, lse2, dsum and dqkv is written; the forward leaves the lse2 pads [N, Np) alone, the backward
     sets them to +inf and the dsum pads to 0."""
-    L = lib()
+    L = _lib.lib()
     g = torch.Generator(DEV).manual_seed(N)
     qkv = make_qkv(B, N, H, "scale1.5", 0)
     dout = torch.randn(B, N, H * 64, device=DEV, generator=g).to(torch.bfloat16)
@@ -209,18 +192,18 @@ def test_guard_bands_and_pads(B, N, H):
     lse2, lse_buf, lse_s = _guarded((B, H, Np), torch.float32, g)
     dsum, dsum_buf, dsum_s = _guarded((B, H, Np), torch.float32, g)
     dqkv, dqkv_buf, dqkv_s = _guarded((B, N, 3, H, 64), torch.bfloat16, g)
-    check(L.dgs_attention_fwd(qkv.data_ptr(), out.data_ptr(), B, N, H, stream()))
+    _lib.check(L.dgs_attention_fwd(qkv.data_ptr(), out.data_ptr(), B, N, H, _lib.stream(None)))
     torch.cuda.synchronize()
     assert _guards_intact(out_buf, out_s)
     out_inf = out.clone()
-    check(L.dgs_attention_fwd_train(qkv.data_ptr(), out.data_ptr(), lse2.data_ptr(), B, N, H, stream()))
+    _lib.check(L.dgs_attention_fwd_train(qkv.data_ptr(), out.data_ptr(), lse2.data_ptr(), B, N, H, _lib.stream(None)))
     torch.cuda.synchronize()
     assert _guards_intact(out_buf, out_s) and _guards_intact(lse_buf, lse_s)
     assert torch.equal(out, out_inf)
     pads = lse_s[4096:4096 + B * H * Np].view(B, H, Np)[..., N:]
     assert torch.equal(lse2[..., N:], pads)  # the forward leaves the pad entries untouched
-    check(L.dgs_attention_bwd(qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse2.data_ptr(), dsum.data_ptr(),
-                              dqkv.data_ptr(), B, N, H, stream()))
+    _lib.check(L.dgs_attention_bwd(qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse2.data_ptr(), dsum.data_ptr(),
+                                   dqkv.data_ptr(), B, N, H, _lib.stream(None)))
     torch.cuda.synchronize()
     assert _guards_intact(lse_buf, lse_s) and _guards_intact(dsum_buf, dsum_s) and _guards_intact(dqkv_buf, dqkv_s)
     assert _guards_intact(out_buf, out_s) and torch.equal(out, out_inf)

@@ -12,7 +12,8 @@ import copy
 import pytest
 import torch
 
-from test_dit_blocks_bwd_gpu import BWD, _rel
+from test_dit_blocks_bwd_gpu import BWD
+from util import rel_l2 as _rel
 
 D, B, N = 1024, 2, 130
 

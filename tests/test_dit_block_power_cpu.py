@@ -14,7 +14,7 @@ import pytest
 import torch
 
 from test_dit_blocks_gpu import BLOCK_MATCHED
-from test_dit_gpu import rel
+from util import rel_l2 as rel
 
 D = 1024
 

@@ -22,6 +22,8 @@ import gc
 import pytest
 import torch
 
+from util import rel_l2 as _rel
+
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 OBJ256 = (1, 4, 256, 256)  # N = 4098 tokens: 32 full 128-row tiles and a 2-row tail
@@ -54,17 +56,12 @@ PLAIN_DX = 4e-2  # dx[l] - dx[l+1] against the plain fp64 backward (all bf16 rou
 RECOMPUTE_PARAM = 5e-7
 
 
-def _rel(a, b):
-    a, b = a.detach().double(), b.detach().double()
-    return float((a - b).norm() / (b.norm() + 1e-30))
-
-
 def backward_run(model, trainer, shape, seed, recompute, names=None):
     """One training forward + traced backward of the loss tests/test_dit_bwd_gpu._grad_compare uses (seeded random
     weights on the five outputs) -> ({name: stacked trace}, {parameter name: gradient copy})."""
-    from test_dit_gpu import _inputs
+    from dit_regime import dit_inputs
     trainer.recompute = recompute
-    inputs = _inputs(*shape, seed=seed)
+    inputs = dit_inputs(*shape, seed=seed)
     tr = trainer.trace_backward() if names is None else trainer.trace_backward(names)
     with torch.enable_grad():
         out, _ = model.image_to_gaussians(*inputs)
@@ -183,12 +180,12 @@ def test_trace_does_not_change_the_backward(obj24):
     the atomically accumulated ones equal to 1e-6.  At M = 4098 the qkv, fc1 and fc2 weight gradients are written tile by
     tile; attn.proj's (64 output tiles of 128 x 128) runs split-K with fp32 atomics, like the biases, the LayerNorm
     weights and the adaLN table's gradients, so its summation order varies from run to run."""
-    from test_dit_gpu import _inputs
+    from dit_regime import dit_inputs
     model, trainer, _ = obj24
     grads = []
     for traced in (False, True):
         trainer.recompute = False
-        inputs = _inputs(*OBJ256, seed=4)
+        inputs = dit_inputs(*OBJ256, seed=4)
         if traced:
             trainer.trace_backward()
         with torch.enable_grad():

@@ -22,7 +22,8 @@ import types
 import pytest
 import torch
 
-from test_dit_gpu import _inputs, rel
+from dit_regime import dit_inputs
+from util import rel_l2 as rel
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -73,7 +74,7 @@ def build_models(layers, scene=False, seed=0):
 def _train_forward(model, trainer, shape, seed, recompute):
     """One training forward (the train state keeps the per-block tensors), then drop it without a backward."""
     trainer.recompute = recompute
-    inputs = _inputs(*shape, seed=seed)
+    inputs = dit_inputs(*shape, seed=seed)
     with torch.enable_grad():
         model.image_to_gaussians(*inputs)
     trainer.reset()

@@ -5,22 +5,13 @@ torch autograd over the fp32 oracle (oracle/dit.py) with the same fp32 master we
 Tolerances: the backward runs its GEMMs / attention with bf16 operands (gradient activations rounded to bf16, like
 torch autocast), fp32 accumulation, fp32 residual-stream gradient and fp32 weight gradients.  Expected norm-wise error
 per tensor ~ a few 1e-3; each bound is written at its assert."""
-import ctypes as C
-
 import pytest
 import torch
 
+from util import rel_l2 as rel
+
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
-
-
-def rel(a, b):
-    a, b = a.double(), b.double()
-    return float((a - b).norm() / (b.norm() + 1e-30))
-
-
-def stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def ptr(t):
@@ -37,7 +28,8 @@ def test_transpose_bf16(M, Cc, f32):
     Mp = (M + 63) // 64 * 64
     out = torch.full((Cc, Mp), 7.0, dtype=torch.bfloat16, device=DEV)
     cs = torch.zeros(Cc, device=DEV)
-    _lib.check(_lib.lib().dgs_transpose_bf16(x.data_ptr(), int(f32), M, Cc, out.data_ptr(), cs.data_ptr(), stream()))
+    _lib.check(_lib.lib().dgs_transpose_bf16(x.data_ptr(), int(f32), M, Cc, out.data_ptr(), cs.data_ptr(),
+                                             _lib.stream(None)))
     xb = x.to(torch.bfloat16)
     assert torch.equal(out[:, :M], xb.t())
     assert torch.all(out[:, M:] == 0)
@@ -57,8 +49,9 @@ def test_attention_backward_vs_autograd(B, N, H):
     lse = torch.full((B, H, Np), float("nan"), device=DEV)
     dsum = torch.full((B, H, Np), float("nan"), device=DEV)
     dqkv = torch.full((B, N, 3, H, 64), float("nan"), dtype=torch.bfloat16, device=DEV)
-    _lib.check(L.dgs_attention_fwd_train(ptr(qkv), ptr(out), ptr(lse), B, N, H, stream()))
-    _lib.check(L.dgs_attention_bwd(ptr(qkv), ptr(out), ptr(dout), ptr(lse), ptr(dsum), ptr(dqkv), B, N, H, stream()))
+    _lib.check(L.dgs_attention_fwd_train(ptr(qkv), ptr(out), ptr(lse), B, N, H, _lib.stream(None)))
+    _lib.check(L.dgs_attention_bwd(ptr(qkv), ptr(out), ptr(dout), ptr(lse), ptr(dsum), ptr(dqkv), B, N, H,
+                                   _lib.stream(None)))
     torch.cuda.synchronize()
     x = qkv.float().requires_grad_(True)
     q, k, v = [t.permute(0, 2, 1, 3) for t in x.unbind(2)]
@@ -95,7 +88,7 @@ def test_ln_modulate_backward():
         dh_in = dh.float().contiguous() if f32 else dh
         _lib.check(_lib.lib().dgs_ln_modulate_bwd(ptr(x), ptr(dh_in), int(f32), ptr(w_), mod[:, D:].data_ptr(), 6 * D, B, R,
                                                   D, eps, ptr(dx), 1, ptr(dmod), dmod[:, D:].data_ptr(),
-                                                  ptr(dw) if w_ is not None else None, ptr(stats), stream()))
+                                                  ptr(dw) if w_ is not None else None, ptr(stats), _lib.stream(None)))
         assert rel(dx - 1, x.grad) < 1e-4
         assert rel(dmod[:, :2 * D], mod.grad[:, :2 * D]) < 1e-4
         if w_ is not None:
@@ -107,7 +100,7 @@ def test_ln_modulate_backward():
     dx = torch.zeros(B, R, D, device=DEV)
     dw = torch.zeros(D, device=DEV)
     _lib.check(_lib.lib().dgs_ln_modulate_bwd(ptr(x), ptr(dh), 0, ptr(lnw), None, 0, B, R, D, 1e-5, ptr(dx), 0, None, None,
-                                              ptr(dw), ptr(stats), stream()))
+                                              ptr(dw), ptr(stats), _lib.stream(None)))
     assert rel(dx, x.grad) < 1e-4 and rel(dw, lnw.grad) < 1e-4
 
 
@@ -124,7 +117,7 @@ def test_gate_backward():
     dmod = torch.zeros(B, 3 * Cc, device=DEV)
     db = torch.zeros(Cc, device=DEV)
     _lib.check(_lib.lib().dgs_gate_bwd(ptr(dx), ptr(y), mod[:, Cc:].data_ptr(), 3 * Cc, R, M, Cc, ptr(dy), ptr(dyT),
-                                       dmod[:, Cc:].data_ptr(), ptr(db), stream()))
+                                       dmod[:, Cc:].data_ptr(), ptr(db), _lib.stream(None)))
     gate = mod[:, Cc:2 * Cc].repeat_interleave(R, dim=0)
     ref_dy = (gate * dx).to(torch.bfloat16)
     assert torch.equal(dy, ref_dy)
@@ -149,7 +142,7 @@ def test_adamw_matches_torch():
         ref_p.grad = grad.clone()
         opt.step()
         _lib.check(_lib.lib().dgs_adamw_step(ptr(p), ptr(grad), ptr(m), ptr(v), n, 1e-3, 0.9, 0.99, 1e-8, 0.01, step, 0.5,
-                                             ptr(two), stream()))
+                                             ptr(two), _lib.stream(None)))
     assert rel(p, ref_p.data) < 1e-6
 
 
@@ -159,7 +152,7 @@ def _grad_compare(layers, B, V, H, W, scene, tag, seed=0, regime=None, sq_errs=N
     from dgs_b200.denoiser import DGSDenoiser, DGSDenoiserScene
     from dgs_b200.train import DitTrainer
     from oracle.dit import DenoiserOracle
-    from test_dit_gpu import _inputs
+    from dit_regime import dit_inputs
     torch.manual_seed(seed)
     cfg = dict(patch_size=8, num_layers=layers, ray_pe_type="plk" if scene else "relative_plk")
     model = (DGSDenoiserScene if scene else DGSDenoiser)(cfg)
@@ -170,7 +163,7 @@ def _grad_compare(layers, B, V, H, W, scene, tag, seed=0, regime=None, sq_errs=N
     oracle.load_state_dict(model.state_dict(), strict=True)
     trainer = DitTrainer(model)
     model.train()
-    images, ray_o, ray_d, t = _inputs(B, V, H, W)
+    images, ray_o, ray_d, t = dit_inputs(B, V, H, W)
     g = torch.Generator(DEV).manual_seed(11)
     out, _ = model.image_to_gaussians(images, ray_o, ray_d, t)
     assert out.xyz.requires_grad
@@ -221,7 +214,7 @@ def test_train_steps_reduce_loss_and_track_oracle():
     from dgs_b200.denoiser import DGSDenoiser
     from dgs_b200.train import DitTrainer
     from oracle.dit import DenoiserOracle
-    from test_dit_gpu import _inputs
+    from dit_regime import dit_inputs
     torch.manual_seed(0)
     model = DGSDenoiser(dict(patch_size=8, num_layers=2)).to(DEV)
     oracle = DenoiserOracle(layers=2).to(DEV)
@@ -229,7 +222,7 @@ def test_train_steps_reduce_loss_and_track_oracle():
     trainer = DitTrainer(model, lr=1e-4, clip=0.0)
     opt = torch.optim.AdamW(oracle.parameters(), lr=1e-4, betas=(0.9, 0.99), eps=1e-8, weight_decay=0.01)
     model.train()
-    images, ray_o, ray_d, t = _inputs(2, 4, 32, 32)
+    images, ray_o, ray_d, t = dit_inputs(2, 4, 32, 32)
     target = {k: None for k in ("xyz", "features", "opacity")}
     g = torch.Generator(DEV).manual_seed(3)
     losses, ref_losses = [], []

@@ -19,7 +19,8 @@ import math
 import pytest
 import torch
 
-from test_dit_gpu import _inputs
+from dit_regime import dit_inputs
+from util import rel_l2 as _rel
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -84,11 +85,6 @@ CLAMP_FRAC = (0.1, 0.4)
 SATURATED_FRAC = (0.03, 0.35)
 
 
-def _rel(a, b):
-    a, b = a.detach().double(), b.detach().double()
-    return float((a - b).norm() / (b.norm() + 1e-30))
-
-
 def build(kind, layers, seed=0):
     """-> (product DGSDenoiser with a DitTrainer, fp64 DenoiserOracle on the device with the same weights)."""
     from dgs_b200.denoiser import DGSDenoiser, DGSDenoiserScene
@@ -118,7 +114,7 @@ def forward_errors(model, trainer, ref, kind, shape, seed=0, recompute=False):
     -> ({check: matched error}, {check: plain error}, {"mod_segments": [...], "clamp": frac, "saturated": frac})."""
     from oracle.dit import cond64, gaussians_epilogue64, heads64, input_stage64, mod_table64, _layernorm64
     B, V, H, W = shape
-    images, ray_o, ray_d, t = inputs = _inputs(B, V, H, W, seed=seed)
+    images, ray_o, ray_d, t = inputs = dit_inputs(B, V, H, W, seed=seed)
     trainer.recompute = recompute
     with torch.enable_grad():
         out, img_xyz = model.image_to_gaussians(*inputs)
@@ -166,7 +162,7 @@ def backward_errors(model, trainer, ref, kind, shape, seed=0, recompute=False):
     fp64 autograd through the reference fed the product's tensors at the stage boundary.  -> {check: {tensor: error}}."""
     from oracle.dit import _bf16, cond64, heads64, input_stage64, mod_table64
     B, V, H, W = shape
-    images, ray_o, ray_d, t = inputs = _inputs(B, V, H, W, seed=seed)
+    images, ray_o, ray_d, t = inputs = dit_inputs(B, V, H, W, seed=seed)
     trainer.recompute = recompute
     with torch.enable_grad():
         out, _ = model.image_to_gaussians(*inputs)
@@ -287,7 +283,7 @@ def test_inference_matches_recompute_bitwise(kind):
     """Inference and a recompute-mode training forward run the same kernels on the same inputs (the decoder's A
     operand lives in the workspace in one and in the train state in the other), so they agree to the bit."""
     model, trainer, ref = build(kind, 2)
-    inputs = _inputs(*SHAPE_B2, seed=3)
+    inputs = dit_inputs(*SHAPE_B2, seed=3)
     with torch.no_grad():
         a, a_img = model.image_to_gaussians(*inputs)
         a = {k: v.clone() for k, v in a.items()}

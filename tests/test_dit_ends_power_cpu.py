@@ -10,7 +10,8 @@
 import pytest
 import torch
 
-from test_dit_ends_gpu import (BWD, CLAMP_FRAC, FWD, OUTS, SATURATED_FRAC, _rel, apply_end_scale)
+from test_dit_ends_gpu import BWD, CLAMP_FRAC, FWD, OUTS, SATURATED_FRAC, apply_end_scale
+from util import rel_l2 as _rel
 
 D = 1024
 

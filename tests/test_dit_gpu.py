@@ -2,23 +2,15 @@
 the whole DGSDenoiser.image_to_gaussians against the fp32 PyTorch oracle (oracle/dit.py).
 Tolerance: 1e-3 relative in bf16, measured norm-wise against fp32 on the SAME
 (bf16-representable where the kernel consumes bf16) inputs; the exact bound per check is written below."""
-import ctypes as C
-
 import numpy as np
 import pytest
 import torch
 
+from dit_regime import dit_inputs
+from util import rel_l2 as rel
+
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
-
-
-def rel(a, b):
-    a, b = a.double(), b.double()
-    return float((a - b).norm() / (b.norm() + 1e-30))
-
-
-def stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 # (1, 2050, 20) / (1, 1500, 16) / (3, 4098, 16): ragged query/key tails at other head counts and batch sizes
@@ -30,7 +22,7 @@ def test_attention_vs_fp32_softmax(B, N, H):
     g = torch.Generator(DEV).manual_seed(N)
     qkv = (torch.randn(B, N, 3, H, 64, device=DEV, generator=g) * 1.5).to(torch.bfloat16)
     out = torch.zeros(B, N, H * 64, dtype=torch.bfloat16, device=DEV)
-    _lib.check(_lib.lib().dgs_attention_fwd(qkv.data_ptr(), out.data_ptr(), B, N, H, stream()))
+    _lib.check(_lib.lib().dgs_attention_fwd(qkv.data_ptr(), out.data_ptr(), B, N, H, _lib.stream(None)))
     q, k, v = [t.float().permute(0, 2, 1, 3) for t in qkv.unbind(2)]  # [B,H,N,64]
     ref = torch.softmax((q @ k.transpose(-1, -2)) * 0.125, dim=-1) @ v
     ref = ref.permute(0, 2, 1, 3).reshape(B, N, H * 64)
@@ -53,25 +45,16 @@ def test_ln_modulate():
     h = torch.empty(B, R, D, dtype=torch.bfloat16, device=DEV)
     for w_, eps in ((None, 1e-6), (lnw, 1e-5)):
         _lib.check(_lib.lib().dgs_ln_modulate(x.data_ptr(), None if w_ is None else w_.data_ptr(), mod.data_ptr(),
-                                              mod[:, D:].data_ptr(), 6 * D, h.data_ptr(), B, R, D, eps, stream()))
+                                              mod[:, D:].data_ptr(), 6 * D, h.data_ptr(), B, R, D, eps,
+                                              _lib.stream(None)))
         ln = torch.nn.functional.layer_norm(x, (D,), w_, None, eps)
         ref = ln * (1 + mod[:, None, D:2 * D]) + mod[:, None, :D]
         assert rel(h.float(), ref) < 2.5e-3
         assert rel(h.float(), ref.to(torch.bfloat16).float()) < 3e-4
 
 
-def _inputs(B, V, H, W, seed=0):
-    g = torch.Generator(DEV).manual_seed(seed)
-    images = torch.rand(B, V, 3, H, W, device=DEV, generator=g)
-    images[:, 1:] = torch.randn(B, V - 1, 3, H, W, device=DEV, generator=g)
-    ray_o = torch.randn(B, V, 3, 1, 1, device=DEV, generator=g).expand(B, V, 3, H, W).contiguous() * 1.5
-    ray_d = torch.nn.functional.normalize(torch.randn(B, V, 3, H, W, device=DEV, generator=g), dim=2)
-    t = torch.randint(0, 1000, (B,), device=DEV, generator=g)
-    return images, ray_o, ray_d, t
-
-
 def _compare_models(model, oracle, B, V, H, W, tag):
-    images, ray_o, ray_d, t = _inputs(B, V, H, W)
+    images, ray_o, ray_d, t = dit_inputs(B, V, H, W)
     with torch.no_grad():
         ref, ref_xyz, ref_tok = oracle.image_to_gaussians(images, ray_o, ray_d, t, return_tokens=True)
         out, xyz_img, tok = model.image_to_gaussians(images, ray_o, ray_d, t, return_tokens=True)
@@ -114,7 +97,7 @@ def test_denoiser_full_depth_obj256_vs_oracle():
     from dgs_b200 import synth
     c2w, fx = synth.orbit_cameras(4, 256, 256)
     c2w, fx = torch.tensor(c2w[None], device=DEV), torch.tensor(fx[None], device=DEV)
-    images, ray_o, ray_d, t = _inputs(1, 4, 256, 256)
+    images, ray_o, ray_d, t = dit_inputs(1, 4, 256, 256)
     with torch.no_grad():
         ref, _ = oracle.image_to_gaussians(images, ray_o, ray_d, t)
         out, _ = model.image_to_gaussians(images, ray_o, ray_d, t)

@@ -1,21 +1,12 @@
 """GPU tests of the DiT kernels at token counts with ragged tails (the GEMM's are in test_gemm_gpu.py): the attention
 forward with last key blocks of 1 to 98 valid keys and last query blocks that leave warpgroup 1 without a valid row."""
-import ctypes as C
-
 import pytest
 import torch
 
+from util import rel_l2 as rel
+
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
-
-
-def rel(a, b):
-    a, b = a.double(), b.double()
-    return float((a - b).norm() / (b.norm() + 1e-30))
-
-
-def stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 # the last key block holds 2, 1, 15, 64, 1, 2 and 98 valid keys; the last query block has as many rows, so its
@@ -31,8 +22,8 @@ def test_attention_tails(N):
     out_t = torch.zeros_like(out)
     Np = (N + 127) // 128 * 128
     lse = torch.full((B, H, Np), float("nan"), device=DEV)
-    _lib.check(L.dgs_attention_fwd(qkv.data_ptr(), out.data_ptr(), B, N, H, stream()))
-    _lib.check(L.dgs_attention_fwd_train(qkv.data_ptr(), out_t.data_ptr(), lse.data_ptr(), B, N, H, stream()))
+    _lib.check(L.dgs_attention_fwd(qkv.data_ptr(), out.data_ptr(), B, N, H, _lib.stream(None)))
+    _lib.check(L.dgs_attention_fwd_train(qkv.data_ptr(), out_t.data_ptr(), lse.data_ptr(), B, N, H, _lib.stream(None)))
     torch.cuda.synchronize()
     q, k, v = [t.float().permute(0, 2, 1, 3) for t in qkv.unbind(2)]
     s = (q @ k.transpose(-1, -2)) * 0.125

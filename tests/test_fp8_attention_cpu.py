@@ -10,6 +10,7 @@ from oracle.fp8 import quantize_e4m3
 from oracle.fp8_attention import (FP8_ATTENTION_DEFECTS, attention_fp8_matched, key_of_slot,
                                   quantize_attention_operands)
 from test_fp8_attention_gpu import ATT_VS_MATCHED
+from util import rel_l2 as _rel
 
 
 def _qkv(B, N, H, seed, std=1.5):
@@ -21,10 +22,6 @@ def _plain(qkv, H):
     B, N, _ = qkv.shape
     q, k, v = qkv.double().reshape(B, N, 3, H, 64).permute(2, 0, 3, 1, 4)
     return (torch.softmax(q @ k.transpose(-1, -2) / 8, -1) @ v).permute(0, 2, 1, 3).reshape(B, N, H * 64)
-
-
-def _rel(a, b):
-    return float((a.double() - b.double()).norm() / b.double().norm())
 
 
 def test_key_order_is_a_permutation_matching_the_fragments():

@@ -6,13 +6,14 @@ error as the yardstick.
 Every bound below was set from the errors measured on an H100 80GB HBM3 over seeds 0, 1, 2; the measured worst case is
 written next to it.
 """
-import gc
 import math
 
 import pytest
 import torch
 
-from test_dit_gpu import _inputs, rel, stream
+from dit_regime import dit_inputs
+from fp8_ops import _attr, _err, _models, _views, attention_fwd_fp8, block_product, quantize_attention
+from util import rel_l2 as rel
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -34,35 +35,6 @@ BLOCK_FP8_ATT = 4.5e-2
 E2E_SLACK = 1e-3  # the bf16 path's own end-to-end bound, added to 1.5 x the emulation's error
 
 
-def lib():
-    from dgs_b200 import _lib
-    return _lib.lib()
-
-
-def check(rc):
-    from dgs_b200 import _lib
-    _lib.check(rc)
-
-
-def quantize(qkv, B, N, H):
-    """dgs_attention_quantize_e4m3 -> the dict of oracle.fp8_attention.quantize_attention_operands."""
-    Nk = (N + 127) // 128 * 128
-    u8 = lambda *s: torch.empty(*s, dtype=torch.uint8, device=DEV)  # noqa: E731
-    ops = dict(q8=u8(B, N, H, 64), k8=u8(B, N, H, 64), vt8=u8(B, H, 64, Nk).fill_(0xAB),  # pads must be written
-               sq=torch.empty(B, H, N, device=DEV), sk=torch.empty(B, H, Nk // 128, device=DEV),
-               sv=torch.empty(B, H, Nk // 128, device=DEV))
-    check(lib().dgs_attention_quantize_e4m3(qkv.data_ptr(), *(ops[k].data_ptr() for k in ("q8", "k8", "vt8", "sq", "sk", "sv")),
-                                            B, N, H, stream()))
-    return ops
-
-
-def attention_fp8(ops, B, N, H):
-    out = torch.zeros(B, N, H * 64, dtype=torch.bfloat16, device=DEV)
-    check(lib().dgs_attention_fwd_fp8(*(ops[k].data_ptr() for k in ("q8", "k8", "vt8", "sq", "sk", "sv")), out.data_ptr(),
-                                      B, N, H, stream()))
-    return out
-
-
 # the shapes of tests/test_dit_gpu.py::test_attention_vs_fp32_softmax
 SHAPES = [(1, 4098, 16), (2, 1026, 16), (1, 128, 2), (1, 130, 1), (2, 77, 4), (1, 1, 1), (1, 16386, 2), (1, 2050, 20),
           (1, 1500, 16), (3, 4098, 16)]
@@ -74,7 +46,7 @@ def test_quantize_pass_bitwise(B, N, H):
     g = torch.Generator(DEV).manual_seed(N)
     qkv = (torch.randn(B, N, 3 * H * 64, device=DEV, generator=g) * 1.5).to(torch.bfloat16)
     qkv[:, :, 2 * H * 64:2 * H * 64 + 64] = 0  # head 0's V all zero: scale 1
-    got = quantize(qkv, B, N, H)
+    got = quantize_attention(qkv, B, N, H)
     ref = quantize_attention_operands(qkv, H)
     torch.cuda.synchronize()
     for k in ref:
@@ -86,8 +58,8 @@ def test_attention_fp8_vs_matched_and_fp32(B, N, H):
     from oracle.fp8_attention import attention_fp8_matched
     g = torch.Generator(DEV).manual_seed(N)
     qkv = (torch.randn(B, N, 3 * H * 64, device=DEV, generator=g) * 1.5).to(torch.bfloat16)
-    ops = quantize(qkv, B, N, H)
-    out = attention_fp8(ops, B, N, H)
+    ops = quantize_attention(qkv, B, N, H)
+    out = attention_fwd_fp8(ops, B, N, H)
     e_m = rel(out.float(), attention_fp8_matched(ops, N).float())
     q, k, v = [t.float().permute(0, 2, 1, 3) for t in qkv.reshape(B, N, 3, H, 64).unbind(2)]
     ref = (torch.softmax((q @ k.transpose(-1, -2)) * 0.125, dim=-1) @ v).permute(0, 2, 1, 3).reshape(B, N, H * 64)
@@ -95,43 +67,6 @@ def test_attention_fp8_vs_matched_and_fp32(B, N, H):
     print(f"fp8 attention B={B} N={N} H={H}: vs matched {e_m:.2e}  vs fp32 softmax {e_f:.2e}")
     assert e_m < ATT_VS_MATCHED
     assert e_f < ATT_VS_FP32
-
-
-def _block_product(blk, x, mod32, N):
-    """The "fp8_attention" block (dgs_dit_forward_fp8_ex's sequence) from the exported building blocks."""
-    from test_fp8_gpu import deq_act, gemm_fp8, ms, quantize_rows
-    B = x.shape[0]
-    M = B * N
-    L = lib()
-    m, f = mod32.data_ptr(), 4
-    out = {}
-    q1 = torch.empty(M, D, dtype=torch.uint8, device=DEV)
-    s1 = torch.zeros(D // 128, ms(M), device=DEV)
-    check(L.dgs_ln_modulate_fp8(x.data_ptr(), m, m + f * D, 6 * D, q1.data_ptr(), s1.data_ptr(), B, N, D, 1e-6, stream()))
-    out["h1q"] = deq_act(q1, s1, M).reshape(B, N, D)
-    wq = {k: quantize_rows(getattr(blk.attn if k == "qkv" else blk.mlp, k).weight.detach().float().contiguous())
-          for k in ("qkv", "fc1", "fc2")}
-    bias = {k: getattr(blk.attn if k in ("qkv", "proj") else blk.mlp, k).bias.detach().float().contiguous()
-            for k in ("qkv", "proj", "fc1", "fc2")}
-    qkv, _ = gemm_fp8(q1, s1, *wq["qkv"], M, 0, bias=bias["qkv"])
-    out["qkv"] = qkv.reshape(B, N, 3 * D)
-    attn = attention_fp8(quantize(qkv, B, N, 16), B, N, 16).reshape(M, D)
-    out["attn"] = attn.reshape(B, N, D)
-    x_mid = x.reshape(M, D).clone()
-    wp = blk.attn.proj.weight.detach().to(torch.bfloat16).contiguous()
-    check(L.dgs_gemm_bf16(attn.data_ptr(), wp.data_ptr(), bias["proj"].data_ptr(), m + f * 2 * D, x_mid.data_ptr(), M, D, D,
-                          2, D, 6 * D, N, stream()))
-    out["x_mid"] = x_mid.reshape(B, N, D).clone()
-    q2 = torch.empty(M, D, dtype=torch.uint8, device=DEV)
-    s2 = torch.zeros(D // 128, ms(M), device=DEV)
-    check(L.dgs_ln_modulate_fp8(x_mid.data_ptr(), m + f * 3 * D, m + f * 4 * D, 6 * D, q2.data_ptr(), s2.data_ptr(), B, N,
-                                D, 1e-6, stream()))
-    u8, su = gemm_fp8(q2, s2, *wq["fc1"], M, 6, bias=bias["fc1"])
-    gemm_fp8(u8, su, *wq["fc2"], M, 2, bias=bias["fc2"], gate=mod32[:, 5 * D:], x=x_mid, rows_per_sample=N,
-             gate_stride=6 * D)
-    out["x_out"] = x_mid.reshape(B, N, D)
-    torch.cuda.synchronize()
-    return out
 
 
 # N = 4098: obj-256; N = 16386: obj-512 / scene-512 / the pipline_obj.py demo (one seed: the fp64 oracle is slow there)
@@ -147,7 +82,7 @@ def test_block_fp8_attention_trained_scale(seed, N):
     g = torch.Generator(DEV).manual_seed(seed)
     x = (torch.randn(1, N, D, device=DEV, generator=g) * 1.5).contiguous()
     mod = block_modulation64(blk, conditioning64(model, torch.tensor([100 + 300 * seed], device=DEV)))
-    prod = _block_product(blk, x, mod.float().contiguous(), N)
+    prod = block_product(blk, x, mod.float().contiguous(), N, attention_fp8=True)
     xd = x.double()
     ref = dit_block_fp8_matched(blk, xd, mod, attention_fp8=True)
     e_blk = rel(prod["x_out"] - x, ref["x_out"] - xd)
@@ -156,13 +91,6 @@ def test_block_fp8_attention_trained_scale(seed, N):
     print(f"fp8-attention block N={N} seed {seed}: increment {e_blk:.2e}  x_mid increment (fed h1q) {e_att:.2e}")
     assert e_blk < BLOCK_FP8_ATT
     assert e_att < BLOCK_FP8_ATT
-
-
-def _models(layers, scene, trained, seed):
-    from test_fp8_gpu import _models as models
-    gc.collect()
-    torch.cuda.empty_cache()
-    return models(layers, scene, trained, seed)
 
 
 E2E_CASES = [(24, False, False), (24, False, True), (2, True, True)]
@@ -176,11 +104,10 @@ def _psnr(a, b):
 @pytest.mark.parametrize("layers,scene,trained", E2E_CASES)
 def test_end_to_end_fp8_attention(layers, scene, trained):
     from oracle.fp8_attention import emulate_fp8
-    from test_fp8_gpu import _attr, _err, _views
     worst = []
     for seed in (0, 1, 2):
         model, oracle = _models(layers, scene, trained, seed)
-        inputs = _inputs(1, 4, 256, 256, seed=seed)
+        inputs = dit_inputs(1, 4, 256, 256, seed=seed)
         with torch.no_grad():
             r_out, r_ia = oracle.image_to_gaussians(*inputs)
             ref = (r_out, r_ia, _views(model, _attr(r_out), 4, 256, 256))
@@ -203,7 +130,7 @@ def test_end_to_end_fp8_attention(layers, scene, trained):
 def test_bf16_and_fp8_untouched_by_an_fp8_attention_call():
     from dgs_b200.train import DitTrainer
     model, _ = _models(2, False, True, 0)
-    inputs = _inputs(1, 4, 64, 64, seed=0)
+    inputs = dit_inputs(1, 4, 64, 64, seed=0)
     outs = {}
     with torch.no_grad():
         for mode in ("bf16", "fp8", "fp8_attention", "fp8", "bf16"):

@@ -12,8 +12,8 @@ import ctypes
 import pytest
 import torch
 
-from test_dit_gpu import rel
 from test_fp8_gpu import BLOCK_FP8
+from util import rel_l2 as rel
 
 D = 1024
 

@@ -5,15 +5,16 @@ denoiser against the fp32 oracle with the emulated-FP8 oracle's own error as the
 Every bound below was set from the errors measured on an H100 80GB HBM3 over seeds 0, 1, 2; the measured worst case is
 written next to it.
 """
-import ctypes as C
-import gc
 import math
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-from test_dit_gpu import _inputs, rel, stream
+from dgs_b200 import _lib
+from dit_regime import dit_inputs
+from fp8_ops import _attr, _err, _models, _views, block_product, deq_act, deq_w, gemm_fp8, ms, quantize_rows
+from util import rel_l2 as rel
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -35,59 +36,6 @@ STAGE_FP8 = dict(qkv=1.5e-3,  # worst 7.02e-4 (bf16 output rounding of a product
                               # and the oracle's fall on either side of a rounding midpoint)
                  x_out=4e-4)  # worst 1.64e-4 (increment, fed the product's u: fc2's accumulation error only)
 E2E_SLACK = 1e-3       # the bf16 path's own end-to-end bound, added to 1.5 x the emulation's error
-
-
-def lib():
-    from dgs_b200 import _lib
-    return _lib.lib()
-
-
-def check(rc):
-    from dgs_b200 import _lib
-    _lib.check(rc)
-
-
-def ms(M):
-    return (M + 3) // 4 * 4
-
-
-def quantize_rows(x):
-    """dgs_quantize_rows_e4m3: x [R, K] fp32 -> (q uint8 [R, K], s [R])."""
-    R, K = x.shape
-    q = torch.empty(R, K, dtype=torch.uint8, device=DEV)
-    s = torch.empty(R, dtype=torch.float32, device=DEV)
-    check(lib().dgs_quantize_rows_e4m3(x.data_ptr(), R, K, q.data_ptr(), s.data_ptr(), stream()))
-    return q, s
-
-
-def deq_act(q, sa, M):
-    """e4m3 [M, K] with group scales [K/128][ms(M)] -> fp64 [M, K]"""
-    K = q.shape[1]
-    return (q.view(torch.float8_e4m3fn).double().reshape(M, K // 128, 128) *
-            sa[:, :M].t().double()[:, :, None]).reshape(M, K)
-
-
-def deq_w(q, s):
-    return q.view(torch.float8_e4m3fn).double() * s.double()[:, None]
-
-
-def gemm_fp8(A, sa, Wq, sw, M, epi, bias=None, gate=None, x=None, rows_per_sample=1, gate_stride=0):
-    N, K = Wq.shape
-    out_scale = None
-    if epi == 0:
-        out = torch.empty(M, N, dtype=torch.bfloat16, device=DEV)
-    elif epi == 2:
-        out = x
-    elif epi == 3:
-        out = torch.empty(M, N, dtype=torch.float32, device=DEV)
-    else:
-        out = torch.empty(M, N, dtype=torch.uint8, device=DEV)
-        out_scale = torch.full((N // 128, ms(M)), float("nan"), device=DEV)
-    check(lib().dgs_gemm_fp8(A.data_ptr(), sa.data_ptr(), Wq.data_ptr(), sw.data_ptr(),
-                             None if bias is None else bias.data_ptr(), None if gate is None else gate.data_ptr(),
-                             out.data_ptr(), None if out_scale is None else out_scale.data_ptr(), M, N, K, epi, N,
-                             gate_stride, rows_per_sample, stream()))
-    return out, out_scale
 
 
 def act_operand(M, K, g):
@@ -134,8 +82,8 @@ def test_ln_modulate_fp8(seed):
     M = B * rows
     q = torch.empty(M, D, dtype=torch.uint8, device=DEV)
     sa = torch.zeros(D // 128, ms(M), device=DEV)
-    check(lib().dgs_ln_modulate_fp8(x.data_ptr(), mod.data_ptr(), mod.data_ptr() + 4 * D, 6 * D, q.data_ptr(),
-                                    sa.data_ptr(), B, rows, D, 1e-6, stream()))
+    _lib.check(_lib.lib().dgs_ln_modulate_fp8(x.data_ptr(), mod.data_ptr(), mod.data_ptr() + 4 * D, 6 * D,
+                                              q.data_ptr(), sa.data_ptr(), B, rows, D, 1e-6, _lib.stream(None)))
     xd = x.double()
     ref = (F.layer_norm(xd, (D,), eps=1e-6) * (1 + mod[:, None, D:2 * D].double()) + mod[:, None, :D].double()).reshape(M, D)
     deq = deq_act(q, sa, M)
@@ -210,45 +158,6 @@ def test_gemm_fp8_epilogues(M, N, K):
 
 
 # ------------------------------------------------------------------ 3. one block from the building blocks
-def _block_product(blk, x, mod32, N):
-    """The FP8 block (dgs_dit_forward_fp8's sequence) from the exported building blocks; -> every intermediate."""
-    B = x.shape[0]
-    M = B * N
-    L = lib()
-    m = mod32.data_ptr()
-    f = 4  # bytes per float
-    out = {}
-    q1 = torch.empty(M, D, dtype=torch.uint8, device=DEV)
-    s1 = torch.zeros(D // 128, ms(M), device=DEV)
-    check(L.dgs_ln_modulate_fp8(x.data_ptr(), m, m + f * D, 6 * D, q1.data_ptr(), s1.data_ptr(), B, N, D, 1e-6, stream()))
-    out["h1q"] = deq_act(q1, s1, M).reshape(B, N, D)
-    wq = {k: quantize_rows(getattr(blk.attn if k in ("qkv", "proj") else blk.mlp, k).weight.detach().float().contiguous())
-          for k in ("qkv", "fc1", "fc2")}
-    bias = {k: getattr(blk.attn if k in ("qkv", "proj") else blk.mlp, k).bias.detach().float().contiguous()
-            for k in ("qkv", "proj", "fc1", "fc2")}
-    qkv, _ = gemm_fp8(q1, s1, *wq["qkv"], M, 0, bias=bias["qkv"])
-    out["qkv"] = qkv.reshape(B, N, 3 * D)
-    attn = torch.empty(M, D, dtype=torch.bfloat16, device=DEV)
-    check(L.dgs_attention_fwd(qkv.data_ptr(), attn.data_ptr(), B, N, 16, stream()))
-    x_mid = x.reshape(M, D).clone()
-    wp = blk.attn.proj.weight.detach().to(torch.bfloat16).contiguous()
-    check(L.dgs_gemm_bf16(attn.data_ptr(), wp.data_ptr(), bias["proj"].data_ptr(), m + f * 2 * D, x_mid.data_ptr(), M, D, D,
-                          2, D, 6 * D, N, stream()))
-    out["x_mid"] = x_mid.reshape(B, N, D).clone()
-    q2 = torch.empty(M, D, dtype=torch.uint8, device=DEV)
-    s2 = torch.zeros(D // 128, ms(M), device=DEV)
-    check(L.dgs_ln_modulate_fp8(x_mid.data_ptr(), m + f * 3 * D, m + f * 4 * D, 6 * D, q2.data_ptr(), s2.data_ptr(), B, N,
-                                D, 1e-6, stream()))
-    out["h2q"] = deq_act(q2, s2, M).reshape(B, N, D)
-    u8, su = gemm_fp8(q2, s2, *wq["fc1"], M, 6, bias=bias["fc1"])
-    out["uq"] = deq_act(u8, su, M).reshape(B, N, 4 * D)
-    gemm_fp8(u8, su, *wq["fc2"], M, 2, bias=bias["fc2"], gate=mod32[:, 5 * D:], x=x_mid, rows_per_sample=N,
-             gate_stride=6 * D)
-    out["x_out"] = x_mid.reshape(B, N, D)
-    torch.cuda.synchronize()
-    return out
-
-
 @pytest.mark.parametrize("seed", [0, 1, 2])
 def test_block_fp8_trained_scale(seed):
     from dgs_b200.denoiser import DGSDenoiser
@@ -263,7 +172,7 @@ def test_block_fp8_trained_scale(seed):
     x = (torch.randn(B, N, D, device=DEV, generator=g) * 1.5).contiguous()
     t = torch.tensor([100 + 300 * seed], device=DEV)
     mod = block_modulation64(blk, conditioning64(model, t))
-    prod = _block_product(blk, x, mod.float().contiguous(), N)
+    prod = block_product(blk, x, mod.float().contiguous(), N)
     xd = x.double()
     ref = dit_block_fp8_matched(blk, xd, mod)
     e_blk = rel(prod["x_out"] - x, ref["x_out"] - xd)
@@ -277,39 +186,6 @@ def test_block_fp8_trained_scale(seed):
 
 
 # ------------------------------------------------------------------ 4.-6. end to end, bf16 untouched, sampler
-def _models(layers, scene, trained, seed):
-    from dgs_b200.denoiser import DGSDenoiser, DGSDenoiserScene
-    from dit_regime import apply_trained_scale
-    from oracle.dit import DenoiserOracle
-    gc.collect()
-    torch.cuda.empty_cache()
-    torch.manual_seed(seed)
-    cfg = dict(patch_size=8, num_layers=layers, ray_pe_type="plk" if scene else "relative_plk")
-    model = (DGSDenoiserScene if scene else DGSDenoiser)(cfg)
-    if trained:
-        apply_trained_scale(model, seed)
-    model = model.to(DEV).eval()
-    oracle = DenoiserOracle(layers=layers, scene=scene).to(DEV)
-    oracle.load_state_dict(model.state_dict(), strict=True)
-    return model, oracle
-
-
-def _views(model, out, V, H, W):
-    from dgs_b200 import synth
-    c2w, fx = synth.orbit_cameras(V, W, H)
-    return model.render_gaussians(out, torch.tensor(c2w[None], device=DEV), torch.tensor(fx[None], device=DEV), H, W)
-
-
-def _attr(d):
-    from dgs_b200.denoiser import AttrDict
-    return AttrDict(d)
-
-
-def _err(out, ia, views, ref):
-    r_out, r_ia, r_views = ref
-    return max([rel(out[k], r_out[k]) for k in r_out] + [rel(ia, r_ia), rel(views, r_views)])
-
-
 E2E_CASES = [(24, False, False), (24, False, True), (2, True, True)]
 
 
@@ -319,7 +195,7 @@ def test_end_to_end_fp8(layers, scene, trained):
     worst = []
     for seed in (0, 1, 2):
         model, oracle = _models(layers, scene, trained, seed)
-        inputs = _inputs(1, 4, 256, 256, seed=seed)
+        inputs = dit_inputs(1, 4, 256, 256, seed=seed)
         with torch.no_grad():
             r_out, r_ia = oracle.image_to_gaussians(*inputs)
             ref = (r_out, r_ia, _views(model, _attr(r_out), 4, 256, 256))
@@ -347,7 +223,7 @@ def test_end_to_end_fp8(layers, scene, trained):
 def test_bf16_path_untouched_and_training_refuses_fp8():
     from dgs_b200.train import DitTrainer
     model, _ = _models(2, False, True, 0)
-    inputs = _inputs(1, 4, 64, 64, seed=0)
+    inputs = dit_inputs(1, 4, 64, 64, seed=0)
     with torch.no_grad():
         a, a_ia = model.image_to_gaussians(*inputs)
         model.set_inference_precision("fp8")
@@ -369,7 +245,7 @@ def test_bf16_path_untouched_and_training_refuses_fp8():
 def test_fp8_weights_follow_parameter_updates():
     model, _ = _models(2, False, True, 0)
     model.set_inference_precision("fp8")
-    inputs = _inputs(1, 4, 64, 64, seed=1)
+    inputs = dit_inputs(1, 4, 64, 64, seed=1)
     with torch.no_grad():
         a, _ = model.image_to_gaussians(*inputs)
         model.transformer[1].mlp.fc2.weight.mul_(1.5)

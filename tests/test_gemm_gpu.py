@@ -17,7 +17,6 @@ split-K choices, and tests/test_gemm_cpu.py checks that the table reaches every 
 Every bound below is the worst measured on an H100 80GB HBM3 (700 W) over seeds 0, 1, 2, with its margin.
 """
 import collections
-import ctypes as C
 import math
 import zlib
 
@@ -421,10 +420,6 @@ def _lib():
     return L
 
 
-def stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
 def _ptr(t):
     return None if t is None else t.data_ptr()
 
@@ -449,13 +444,13 @@ def launch(c, inp, ldc, mis):
     before = (out.bits().clone(), None if aux is None else aux.bits().clone())
     A, W = inp["A"], inp["W"]
     if c.epi == "tn":
-        L.check(lib.dgs_gemm_bf16_tn(_ptr(A), _ptr(W), out.ptr(), M, N, K, A.shape[1], W.shape[1], ldc, stream()))
+        L.check(lib.dgs_gemm_bf16_tn(_ptr(A), _ptr(W), out.ptr(), M, N, K, A.shape[1], W.shape[1], ldc, L.stream(None)))
     else:
         gate = inp.get("gate")
         lda = A.shape[1] if c.kpad else 0
         L.check(lib.dgs_gemm_bf16_ex(_ptr(A), _ptr(W), _ptr(inp["bias"]), None if gate is None else gate[:, N:].data_ptr(),
                                      out.ptr(), None if aux is None else aux.ptr(), _ptr(resid), M, N, K, lda, lda, c.epi,
-                                     ldc, 0 if gate is None else gate.stride(0), c.rps, stream()))
+                                     ldc, 0 if gate is None else gate.stride(0), c.rps, L.stream(None)))
     return out, aux, resid, before
 
 
@@ -562,7 +557,7 @@ def test_cast_transpose_f32(M, Cc, layers, with_rm):
     tr = torch.full((n + 2 * PRE,), SENT16, dtype=torch.int16, device=DEV)
     L.check(L.lib().dgs_cast_transpose_f32(arena.data_ptr(), stride, layers, M, Cc,
                                            rm.data_ptr() + 2 * PRE if with_rm else None, tr.data_ptr() + 2 * PRE,
-                                           stream()))
+                                           L.stream(None)))
     torch.cuda.synchronize()
     ref = mats.to(torch.bfloat16)
     assert torch.equal(tr[PRE:PRE + n].view(torch.bfloat16).view(layers, Cc, M), ref.transpose(1, 2))

@@ -10,14 +10,10 @@ import torch
 
 from dgs_b200 import _lib
 from oracle.geometry_loss import geometry_grad64, geometry_losses64
+from util import rel_l2 as rel
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CASES = ("tc3", "tc4", "ragged", "edge")
-
-
-def rel(a, b):
-    a, b = torch.as_tensor(a).double(), torch.as_tensor(b).double()
-    return float((a - b).norm() / (b.norm() + 1e-300))
 
 
 def fixture_case(z, name):

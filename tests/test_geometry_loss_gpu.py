@@ -8,6 +8,8 @@ import numpy as np
 import pytest
 import torch
 
+from util import rel_l2 as rel
+
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -15,11 +17,6 @@ G_XYZ = 0.025
 # diffusionGS_rel.yaml's loss block, lambda_lpips set to 0 (no LPIPS checkpoint here)
 REL_LAMBDAS = dict(lambda_diffusion=[150, 0.0, 1.0, 151], lambda_lpips=0.0, lambda_ssim=0.0,
                    lambda_pointsdist=[150, 1.0, 0.0, 151], lambda_xyz=[150, 0.0, 0.025, 151], lambda_depth=0.0)
-
-
-def rel(a, b):
-    a, b = a.detach().double(), b.detach().double()
-    return float((a - b).norm() / (b.norm() + 1e-300))
 
 
 def kernel_run(x, o, gt, m, g_pd, g_xyz):
@@ -145,9 +142,9 @@ def test_dit_backward_folds_d_img_exactly(kind, recompute):
     float atomics, whose order varies from run to run, so the claim is made per parameter tensor: every tensor the
     (d_xyz + scatter, NULL) call reproduces bit for bit on a second run (the GEMM weight gradients among them) must come
     out bit for bit, and the whole arena within that call's run-to-run spread."""
-    from test_dit_gpu import _inputs
+    from dit_regime import dit_inputs
     model, trainer = build(kind, 2, recompute)
-    inputs = _inputs(2, 4, 32, 48)
+    inputs = dit_inputs(2, 4, 32, 48)
     B, V, _, H, W = inputs[0].shape
     G, p = model.cfg.n_gaussians, model.cfg.patch_size
     P = G + V * H * W
@@ -181,11 +178,11 @@ def test_geometry_terms_through_the_model_vs_oracle_autograd():
     from dgs_b200.geometry_loss import geometry_losses
     from oracle.dit import DenoiserOracle
     from oracle.geometry_loss import geometry_losses64
-    from test_dit_gpu import _inputs
+    from dit_regime import dit_inputs
     model, trainer = build("obj-rel", 4, True)
     oracle = DenoiserOracle(layers=4).to(DEV)
     oracle.load_state_dict(model.state_dict(), strict=True)
-    images, ray_o, ray_d, t = _inputs(1, 4, 64, 64)
+    images, ray_o, ray_d, t = dit_inputs(1, 4, 64, 64)
     gen = torch.Generator(DEV).manual_seed(9)
     gt = ray_o + ray_d * (2.7 + 0.3 * torch.rand(1, 4, 1, 64, 64, device=DEV, generator=gen))
     m = (torch.rand(1, 4, 1, 64, 64, device=DEV, generator=gen) > 0.4).float()
@@ -206,10 +203,10 @@ def test_geometry_terms_through_the_model_vs_oracle_autograd():
 
 def _recipe_setup():
     from dgs_b200 import synth
-    from test_dit_gpu import _inputs
+    from dit_regime import dit_inputs
     model, trainer = build("obj-rel", 2, True)
     B, V, H, W = 2, 4, 64, 64
-    images, ray_o, ray_d, t = _inputs(B, V, H, W)
+    images, ray_o, ray_d, t = dit_inputs(B, V, H, W)
     c2w, fx = synth.orbit_cameras(V, W, H)
     c2w = torch.tensor(c2w[None], device=DEV).expand(B, -1, -1, -1).contiguous()
     fx = torch.tensor(fx[None], device=DEV).expand(B, -1, -1).contiguous()

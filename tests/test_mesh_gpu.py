@@ -9,6 +9,7 @@ import torch
 
 from mesh_shapes import closed_and_oriented
 from oracle import mesh as om
+from util import rel_l2 as _rel
 
 pytestmark = pytest.mark.gpu
 
@@ -25,10 +26,6 @@ FIELD_TOL, REF_TOL = 2e-6, 3e-6
 def _field(t, R, nb, rr=1.5, smod=None):
     from dgs_b200 import mesh
     return mesh.opacity_field(*t, scaling_modifier=smod, resolution=R, num_blocks=nb, relax_ratio=rr, return_counts=True)
-
-
-def _rel(a, b):
-    return float((a.double() - b.double()).norm() / b.double().norm())
 
 
 def _shell(P, seed, dist="trained"):

@@ -19,16 +19,12 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 import make_dit_golden as mdg  # noqa: E402
 import ref_import as ri  # noqa: E402
+from util import rel_l2 as rel  # noqa: E402
 
 from oracle.dit import DenoiserOracle  # noqa: E402
 
 SMALL = [n for n in ri.DIT_CASES if n.startswith("s_")]
 WIDE = [n for n in ri.DIT_CASES if n.startswith("w1024_")]
-
-
-def rel(a, b):
-    a, b = a.detach().double(), b.detach().double()
-    return float(((a - b).norm() / (b.norm() + 1e-30)).detach())
 
 
 def _oracle_for(name):

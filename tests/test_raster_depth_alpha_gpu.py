@@ -12,7 +12,7 @@ import pytest
 import torch
 
 from test_raster_gpu import DEV, TOL, T, _batch_inputs
-from util import rel_l2
+from util import rel_l2 as _rel
 
 pytestmark = pytest.mark.gpu
 NAMES = ("xyz", "features", "scaling", "rotation", "opacity")
@@ -21,10 +21,6 @@ NAMES = ("xyz", "features", "scaling", "rotation", "opacity")
 class Cfg:
     gaussians_sh_degree = 0
     use_gssplat = False
-
-
-def _rel(a, b):
-    return rel_l2(a.detach().cpu().numpy(), b.detach().cpu().numpy())
 
 
 def _upstream(B, V, H, W, seed):

@@ -21,14 +21,10 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 import make_renderer_golden as mg  # noqa: E402
+from util import rel_l2 as rel  # noqa: E402
 
 NAMES = mg.NAMES
 TOL = 1e-4
-
-
-def rel(a, b):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    return float(np.linalg.norm(a - b) / (np.linalg.norm(b) + 1e-30))
 
 
 def fixture(case):

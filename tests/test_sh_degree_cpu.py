@@ -1,5 +1,5 @@
 """The denoiser at gaussians_sh_degree 0..3 without a GPU: the module tree against the reference's, the configuration
-checks of the Python modules and of the C ABI, the degree-aware oracle (tests/dit_sh_oracle.py) against outputs of the
+checks of the Python modules and of the C ABI, the degree-aware oracle (oracle/dit.py) against outputs of the
 reference's own code (tests/golden/make_dit_sh_golden.py), and the degree-3 Gaussians through prepare_to_save and the
 PLY files."""
 import ctypes as C
@@ -13,19 +13,14 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 sys.path.insert(0, os.path.join(HERE, "golden"))
-import dit_sh_oracle as so  # noqa: E402
 import make_dit_sh_golden as msg  # noqa: E402
 import ref_import as ri  # noqa: E402
+from util import rel_l2 as rel  # noqa: E402
 
 from oracle import dit as od  # noqa: E402
 
 SMALL = [n for n in msg.DIT_SH_CASES if n.startswith("s_")]
 WIDE = [n for n in msg.DIT_SH_CASES if n.startswith("w1024_")]
-
-
-def rel(a, b):
-    a, b = a.detach().double(), b.detach().double()
-    return float((a - b).norm() / (b.norm() + 1e-30))
 
 
 def _model(scene, **cfg):
@@ -42,7 +37,7 @@ def test_state_dict_keys_and_shapes_equal_reference(scene, degree):
     assert list(sd) == [str(k) for k in z[pre + "keys"]]
     for k, v in sd.items():
         assert tuple(v.shape) == tuple(z[pre + "shape/" + k]), k
-    C_ = so.head_channels(degree)
+    C_ = od.head_channels(degree)
     assert tuple(sd["upsampler.linear.weight"].shape) == (C_, 64)
     assert tuple(sd["image_token_decoder.linear.weight"].shape) == (64 * C_, 64)
 
@@ -92,7 +87,7 @@ def test_c_abi_sh_degree_field_and_checks():
     assert sizes[0] == L.dgs_dit_workspace_bytes(C.byref(_abi_weights()), 1, 4, 64, 64) > 0
     T = 4 * 8 * 8
     for d in range(1, 4):  # gs_tok [B*G, C] and img_gs [B*T, 64 C], fp32, up to the carver's alignment
-        extra = (2 * (so.head_channels(d) - 14) + T * 64 * (so.head_channels(d) - 14)) * 4
+        extra = (2 * (od.head_channels(d) - 14) + T * 64 * (od.head_channels(d) - 14)) * 4
         assert extra - 256 <= sizes[d] - sizes[0] <= extra + 256, d
     for bad in (dict(sh_degree=4), dict(sh_degree=-1)):
         assert L.dgs_dit_workspace_bytes(C.byref(_abi_weights(**bad)), 1, 4, 64, 64) == 0
@@ -106,7 +101,7 @@ def test_c_abi_sh_degree_field_and_checks():
 
 def _oracle_for(name):
     scene, pe, cfg, _, seed = msg.DIT_SH_CASES[name]
-    o = so.DenoiserOracle(width=cfg["width"], heads=cfg["width"] // cfg["dim_heads"], layers=cfg["num_layers"],
+    o = od.DenoiserOracle(width=cfg["width"], heads=cfg["width"] // cfg["dim_heads"], layers=cfg["num_layers"],
                           patch=cfg["patch_size"], scene=scene, ray_pe_type=pe, sh_degree=cfg["gaussians_sh_degree"])
     z = np.load(os.path.join(HERE, "golden", f"dit_ref_{name}.npz"))
     keys = [str(k) for k in z["keys"]]
@@ -165,34 +160,16 @@ def test_oracle_equals_reference_code_directly():
         assert rel(g, grads[k]) < 2e-5, k
 
 
-def test_degree0_helpers_are_the_oracle_ones():
-    """At degree 0 the degree-aware epilogue is oracle/dit.py's, bit for bit, forward and backward."""
-    g = torch.Generator().manual_seed(0)
-    b, v, h, w, p, G = 2, 2, 16, 16, 8, 2
-    ro = torch.randn(b, v, 3, 1, 1, generator=g).expand(b, v, 3, h, w).double()
-    rd = torch.nn.functional.normalize(torch.randn(b, v, 3, h, w, generator=g), dim=2).double()
-    gs = torch.randn(b, G, 14, generator=g, dtype=torch.float64, requires_grad=True)
-    ig = torch.randn(b, v * (h // p) * (w // p), p * p * 14, generator=g, dtype=torch.float64, requires_grad=True)
-    for mode in (0, 1, 2):
-        a = od.gaussians_epilogue64(gs, ig, ro, rd, mode)
-        c = so.gaussians_epilogue64(gs, ig, ro, rd, mode, 0)
-        for k in a:
-            assert torch.equal(a[k], c[k]), (mode, k)
-        la = sum(a[k].sum() * (i + 1) for i, k in enumerate(ri.GS_KEYS))
-        lc = sum(c[k].sum() * (i + 1) for i, k in enumerate(ri.GS_KEYS))
-        assert all(torch.equal(x, y) for x, y in zip(torch.autograd.grad(la, [gs, ig]), torch.autograd.grad(lc, [gs, ig])))
-
-
 def test_features_are_coefficient_major_copies():
     """feature (k, c) of a Gaussian is raw channel 3 + 3k + c, for free and image tokens, at every degree."""
     b, v, h, w, p, G = 1, 1, 8, 8, 8, 2
     ro = torch.zeros(b, v, 3, h, w, dtype=torch.float64)
     rd = torch.ones(b, v, 3, h, w, dtype=torch.float64)
     for d in range(4):
-        C_ = so.head_channels(d)
+        C_ = od.head_channels(d)
         gs = torch.arange(b * G * C_, dtype=torch.float64).reshape(b, G, C_)
         ig = 1000 + torch.arange(b * p * p * C_, dtype=torch.float64).reshape(b, 1, p * p * C_)
-        f = so.gaussians_epilogue64(gs, ig, ro, rd, 0, d)["features"]
+        f = od.gaussians_epilogue64(gs, ig, ro, rd, 0)["features"]
         raw = torch.cat([gs, ig.reshape(b, -1, C_)], dim=1)
         for k in range((d + 1) ** 2):
             for c in range(3):

@@ -1,19 +1,20 @@
 """The DiT's Gaussian heads at gaussians_sh_degree 1..3 on the device, forward and backward: the epilogue kernels
-teacher-forced against tests/dit_sh_oracle.py's fp64 epilogue, the GEMM at the decoder head's shapes against torch,
+teacher-forced against oracle/dit.py's fp64 epilogue, the GEMM at the decoder head's shapes against torch,
 the whole denoiser against the degree-aware fp32 oracle (outputs, renders, parameter gradients in both train modes),
 a training step through the rasterizer's SH backward, and the FP8 inference path at degree 3.
 
 Bounds: those of the degree-0 tests the same checks copy (tests/test_dit_gpu.py, test_dit_bwd_gpu.py,
 test_dit_ends_gpu.py, test_fp8_gpu.py) unless a comment says otherwise; each run prints what it measured."""
-import ctypes as C
 import gc
 import math
 
 import pytest
 import torch
 
-import dit_sh_oracle as so
-from test_dit_gpu import _inputs
+from dgs_b200 import _lib
+from dit_regime import dit_inputs, oracle_like
+from oracle.dit import gaussians_epilogue64, head_channels
+from util import rel_l2 as rel
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -21,15 +22,6 @@ OUTS = ("xyz", "features", "scaling", "rotation", "opacity")
 # raw channel std of the epilogue inputs, as test_dit_ends_gpu's end-stage regime: the depth sigmoid saturates for part
 # of the pixels and about a quarter of the scaling channels hit the clamp
 XYZ_STD, SCALING_STD = 4.8, 1.6
-
-
-def rel(a, b):
-    a, b = a.detach().double(), b.detach().double()
-    return float((a - b).norm() / (b.norm() + 1e-30))
-
-
-def stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _raw(n_rows, C_, g):
@@ -45,9 +37,8 @@ EPI_SHAPES = [(1, 3, 1, 16, 16), (3, 1, 2, 16, 24), (2, 2, 3, 8, 16)]
 
 @pytest.mark.parametrize("degree", [1, 2, 3])
 def test_epilogue_teacher_forced(degree):
-    from dgs_b200 import _lib
     L = _lib.lib()
-    C_, M = so.head_channels(degree), (degree + 1) ** 2
+    C_, M = head_channels(degree), (degree + 1) ** 2
     p = 8
     for si, (B, G, V, H, W) in enumerate(EPI_SHAPES):
         for mode in (0, 1, 2):
@@ -64,9 +55,9 @@ def test_epilogue_teacher_forced(degree):
             ia = torch.full((B, V, 3, H, W), float("nan"), device=DEV)
             _lib.check(L.dgs_gaussians_epilogue(gs.data_ptr(), ig.data_ptr(), ro.data_ptr(), rd.data_ptr(),
                                                 *(out[k].data_ptr() for k in OUTS), ia.data_ptr(), B, G, V, H, W, p,
-                                                degree, mode, near, far, stream()))
+                                                degree, mode, near, far, _lib.stream(None)))
             gs64, ig64 = gs.double().requires_grad_(), ig.double().requires_grad_()
-            ref = so.gaussians_epilogue64(gs64, ig64, ro, rd, mode, degree, near, far)
+            ref = gaussians_epilogue64(gs64, ig64, ro, rd, mode, near, far)
             raw = torch.cat([gs, ig.reshape(B, -1, C_)], dim=1)
             # the features are copies of raw channels 3 + 3k + c: bit-exact
             assert torch.equal(out["features"], raw[..., 3:C_ - 8].reshape(B, P, M, 3)), (degree, si, mode)
@@ -86,7 +77,7 @@ def test_epilogue_teacher_forced(degree):
             _lib.check(L.dgs_gaussians_epilogue_bwd(gs.data_ptr(), ig.data_ptr(), rd.data_ptr(),
                                                     *(cot[k].data_ptr() for k in OUTS), d_gs.data_ptr(),
                                                     d_img.data_ptr(), B, G, V, H, W, p, degree, mode, near, far,
-                                                    stream()))
+                                                    _lib.stream(None)))
             r_gs, r_img = torch.autograd.grad(sum((ref[k] * cot[k].double()).sum() for k in OUTS), [gs64, ig64])
             # free tokens: every channel's gradient is a copy (or a masked copy) of an output gradient
             assert torch.equal(d_gs.double(), r_gs.reshape(B * G, C_)), (degree, si, mode)
@@ -113,23 +104,23 @@ def test_gemm_at_decoder_head_shapes(Ndec):
     """The decoder head's three GEMMs at obj-256 (Mt = 4096 image tokens, K = 3 * 1024 split-bf16): the forward
     Mt x Ndec x 3w with the fp32 epilogue (Ndec = 64 C: a 64-column N tail for odd C), the dgrad Mt x w x Ndec (bf16
     out) and the weight gradient Ndec x w over the Mt tokens (TN, the hi third of the [hi|lo|hi] operand)."""
-    from dgs_b200 import _lib
     L = _lib.lib()
     Mt, D = 4096, 1024
     A, Wd = _gemm_operands(Mt, Ndec, 3 * D, Ndec)
     out = torch.full((Mt, Ndec), float("nan"), device=DEV)
     _lib.check(L.dgs_gemm_bf16(A.data_ptr(), Wd.data_ptr(), None, None, out.data_ptr(), Mt, Ndec, 3 * D, 3, Ndec, 0, 0,
-                               stream()))
+                               _lib.stream(None)))
     e_fwd = rel(out, A.float() @ Wd.float().t())
     dimg, WdT = _gemm_operands(Mt, D, Ndec, Ndec + 1)
     dh = torch.empty(Mt, D, dtype=torch.bfloat16, device=DEV)
     _lib.check(L.dgs_gemm_bf16(dimg.data_ptr(), WdT.data_ptr(), None, None, dh.data_ptr(), Mt, D, Ndec, 0, D, 0, 0,
-                               stream()))
+                               _lib.stream(None)))
     ref_dh = dimg.float() @ WdT.float().t()
     e_dgrad = rel(dh.float(), ref_dh.to(torch.bfloat16).float())
     d_img = torch.randn(Mt, Ndec, device=DEV, generator=torch.Generator(DEV).manual_seed(Ndec + 2)).to(torch.bfloat16)
     dw = torch.full((Ndec, D), float("nan"), device=DEV)
-    _lib.check(L.dgs_gemm_bf16_tn(d_img.data_ptr(), A.data_ptr(), dw.data_ptr(), Ndec, D, Mt, Ndec, 3 * D, D, stream()))
+    _lib.check(L.dgs_gemm_bf16_tn(d_img.data_ptr(), A.data_ptr(), dw.data_ptr(), Ndec, D, Mt, Ndec, 3 * D, D,
+                                  _lib.stream(None)))
     torch.cuda.synchronize()
     e_wgrad = rel(dw, d_img.float().t() @ A[:, :D].float())
     print(f"decoder GEMMs Ndec={Ndec}: fwd {e_fwd:.2e}  dgrad (vs bf16 of fp32) {e_dgrad:.2e}  wgrad {e_wgrad:.2e}")
@@ -147,11 +138,11 @@ def _pair(degree, scene=False, layers=2, seed=0):
     cfg = dict(patch_size=8, num_layers=layers, ray_pe_type="plk" if scene else "relative_plk",
                gaussians_sh_degree=degree)
     model = (DGSDenoiserScene if scene else DGSDenoiser)(cfg).to(DEV)
-    return model, so.oracle_like(model)
+    return model, oracle_like(model)
 
 
 def _compare(model, oracle, shape, tag, seed=0):
-    images, ray_o, ray_d, t = _inputs(*shape, seed=seed)
+    images, ray_o, ray_d, t = dit_inputs(*shape, seed=seed)
     with torch.no_grad():
         ref, ref_ia = oracle.image_to_gaussians(images, ray_o, ray_d, t)
         out, ia = model.image_to_gaussians(images, ray_o, ray_d, t)
@@ -201,7 +192,7 @@ def _grad_compare(degree, recompute, shape=(2, 4, 32, 32), scene=False, seed=0):
     trainer = DitTrainer(model)
     trainer.recompute = recompute
     model.train()
-    images, ray_o, ray_d, t = _inputs(*shape)
+    images, ray_o, ray_d, t = dit_inputs(*shape)
     g = torch.Generator(DEV).manual_seed(11)
     out, _ = model.image_to_gaussians(images, ray_o, ray_d, t)
     wts = {k: torch.randn(out[k].shape, device=DEV, generator=g) for k in OUTS}
@@ -244,7 +235,7 @@ def test_training_step_through_renderer_sh_backward():
     opt = torch.optim.AdamW(oracle.parameters(), lr=1e-4, betas=(0.9, 0.99), eps=1e-8, weight_decay=0.01)
     model.train()
     B, V, H, W = 2, 4, 32, 32
-    images, ray_o, ray_d, t = _inputs(B, V, H, W)
+    images, ray_o, ray_d, t = dit_inputs(B, V, H, W)
     c2w, fx = synth.orbit_cameras(V, W, H)
     c2w = torch.tensor(c2w[None], device=DEV).expand(B, -1, -1, -1).contiguous()
     fx = torch.tensor(fx[None], device=DEV).expand(B, -1, -1).contiguous()
@@ -284,7 +275,7 @@ def test_fp8_inference_at_degree3():
     from test_fp8_gpu import E2E_SLACK
     model, oracle = _pair(3, layers=24)
     model.eval()
-    inputs = _inputs(1, 4, 256, 256)
+    inputs = dit_inputs(1, 4, 256, 256)
     with torch.no_grad():
         r_out, r_ia = oracle.image_to_gaussians(*inputs)
         e_out, e_ia = emulate_fp8(oracle).image_to_gaussians(*inputs)

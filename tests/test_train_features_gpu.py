@@ -6,19 +6,16 @@ import numpy as np
 import pytest
 import torch
 
+from util import rel_l2 as rel
+
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
-
-
-def rel(a, b):
-    a, b = a.detach().double(), b.detach().double()
-    return float((a - b).norm() / (b.norm() + 1e-30))
 
 
 def _model_and_inputs(layers=2, B=2, V=4, H=32, W=32, scene=False, **trainer_kw):
     from dgs_b200.denoiser import DGSDenoiser, DGSDenoiserScene
     from dgs_b200.train import DitTrainer
-    from test_dit_gpu import _inputs
+    from dit_regime import dit_inputs
     torch.manual_seed(0)
     cfg = dict(patch_size=8, num_layers=layers, ray_pe_type="plk" if scene else "relative_plk")
     model = (DGSDenoiserScene if scene else DGSDenoiser)(cfg).to(DEV)
@@ -30,7 +27,7 @@ def _model_and_inputs(layers=2, B=2, V=4, H=32, W=32, scene=False, **trainer_kw)
                 p.copy_(0.05 * torch.randn(p.shape, device=DEV, generator=g))
     trainer = DitTrainer(model, **trainer_kw)
     model.train()
-    return model, trainer, _inputs(B, V, H, W)
+    return model, trainer, dit_inputs(B, V, H, W)
 
 
 def _backward_once(model, trainer, inputs, seed=11):

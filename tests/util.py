@@ -1,5 +1,6 @@
 """Shared helpers of the parity tests: seeded scenes and error metrics."""
 import numpy as np
+import torch
 
 from dgs_b200 import synth
 
@@ -26,6 +27,11 @@ def oracle_forward(sc, sh=None, degree=0, colors=None, cov3d=None, bg=(1.0, 1.0,
 
 
 def rel_l2(a, b):
+    """||a - b|| / (||b|| + 1e-30) in float64: in torch on a's device when either is a tensor, else in numpy."""
+    if isinstance(a, torch.Tensor) or isinstance(b, torch.Tensor):
+        a = torch.as_tensor(a).detach().double()
+        b = torch.as_tensor(b).detach().to(a.device, torch.float64)
+        return float((a - b).norm() / (b.norm() + 1e-30))
     a = np.asarray(a, np.float64).ravel()
     b = np.asarray(b, np.float64).ravel()
     return float(np.linalg.norm(a - b) / (np.linalg.norm(b) + 1e-30))
