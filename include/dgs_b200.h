@@ -758,6 +758,35 @@ int dgs_mesh_remesh(const float* vertices, long long num_vertices, const int* fa
 int dgs_mesh_closest_points(const float* vertices, long long num_vertices, const int* faces, long long num_faces,
                             const double* queries, long long num_queries, double* out_points, double* out_d2,
                             int* out_faces, dgs_alloc_fn alloc, void* alloc_user, void* stream);
+/* Per-vertex normals and colours of a mesh extracted from Gaussians (GaussianModel.extract_mesh(vertex_colors=True)).
+ * The Gaussians and the field parameters are dgs_mesh_field's (the same records and per-block lists), plus features
+ * (device fp32 [P, (sh_degree + 1)^2, 3], the SH coefficients) and sh_degree in [0, 3]; vertices (device fp32 [V, 3],
+ * in the field's normalised frame, as extract_mesh returns them) and faces (device int32 [F, 3], every index in [0, V);
+ * checked on the device, a bad face is DGS_ERR_INVALID_ARGUMENT naming it; a repeated index is legal).  P = 0 and
+ * F = 0 are legal.  Per vertex v:
+ *   1. normal n_v: the sum of (b - a) x (c - a) over the faces incident to v, in fp64, in face order (a face counted
+ *      once per corner at v), over its length, rounded to fp32; (0, 0, 0) without faces or for a zero sum.  Marching
+ *      cubes orients faces from inside to outside, so n_v points out;
+ *   2. block: on each axis the largest grid index i with lin[i] <= p, clamped to [0, resolution - 1] (0 below -1 and
+ *      for NaN), over resolution / num_blocks.  v is evaluated against that block's Gaussian list, the one
+ *      dgs_mesh_field sums for the block's grid points, in its Gaussian order;
+ *   3. colour: w_i = opacity_i exp(power_i(v)) (0 where the power is > 0), as the field weighs a grid point;
+ *      c_i = max(0.5 + sum_k Y_k(-n_v) sh_ik, 0) per channel, the rasterizer's colour of Gaussian i seen from a camera
+ *      on v's outward normal (the 3DGS SH basis; n_v = 0 leaves the DC term only); rgb = clamp(sum w_i c_i / sum w_i,
+ *      0, 1), summed in list order in fp32 relative to the largest weight (so no weight underflows, however far v lies
+ *      from its Gaussians).  A vertex with sum w_i = 0 (an empty list, or every weight 0: a power > 0 or an opacity of
+ *      0) is white (1, 1, 1).
+ * out_rgb (device fp32 [V, 3]) receives the colours, out_normals (NULL or device fp32 [V, 3]) the normals and
+ * *num_unweighted (NULL or host) the number of white vertices.  No floating-point atomics: the result is the same bits
+ * on every run and does not depend on the vertex order.  alloc is called once for scratch (about 170 B per face plus
+ * 45 B per vertex and 8 B per block), then when P > 0 as dgs_mesh_field calls it for its lists; all of it is free after
+ * the call.  The stream is synchronised to check the indices, to read the pair count and to read the white count. */
+int dgs_mesh_vertex_colors(int P, const float* xyz, const float* features, int sh_degree, const float* scaling,
+                           const float* rotation, const float* opacity, float scale_modifier, const float* center,
+                           float scale, int resolution, int num_blocks, double relax_ratio, const float* lin,
+                           const float* vertices, long long num_vertices, const int* faces, long long num_faces,
+                           float* out_rgb, float* out_normals, long long* num_unweighted, dgs_alloc_fn alloc,
+                           void* alloc_user, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * B3. The elementwise callers either side of the path.

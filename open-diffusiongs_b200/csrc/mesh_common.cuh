@@ -88,16 +88,21 @@ struct MeshOut {
   }
 };
 
-// The checks every mesh entry point makes, in this order, before its own and before any CUDA call; size_ok is the
-// pass's own size limit, described by `limit`.
-inline int check_mesh_args(const char* name, const float* vertices, long long V, const int* faces, long long F,
-                           bool size_ok, const char* limit, const MeshOut& out) {
-  DGS_REQUIRE(out.alloc && out.vertices && out.faces && out.num_vertices && out.num_faces,
-              "%s: alloc and the four outputs must not be NULL", name);
+// The checks of an input mesh, in this order; size_ok is the pass's own size limit, described by `limit`.
+inline int check_mesh_input(const char* name, const float* vertices, long long V, const int* faces, long long F,
+                            bool size_ok, const char* limit) {
   DGS_REQUIRE(V >= 0 && F >= 0, "%s: negative size (%lld vertices, %lld faces)", name, V, F);
   DGS_REQUIRE(size_ok, "%s: %lld vertices / %lld faces is too many (%s)", name, V, F, limit);
   DGS_REQUIRE((V == 0 || vertices) && (F == 0 || faces), "%s: vertices and faces must not be NULL", name);
   return DGS_OK;
+}
+
+// The checks every mesh entry point that returns a mesh makes, in this order, before its own and before any CUDA call.
+inline int check_mesh_args(const char* name, const float* vertices, long long V, const int* faces, long long F,
+                           bool size_ok, const char* limit, const MeshOut& out) {
+  DGS_REQUIRE(out.alloc && out.vertices && out.faces && out.num_vertices && out.num_faces,
+              "%s: alloc and the four outputs must not be NULL", name);
+  return check_mesh_input(name, vertices, V, faces, F, size_ok, limit);
 }
 
 // -------------------------------------------------------------------------------------------------------- face check

@@ -1,15 +1,17 @@
 """Mesh extraction on libdgs_b200.so (dgs_mesh_field / dgs_marching_cubes / dgs_mesh_clean / dgs_mesh_remesh /
-dgs_mesh_decimate): the layer under `GaussianModel.extract_fields` / `extract_mesh`, and a command line that meshes a
-saved Gaussian PLY.
+dgs_mesh_decimate / dgs_mesh_vertex_colors): the layer under `GaussianModel.extract_fields` / `extract_mesh`, and a
+command line that meshes a saved Gaussian PLY.
 
     python -m dgs_b200.mesh in.ply out.obj [--resolution 256] [--density-thresh 0.005] [--clean] [--remesh [LEN]]
-                                           [--decimate-target N]
+                                           [--decimate-target N] [--colors]
 
 reads a PLY written by `GaussianModel.save_ply` (or the reference's), extracts the mesh exactly as
 `extract_mesh(density_thresh, resolution)` does and writes it as OBJ or binary PLY, chosen by the suffix; with `--clean`
 the mesh is first cleaned (`clean`, dgs_mesh_clean), with `--remesh [LEN]` then remeshed to edges of about LEN (default
 0.015; `remesh`, dgs_mesh_remesh), and with `--decimate-target N` then decimated to at most N faces (`decimate`,
-dgs_mesh_decimate).
+dgs_mesh_decimate).  With `--colors` the final vertices get colours and normals from the Gaussians (`vertex_colors`,
+dgs_mesh_vertex_colors), written as PLY vertex properties or OBJ `v x y z r g b` / `vn` lines; the model is then loaded at
+the SH degree its `f_rest_*` properties give.
 
 Marching cubes produces the same vertex set as PyMCubes (one vertex per sign-changing grid edge, at the linear
 interpolation of the iso value); on the ambiguous cases the triangulation may differ (a face with two diagonally
@@ -266,33 +268,120 @@ def clean_remesh_then_decimate(vertices, faces, decimate_target):
     return _chain(vertices, faces, True, 0.015, decimate_target)
 
 
+def vertex_colors(xyz, features, scaling, rotation, opacity, vertices, faces, mesh_center, mesh_scale,
+                  scaling_modifier=None, resolution=256, num_blocks=64, relax_ratio=1.5, stats=None):
+    """Per-vertex colours and normals of a mesh extract_mesh returned, from the Gaussians of its field
+    (dgs_mesh_vertex_colors; the semantics are include/dgs_b200.h's) -> (rgb float32 [V, 3] in [0, 1], normals float32
+    [V, 3], unit or 0).  The Gaussians are the raw xyz [P, 3], features [P, (d + 1)^2, 3] (SH degree d in 0..3),
+    scaling [P, 3], rotation [P, 4] and opacity [P, 1]; mesh_center / mesh_scale, scaling_modifier, resolution,
+    num_blocks and relax_ratio are the field's (what extract_fields used and set).  Each vertex gets the weighted mean,
+    by the field's own weights over its block's Gaussians, of their colours seen from its outward normal; a vertex that
+    no Gaussian weighs is white.  Input and output types as `decimate` (the Gaussians may be numpy arrays or tensors on
+    any device); the result is the same bits on every run and does not depend on the vertex order.  `stats`, a dict,
+    receives "unweighted", the number of white vertices."""
+    is_numpy = _mesh_check("vertex_colors", vertices, faces)
+    if resolution % (2 / num_blocks) != 0:
+        raise ValueError(f"vertex_colors: resolution {resolution} is not a multiple of the block size 2 / {num_blocks}")
+    P = len(xyz)
+    # a model without Gaussians may hold features of no particular shape
+    fshape = tuple(features.shape) if P or len(features.shape) == 3 else (0, 1, 3)
+    if len(fshape) != 3 or fshape[0] != P or fshape[2] != 3 or fshape[1] not in (1, 4, 9, 16):
+        raise ValueError(f"vertex_colors: expected features [P, (d + 1)^2, 3] with d in 0..3 and P = {P}, got "
+                         f"{tuple(features.shape)}")
+    if torch.as_tensor(mesh_center).numel() != 3:
+        raise ValueError(f"vertex_colors: mesh_center must have 3 values (got {mesh_center!r})")
+    dev, v, f = _mesh_in("vertex_colors", is_numpy, vertices, faces)
+    xyz, features, scaling, rotation, opacity, center = (
+        f32(torch.as_tensor(t).to(dev)) for t in (xyz, features, scaling, rotation, opacity, mesh_center))
+    features = features.reshape(fshape)
+    sh_degree = int(round(fshape[1] ** 0.5)) - 1
+    V = len(v)
+    rgb = torch.empty(V, 3, dtype=torch.float32, device=dev)
+    normals = torch.empty(V, 3, dtype=torch.float32, device=dev)
+    unweighted = C.c_longlong(0)
+    smod = 1.0 if scaling_modifier is None else float(scaling_modifier)
+    alloc = Alloc(dev, _SCRATCH, (str(dev), "colors"), cached=3)  # the mesh scratch and the field's two lists
+    with torch.cuda.device(dev):
+        lin = torch.linspace(-1, 1, resolution).to(dev)
+        # the field's fp32 roundings of the Python floats (opacity_field)
+        check(_lib.lib().dgs_mesh_vertex_colors(P, xyz.data_ptr(), features.data_ptr(), sh_degree, scaling.data_ptr(),
+                                                rotation.data_ptr(), opacity.data_ptr(), float(np.float32(smod)),
+                                                center.data_ptr(), float(np.float32(mesh_scale)), int(resolution),
+                                                int(num_blocks), float(relax_ratio), lin.data_ptr(), v.data_ptr(), V,
+                                                f.data_ptr(), len(f), rgb.data_ptr(), normals.data_ptr(),
+                                                C.byref(unweighted), alloc.cb, None, stream(dev)))
+    if stats is not None:
+        stats["unweighted"] = unweighted.value
+    if is_numpy:
+        return rgb.cpu().numpy(), normals.cpu().numpy()
+    return rgb, normals
+
+
 class Mesh:
     """The triangle mesh extract_mesh returns: `vertices` float32 [V, 3] and `faces` int64 [F, 3] numpy arrays (the
-    attribute names of trimesh.Trimesh)."""
+    attribute names of trimesh.Trimesh), and optionally `vertex_colors` (float32 [V, 3] in [0, 1]) and
+    `vertex_normals` (float32 [V, 3]), as `vertex_colors` computes them."""
 
-    def __init__(self, vertices, faces):
+    def __init__(self, vertices, faces, vertex_colors=None, vertex_normals=None):
         self.vertices = np.ascontiguousarray(vertices, dtype=np.float32).reshape(-1, 3)
         self.faces = np.ascontiguousarray(faces, dtype=np.int64).reshape(-1, 3)
+        self.vertex_colors = self._per_vertex("vertex_colors", vertex_colors)
+        self.vertex_normals = self._per_vertex("vertex_normals", vertex_normals)
+
+    def _per_vertex(self, name, a):
+        if a is None:
+            return None
+        a = np.ascontiguousarray(a, dtype=np.float32)
+        if a.shape != self.vertices.shape:
+            raise ValueError(f"Mesh: {name} must be [{len(self.vertices)}, 3], got {a.shape}")
+        return a
 
     def export(self, path):
-        """Writes binary little-endian PLY (.ply) or Wavefront OBJ (.obj), by suffix.  -> path"""
+        """Writes binary little-endian PLY (.ply) or Wavefront OBJ (.obj), by suffix, with the colours and normals when
+        the mesh has them: PLY vertex properties `nx ny nz` (float) and `red green blue` (uchar, (c * 255) clipped to
+        [0, 255] and truncated, as GaussianModel.save_ply quantises), OBJ `v x y z r g b` lines (float colours), `vn`
+        lines and `f a//a b//b c//c` faces.  -> path"""
         ext = os.path.splitext(path)[1].lower()
         os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
         V, F = len(self.vertices), len(self.faces)
+        rgb, nrm = self.vertex_colors, self.vertex_normals
         if ext == ".ply":
+            props = [("x", "<f4"), ("y", "<f4"), ("z", "<f4")]
+            if nrm is not None:
+                props += [("nx", "<f4"), ("ny", "<f4"), ("nz", "<f4")]
+            if rgb is not None:
+                props += [("red", "u1"), ("green", "u1"), ("blue", "u1")]
+            ply_type = {"<f4": "float", "u1": "uchar"}
             header = ("ply\nformat binary_little_endian 1.0\n"
-                      f"element vertex {V}\nproperty float x\nproperty float y\nproperty float z\n"
+                      f"element vertex {V}\n" + "".join(f"property {ply_type[t]} {n}\n" for n, t in props) +
                       f"element face {F}\nproperty list uchar int vertex_indices\nend_header\n")
+            vert = np.empty(V, dtype=props)
+            for k, n in enumerate("xyz"):
+                vert[n] = self.vertices[:, k]
+            if nrm is not None:
+                for k, n in enumerate(("nx", "ny", "nz")):
+                    vert[n] = nrm[:, k]
+            if rgb is not None:
+                q = (rgb * 255.0).clip(0.0, 255.0).astype(np.uint8)
+                for k, n in enumerate(("red", "green", "blue")):
+                    vert[n] = q[:, k]
             face = np.empty(F, dtype=[("n", "u1"), ("v", "<i4", (3,))])
             face["n"], face["v"] = 3, self.faces
             with open(path, "wb") as fh:
                 fh.write(header.encode("ascii"))
-                fh.write(self.vertices.astype("<f4").tobytes())
+                fh.write(vert.tobytes())
                 fh.write(face.tobytes())
         elif ext == ".obj":
             with open(path, "w") as fh:
-                np.savetxt(fh, self.vertices, fmt="v %.9g %.9g %.9g")
-                np.savetxt(fh, self.faces + 1, fmt="f %d %d %d")
+                if rgb is None:
+                    np.savetxt(fh, self.vertices, fmt="v %.9g %.9g %.9g")
+                else:
+                    np.savetxt(fh, np.concatenate([self.vertices, rgb], 1), fmt="v %.9g %.9g %.9g %.9g %.9g %.9g")
+                if nrm is None:
+                    np.savetxt(fh, self.faces + 1, fmt="f %d %d %d")
+                else:
+                    np.savetxt(fh, nrm, fmt="vn %.9g %.9g %.9g")
+                    np.savetxt(fh, np.repeat(self.faces + 1, 2, axis=1), fmt="f %d//%d %d//%d %d//%d")
         else:
             raise ValueError(f"Mesh.export: unsupported suffix {ext!r} (use .ply or .obj)")
         return path
@@ -322,7 +411,20 @@ def parser():
                          "non-manifold parts), as the reference's clean_mesh without remeshing")
     ap.add_argument("--remesh", type=float, nargs="?", const=0.015, default=None, metavar="LEN",
                     help="remesh isotropically to edges of about LEN (default 0.015), after --clean when both are given")
+    ap.add_argument("--colors", action="store_true",
+                    help="colour the final vertices from the Gaussians (at the SH degree of the file's f_rest_* "
+                         "properties) and write the colours and vertex normals")
     return ap
+
+
+def ply_sh_degree(path):
+    """The SH degree of a Gaussian PLY from its number of f_rest_* properties (0, 9, 24 or 45)"""
+    from .renderer import _read_ply_vertices
+    n = sum(k.startswith("f_rest_") for k in _read_ply_vertices(path).dtype.names)
+    degrees = {0: 0, 9: 1, 24: 2, 45: 3}
+    if n not in degrees:
+        raise ValueError(f"{path}: {n} f_rest_* properties is no SH degree of 0 to 3 (expected 0, 9, 24 or 45)")
+    return degrees[n]
 
 
 def _postprocess(args):
@@ -342,10 +444,10 @@ def _postprocess(args):
 def main(argv=None):
     args = parser().parse_args(argv)
     from .renderer import GaussianModel
-    gm = GaussianModel(0)
+    gm = GaussianModel(ply_sh_degree(args.ply) if args.colors else 0)
     gm.load_ply(args.ply)
     mesh = gm.to("cuda").extract_mesh(density_thresh=args.density_thresh, resolution=args.resolution,
-                                      **_postprocess(args))
+                                      vertex_colors=args.colors, **_postprocess(args))
     mesh.export(args.out)
     print(f"{args.out}: {len(mesh.vertices)} vertices, {len(mesh.faces)} faces")
 

@@ -272,7 +272,8 @@ class GaussianModel:
             relax_ratio)
         return occ
 
-    def extract_mesh(self, density_thresh=0.005, resolution=256, decimate_target=1e5, postprocess=None):
+    def extract_mesh(self, density_thresh=0.005, resolution=256, decimate_target=1e5, postprocess=None,
+                     vertex_colors=False):
         """gs_core.py:855-869: extract_fields(resolution, num_blocks=64), marching cubes at density_thresh on the GPU,
         vertices mapped by v / (resolution - 1) * 2 - 1 (in the normalised frame: not mapped back by mesh_center /
         mesh_scale, as in the reference) -> dgs_b200.mesh.Mesh (vertices float32 [V, 3], faces int64 [F, 3]).
@@ -280,10 +281,18 @@ class GaussianModel:
         mesh is returned and `decimate_target` is unused.  `postprocess(vertices, faces, decimate_target) -> (vertices,
         faces)` runs on the numpy arrays: `dgs_b200.mesh.clean_remesh_then_decimate` is the reference's whole chain
         (clean, isotropic remeshing to edges of 0.015, then decimate to decimate_target faces),
-        `dgs_b200.mesh.clean_then_decimate` the chain without its remeshing, `dgs_b200.mesh.decimate` decimates only."""
+        `dgs_b200.mesh.clean_then_decimate` the chain without its remeshing, `dgs_b200.mesh.decimate` decimates only.
+        With `vertex_colors`, the final vertices (after `postprocess`) also get `Mesh.vertex_colors` and
+        `Mesh.vertex_normals` from the model's Gaussians and SH features on the field's grid
+        (`dgs_b200.mesh.vertex_colors`); the geometry is the same as without."""
         from . import mesh as _mesh
         occ = self.extract_fields(resolution, num_blocks=64)
-        return _mesh.extract_mesh(occ, density_thresh, resolution, postprocess, decimate_target)
+        mesh = _mesh.extract_mesh(occ, density_thresh, resolution, postprocess, decimate_target)
+        if vertex_colors:
+            mesh.vertex_colors, mesh.vertex_normals = _mesh.vertex_colors(
+                self._xyz, self.get_features, self._scaling, self._rotation, self._opacity, mesh.vertices, mesh.faces,
+                self.mesh_center, self.mesh_scale, self.scaling_modifier, resolution, 64)
+        return mesh
 
 
 def _covariance6(stds, r):
