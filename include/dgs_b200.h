@@ -787,6 +787,43 @@ int dgs_mesh_vertex_colors(int P, const float* xyz, const float* features, int s
                            const float* vertices, long long num_vertices, const int* faces, long long num_faces,
                            float* out_rgb, float* out_normals, long long* num_unweighted, dgs_alloc_fn alloc,
                            void* alloc_user, void* stream);
+/* Depth-tested rasterization of a triangle mesh from n_views cameras, forward only (dgs_b200.mesh_render; the serial
+ * specification, operation for operation, is oracle/mesh_render.py).  vertices device fp32 [V, 3], faces device int32
+ * [F, 3] (every index in [0, V); checked on the device, a bad face is DGS_ERR_INVALID_ARGUMENT naming it), normals and
+ * colors NULL or device fp32 [V, 3], clip device fp32 [n_views, 4, 4] row-major world -> clip matrices; 1 <= H, W <=
+ * 8192, near > 0.  normal_bg and color_bg are NULL (zeros) or host fp32 [3].  Every output is NULL or device
+ * [n_views, H, W] (int32 face_id, fp32 depth and alpha) or [n_views, H, W, 3] (fp32 normal, rgb); a normal map needs
+ * normals and a colour map colours.  All fp32 arithmetic is rounded product by product, in the oracle's order:
+ *   1. setup per (view, face): each corner to (X, Y, w) = ((x_c + w_c) W / 2, (y_c + w_c) H / 2, w_c), so pixel (i, j)
+ *      has its centre at X / w = i + 0.5, Y / w = j + 0.5; Sutherland-Hodgman clipping against w >= near and a guard
+ *      band of 8192 pixels on each side (a crossing is computed from the inside end of its edge; a polygon that would
+ *      exceed 8 corners, which only rounding on a near-degenerate face can cause, is culled); the polygon snapped
+ *      to 1/256 pixel (rint), its orientation made positive; zero area or an empty pixel box culls it.  Back faces are
+ *      drawn.  The facing is the sign of det[(X, Y, w) of the three unclipped corners].
+ *   2. coverage: a pixel centre is covered when every non-degenerate edge function of the snapped polygon (int64) is
+ *      > 0, or = 0 on a top or left edge, so a centre on an edge shared by two faces is covered once.  A covered pixel
+ *      takes the perspective-correct barycentrics u of the unclipped face (homogeneous edge functions over their sum;
+ *      a zero sum covers nothing) and depth = u . w; the smallest (order-preserving depth bits << 32 | face) wins, so
+ *      exact depth ties go to the lower face.  Triangles whose pixel box fits 8 x 8 take one thread, larger ones one
+ *      thread per 8 x 8 tile of their box.
+ *   3. resolve: face_id (-1 for background), depth (clip w, 0 for background), normal = normalised u . n (0 for a zero
+ *      sum), rgb = u . c; background pixels take normal_bg and color_bg.
+ *   4. antialias (alpha, normal, rgb; not depth): for each 4-neighbour pair with different faces, the occluder is the
+ *      pixel with the smaller key (background is farthest).  Walking from its centre to the other's, take the first
+ *      edge of the occluder's face the segment leaves through, at distance t in pixels.  When that edge is a silhouette
+ *      edge (boundary, non-manifold, or its neighbour's facing differs in this view; neighbours from the mesh's
+ *      half-edge table) and it is steeper than 45 degrees for a horizontal pair or not for a vertical pair, then for
+ *      t > 1/2 the far pixel moves t - 1/2 of the way to the occluder's value, and for t < 1/2 the occluder's pixel
+ *      moves 1/2 - t of the way to the far pixel's.  Each pixel adds its contributions from the left, right, upper and
+ *      lower pair in this order; alpha is 1 on faces and 0 on background before it.
+ * No floating-point atomics: every output is the same bits on every run.  Views are rendered in chunks, as many as
+ * max_arena_bytes holds (at least one); alloc is called once for the scratch: about 110 B per face plus the half-edge
+ * sort's temporary storage, and per view of a chunk 9 B per face and 32 B per pixel.  The stream is synchronised to check the indices and once per chunk. */
+int dgs_mesh_render(const float* vertices, long long num_vertices, const int* faces, long long num_faces,
+                    const float* normals, const float* colors, const float* clip, int n_views, int H, int W,
+                    float near, const float* normal_bg, const float* color_bg, size_t max_arena_bytes,
+                    int* out_face_id, float* out_depth, float* out_alpha, float* out_normal, float* out_rgb,
+                    dgs_alloc_fn alloc, void* alloc_user, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * B3. The elementwise callers either side of the path.

@@ -232,6 +232,8 @@ def lib():
         L.dgs_mesh_vertex_colors.argtypes = [C.c_int, vp, vp, C.c_int, vp, vp, vp, C.c_float, vp, C.c_float, C.c_int,
                                              C.c_int, C.c_double, vp, vp, C.c_longlong, vp, C.c_longlong, vp, vp,
                                              C.POINTER(C.c_longlong), ALLOC_FN, vp, vp]
+        L.dgs_mesh_render.argtypes = [vp, C.c_longlong, vp, C.c_longlong, vp, vp, vp, C.c_int, C.c_int, C.c_int,
+                                      C.c_float, vp, vp, C.c_size_t] + [vp] * 5 + [ALLOC_FN, vp, vp]
         _lib = L
     return _lib
 
@@ -322,5 +324,5 @@ EXPORTED = [  # every symbol include/dgs_b200.h declares (checked by tests/test_
     "dgs_mesh_field", "dgs_marching_cubes",
     "dgs_dit_workspace_bytes_fp8_ex", "dgs_dit_forward_fp8_ex", "dgs_attention_quantize_e4m3", "dgs_attention_fwd_fp8",
     "dgs_mesh_decimate", "dgs_render_frames", "dgs_mesh_clean", "dgs_mesh_remesh",
-    "dgs_mesh_closest_points", "dgs_mesh_vertex_colors",
+    "dgs_mesh_closest_points", "dgs_mesh_vertex_colors", "dgs_mesh_render",
 ]
