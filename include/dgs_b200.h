@@ -787,6 +787,55 @@ int dgs_mesh_vertex_colors(int P, const float* xyz, const float* features, int s
                            const float* vertices, long long num_vertices, const int* faces, long long num_faces,
                            float* out_rgb, float* out_normals, long long* num_unweighted, dgs_alloc_fn alloc,
                            void* alloc_user, void* stream);
+/* Exact k-nearest neighbours (csrc/knn.cu): points device fp32 [P, 3] (finite; a non-finite coordinate is
+ * DGS_ERR_INVALID_ARGUMENT), 1 <= k <= 32, 0 <= P < 2^26.  out_idx (device int32 [P, k]) and out_d2 (device fp32
+ * [P, k]) receive, per point, its k nearest points of the cloud in (squared distance, index) order: the point itself
+ * counts (distance 0), as do duplicates; the squared distance is the fp32 (dx*dx + dy*dy) + dz*dz, rounded product by
+ * product; ties go to the smaller index; slots beyond P get index -1 and distance +inf.  A uniform grid sorted by cell
+ * and a ring search, no floating-point atomics: the same bits on every run.  alloc is called once for scratch (about
+ * 40 B per point plus 8 B per grid cell, at most 16 P + 64 cells); the stream is synchronised to read the bounding box
+ * and to size the grid. */
+int dgs_knn(const float* points, long long num_points, int k, int* out_idx, float* out_d2, dgs_alloc_fn alloc,
+            void* alloc_user, void* stream);
+/* What dgs_poisson_reconstruct reports: CG iterations, the final ||r|| / ||b||, the iso value, the inlier count, the
+ * marching-cubes vertex and face counts before the trim and the output's after it, and (filled whenever stats is
+ * given) the device time in ms of its stages: kNN, outliers + normals, grid + splat, solve, iso + marching cubes, trim. */
+typedef struct {
+  int iterations;
+  double residual;
+  double iso;
+  long long inliers;
+  long long vertices_before, faces_before, vertices, faces;
+  double stage_ms[6];
+} dgs_poisson_stats;
+/* Intermediate results of dgs_poisson_reconstruct, each copied when its pointer is not NULL (device memory):
+ * inliers uint8 [P] (1 = kept), normals fp32 [P, 3] (the first N rows: the inliers' normals as splatted), chi fp32
+ * [R^3] (the solution, x-major), density fp32 [density_capacity] (the first min(V, capacity) marching-cubes vertices'
+ * densities, before the trim). */
+typedef struct {
+  unsigned char* inliers;
+  float* normals;
+  float* chi;
+  float* density;
+  long long density_capacity;
+} dgs_poisson_trace;
+/* Screened Poisson surface reconstruction from points (device fp32 [P, 3]) and optional normals (NULL or device fp32
+ * [P, 3]): the reference's poisson_mesh_reconstruction (utils/mesh_utils.py:5-41) with Open3D replaced by the exact
+ * contract of csrc/poisson.cu's header (outlier removal over nb_neighbors in [1, 32] nearest points with std_ratio,
+ * given or PCA normals, splat onto 2^depth + 1 nodes per axis (depth in [4, 9]) over the inliers' bounding cube scaled
+ * by scale >= 1, the screened system with point_weight, multigrid-preconditioned CG to tol or max_iters, marching cubes
+ * at the mean of chi over the inliers, and the removal of the vertices below the density_quantile in [0, 1] (0: none)).
+ * nb_neighbors <= P < 2^26.  *out_vertices (fp32 [V, 3], in the input's frame) and *out_faces (int32 [F, 3], oriented
+ * outwards for outward normals) are allocated by alloc after all scratch, vertices first, each only when not empty.
+ * alloc is also called for scratch: about 100 B per point plus 50 B per grid node at depth d (R = 2^d + 1: 6.7 GB at
+ * depth 9), then dgs_knn's and dgs_marching_cubes's own.  Depth 10 is refused: its 1025^3 grid exceeds the size
+ * dgs_marching_cubes accepts.  stats and trace may be NULL.  No floating-point atomics: the
+ * same bits on every run.  The stream is synchronised at each data-dependent size and once per CG iteration. */
+int dgs_poisson_reconstruct(const float* points, long long num_points, const float* normals, int depth, int nb_neighbors,
+                            double std_ratio, double scale, double point_weight, double density_quantile, double tol,
+                            int max_iters, dgs_alloc_fn alloc, void* alloc_user, float** out_vertices, int** out_faces,
+                            long long* out_num_vertices, long long* out_num_faces, dgs_poisson_stats* stats,
+                            const dgs_poisson_trace* trace, void* stream);
 /* Depth-tested rasterization of a triangle mesh from n_views cameras, forward only (dgs_b200.mesh_render; the serial
  * specification, operation for operation, is oracle/mesh_render.py).  vertices device fp32 [V, 3], faces device int32
  * [F, 3] (every index in [0, V); checked on the device, a bad face is DGS_ERR_INVALID_ARGUMENT naming it), normals and

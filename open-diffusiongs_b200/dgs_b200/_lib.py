@@ -103,6 +103,17 @@ class DitOutGrads(C.Structure):  # dgs_dit_out_grads
                                           "d_img_aligned_xyz")]
 
 
+class PoissonStats(C.Structure):  # dgs_poisson_stats
+    _fields_ = [("iterations", C.c_int), ("residual", C.c_double), ("iso", C.c_double), ("inliers", C.c_longlong),
+                ("vertices_before", C.c_longlong), ("faces_before", C.c_longlong), ("vertices", C.c_longlong),
+                ("faces", C.c_longlong), ("stage_ms", C.c_double * 6)]
+
+
+class PoissonTrace(C.Structure):  # dgs_poisson_trace
+    _fields_ = [("inliers", C.c_void_p), ("normals", C.c_void_p), ("chi", C.c_void_p), ("density", C.c_void_p),
+                ("density_capacity", C.c_longlong)]
+
+
 _lib = None
 
 
@@ -234,6 +245,12 @@ def lib():
                                              C.POINTER(C.c_longlong), ALLOC_FN, vp, vp]
         L.dgs_mesh_render.argtypes = [vp, C.c_longlong, vp, C.c_longlong, vp, vp, vp, C.c_int, C.c_int, C.c_int,
                                       C.c_float, vp, vp, C.c_size_t] + [vp] * 5 + [ALLOC_FN, vp, vp]
+        L.dgs_knn.argtypes = [vp, C.c_longlong, C.c_int, vp, vp, ALLOC_FN, vp, vp]
+        L.dgs_poisson_reconstruct.argtypes = [vp, C.c_longlong, vp, C.c_int, C.c_int, C.c_double, C.c_double,
+                                              C.c_double, C.c_double, C.c_double, C.c_int, ALLOC_FN, vp,
+                                              C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_longlong),
+                                              C.POINTER(C.c_longlong), C.POINTER(PoissonStats),
+                                              C.POINTER(PoissonTrace), vp]
         _lib = L
     return _lib
 
@@ -324,5 +341,5 @@ EXPORTED = [  # every symbol include/dgs_b200.h declares (checked by tests/test_
     "dgs_mesh_field", "dgs_marching_cubes",
     "dgs_dit_workspace_bytes_fp8_ex", "dgs_dit_forward_fp8_ex", "dgs_attention_quantize_e4m3", "dgs_attention_fwd_fp8",
     "dgs_mesh_decimate", "dgs_render_frames", "dgs_mesh_clean", "dgs_mesh_remesh",
-    "dgs_mesh_closest_points", "dgs_mesh_vertex_colors", "dgs_mesh_render",
+    "dgs_mesh_closest_points", "dgs_mesh_vertex_colors", "dgs_mesh_render", "dgs_knn", "dgs_poisson_reconstruct",
 ]

@@ -3,7 +3,7 @@ dgs_mesh_decimate / dgs_mesh_vertex_colors): the layer under `GaussianModel.extr
 command line that meshes a saved Gaussian PLY.
 
     python -m dgs_b200.mesh in.ply out.obj [--resolution 256] [--density-thresh 0.005] [--clean] [--remesh [LEN]]
-                                           [--decimate-target N] [--colors]
+                                           [--decimate-target N] [--colors] [--poisson [DEPTH]]
 
 reads a PLY written by `GaussianModel.save_ply` (or the reference's), extracts the mesh exactly as
 `extract_mesh(density_thresh, resolution)` does and writes it as OBJ or binary PLY, chosen by the suffix; with `--clean`
@@ -11,7 +11,9 @@ the mesh is first cleaned (`clean`, dgs_mesh_clean), with `--remesh [LEN]` then 
 0.015; `remesh`, dgs_mesh_remesh), and with `--decimate-target N` then decimated to at most N faces (`decimate`,
 dgs_mesh_decimate).  With `--colors` the final vertices get colours and normals from the Gaussians (`vertex_colors`,
 dgs_mesh_vertex_colors), written as PLY vertex properties or OBJ `v x y z r g b` / `vn` lines; the model is then loaded at
-the SH degree its `f_rest_*` properties give.
+the SH degree its `f_rest_*` properties give.  With `--poisson [DEPTH]` the surface is reconstructed instead by screened
+Poisson (`poisson_reconstruction`, dgs_poisson_reconstruct) from the Gaussians' centres and shortest axes, as
+`extract_mesh(method="poisson", depth=DEPTH)` does; the flags above apply to it unchanged.
 
 Marching cubes produces the same vertex set as PyMCubes (one vertex per sign-changing grid edge, at the linear
 interpolation of the iso value); on the ambiguous cases the triangulation may differ (a face with two diagonally
@@ -31,6 +33,15 @@ from ._lib import Alloc, check, f32, stream
 _SCRATCH = {}  # grow-only scratch buffers, re-used across calls: {((device, name), i): uint8 tensor}
 
 
+def mesh_frame(xyz):
+    """The normalisation of extract_fields: (mesh_center fp32 [3], mesh_scale float) that map the centres xyz (fp32
+    [P, 3]) to about [-0.9, 0.9]^3 by (xyz - mesh_center) * mesh_scale; centre 0 and scale 1 without centres"""
+    if xyz.shape[0] == 0:
+        return torch.zeros(3, dtype=torch.float32, device=xyz.device), 1.0
+    mn, mx = xyz.amin(0), xyz.amax(0)
+    return (mn + mx) / 2, 1.8 / (mx - mn).amax().item()
+
+
 def opacity_field(xyz, scaling, rotation, opacity, scaling_modifier=None, resolution=128, num_blocks=16, relax_ratio=1.5,
                   return_counts=False):
     """GaussianModel.extract_fields on raw CUDA tensors -> (occ [R, R, R] fp32, mesh_center fp32 [3], mesh_scale float),
@@ -44,12 +55,7 @@ def opacity_field(xyz, scaling, rotation, opacity, scaling_modifier=None, resolu
     xyz, scaling, rotation, opacity = (f32(t) for t in (xyz, scaling, rotation, opacity))
     P = xyz.shape[0]
     with torch.cuda.device(dev):
-        if P > 0:
-            mn, mx = xyz.amin(0), xyz.amax(0)
-            center = (mn + mx) / 2
-            scale = 1.8 / (mx - mn).amax().item()
-        else:
-            center, scale = torch.zeros(3, dtype=torch.float32, device=dev), 1.0
+        center, scale = mesh_frame(xyz)
         lin = torch.linspace(-1, 1, resolution).to(dev)
         nc = -(-resolution // (resolution // num_blocks))
         occ = torch.empty([resolution] * 3, dtype=torch.float32, device=dev)
@@ -261,6 +267,142 @@ def closest_points(vertices, faces, queries):
     return pts, d2, fi.long()
 
 
+def _points_check(name, points, normals=None):
+    """Checks a point cloud argument (and its normals) -> whether it is numpy (else CUDA tensors)"""
+    is_numpy = isinstance(points, np.ndarray)
+    if not is_numpy and not (isinstance(points, torch.Tensor) and points.is_cuda):
+        raise TypeError(f"{name}: points must be a numpy array or a CUDA tensor")
+    if points.ndim != 2 or points.shape[1] != 3:
+        raise ValueError(f"{name}: expected points [P, 3], got {tuple(points.shape)}")
+    if normals is not None:
+        if is_numpy != isinstance(normals, np.ndarray) or (not is_numpy and not (
+                isinstance(normals, torch.Tensor) and normals.device == points.device)):
+            raise TypeError(f"{name}: points and normals must both be numpy arrays or CUDA tensors on one device")
+        if tuple(normals.shape) != tuple(points.shape):
+            raise ValueError(f"{name}: normals {tuple(normals.shape)} do not match points {tuple(points.shape)}")
+    if is_numpy:
+        for a, what in ((points, "points"), (normals, "normals")):
+            if a is not None and not np.isfinite(a).all():
+                raise ValueError(f"{name}: {what} have a non-finite coordinate")
+    return is_numpy
+
+
+def _points_in(is_numpy, a):
+    """A checked point array -> a contiguous fp32 CUDA tensor (numpy goes to the current CUDA device)"""
+    if is_numpy:
+        return torch.from_numpy(np.ascontiguousarray(a, np.float32)).to(torch.device("cuda", torch.cuda.current_device()))
+    return a.detach().to(torch.float32).contiguous()
+
+
+def knn(points, k):
+    """Exact k nearest neighbours of every point (dgs_knn) -> (idx int32 [P, k], d2 float32 [P, k]): in (squared
+    distance, index) order, the point itself included at distance 0, duplicates included; d2 is the fp32
+    (dx*dx + dy*dy) + dz*dz, ties go to the smaller index, and slots beyond P get index -1 and distance inf.  numpy
+    input (float [P, 3]) runs on the current CUDA device and returns numpy; CUDA tensors return CUDA tensors.  The result
+    is the same bits on every run."""
+    is_numpy = _points_check("knn", points)
+    if int(k) != k or not 1 <= k <= 32:
+        raise ValueError(f"knn: k must be an integer in [1, 32] (got {k!r})")
+    p = _points_in(is_numpy, points)
+    dev, P, k = p.device, len(p), int(k)
+    idx = torch.empty(P, k, dtype=torch.int32, device=dev)
+    d2 = torch.empty(P, k, dtype=torch.float32, device=dev)
+    alloc = Alloc(dev)
+    with torch.cuda.device(dev):
+        check(_lib.lib().dgs_knn(p.data_ptr(), P, k, idx.data_ptr(), d2.data_ptr(), alloc.cb, None, stream(dev)))
+    alloc.tensors.clear()  # the callback keeps the Alloc in a reference cycle: free the scratch now, not at collection
+    alloc.tensor = None
+    if is_numpy:
+        return idx.cpu().numpy(), d2.cpu().numpy()
+    return idx, d2
+
+
+POISSON_STAGES = ("knn", "outliers_normals", "splat", "solve", "marching_cubes", "trim")
+
+
+def poisson_reconstruction(points, normals=None, depth=9, nb_neighbors=20, std_ratio=10.0, scale=1.1, point_weight=4.0,
+                           density_quantile=0.1, tol=1e-6, max_iters=100, stats=None, trace=None):
+    """The reference's poisson_mesh_reconstruction (dgs_poisson_reconstruct; the exact contract is csrc/poisson.cu's
+    header) -> (vertices, faces): statistical outlier removal over nb_neighbors nearest points, the given normals or PCA
+    normals oriented away from the centroid, screened Poisson on 2^depth + 1 nodes per axis over the points' bounding
+    cube scaled by `scale`, marching cubes at the mean indicator value of the points, then the removal of the vertices
+    whose sample density is below the density_quantile (0: none) and of the faces that touch them.  The defaults are
+    the reference call's (depth 9, 20 neighbours, std_ratio 10, the 10 % quantile).  Faces are oriented outwards for
+    outward normals; the vertices are in the input's frame.  numpy input (points float [P, 3], normals None or float
+    [P, 3]) runs on the current CUDA device and returns numpy float32 [V, 3] / int64 [F, 3]; CUDA tensors return CUDA
+    tensors.  The result is the same bits on every run.  `stats`, a dict, receives "iterations", "residual" (the final
+    ||r|| / ||b||), "iso", "inliers", "vertices_before" / "faces_before" (before the trim), "vertices", "faces" and
+    "stage_ms" (device ms per stage of POISSON_STAGES); `trace`, a dict, receives the CUDA tensors "inliers" (bool [P]),
+    "normals" (float32 [inliers, 3]), "chi" (float32 [R, R, R]) and "density" (float32 [vertices_before])."""
+    name = "poisson_reconstruction"
+    is_numpy = _points_check(name, points, normals)
+    P = len(points)
+    if int(nb_neighbors) != nb_neighbors or not 1 <= nb_neighbors <= 32:
+        raise ValueError(f"{name}: nb_neighbors must be an integer in [1, 32] (got {nb_neighbors!r})")
+    if P < nb_neighbors:
+        raise ValueError(f"{name}: {P} points is fewer than nb_neighbors = {nb_neighbors}")
+    if int(depth) != depth or not 4 <= depth <= 9:
+        raise ValueError(f"{name}: depth must be an integer in [4, 9] (got {depth!r})")
+    if not (np.isfinite(scale) and scale >= 1):
+        raise ValueError(f"{name}: scale must be finite and >= 1 (got {scale!r})")
+    if not 0 <= density_quantile <= 1:
+        raise ValueError(f"{name}: density_quantile must be in [0, 1] (got {density_quantile!r})")
+    p = _points_in(is_numpy, points)
+    n = None if normals is None else _points_in(is_numpy, normals)
+    dev, R = p.device, 2 ** int(depth) + 1
+    st = _lib.PoissonStats()
+    tr, cap = None, 0
+    if trace is not None:
+        cap = 8 * R * R + 1024
+        tensors = dict(inliers=torch.empty(P, dtype=torch.uint8, device=dev),
+                       normals=torch.empty(P, 3, dtype=torch.float32, device=dev),
+                       chi=torch.empty(R, R, R, dtype=torch.float32, device=dev))
+    while True:
+        if trace is not None:
+            tensors["density"] = torch.empty(cap, dtype=torch.float32, device=dev)
+            tr = _lib.PoissonTrace(*(tensors[k].data_ptr() for k in ("inliers", "normals", "chi", "density")), cap)
+        alloc = Alloc(dev)  # no cache: the last two buffers are the caller's output
+        vp, fp = C.c_void_p(), C.c_void_p()
+        nv, nf = C.c_longlong(0), C.c_longlong(0)
+        with torch.cuda.device(dev):
+            check(_lib.lib().dgs_poisson_reconstruct(
+                p.data_ptr(), P, None if n is None else n.data_ptr(), int(depth), int(nb_neighbors), float(std_ratio),
+                float(scale), float(point_weight), float(density_quantile), float(tol), int(max_iters), alloc.cb, None,
+                C.byref(vp), C.byref(fp), C.byref(nv), C.byref(nf), C.byref(st), C.byref(tr) if tr is not None else None,
+                stream(dev)))
+        if trace is None or st.vertices_before <= cap:
+            break
+        alloc.tensors.clear()
+        alloc.tensor = None
+        cap = st.vertices_before  # the densities did not fit: once more, with room for all of them
+    if stats is not None:
+        stats.update({k: getattr(st, k) for k in ("iterations", "residual", "iso", "inliers", "vertices_before",
+                                                  "faces_before", "vertices", "faces")})
+        stats["stage_ms"] = dict(zip(POISSON_STAGES, st.stage_ms))
+    if trace is not None:
+        trace.update(inliers=tensors["inliers"].bool(), normals=tensors["normals"][:st.inliers], chi=tensors["chi"],
+                     density=tensors["density"][:st.vertices_before])
+    out = _mesh_out(is_numpy, dev, alloc, nv.value, nf.value)
+    alloc.tensors.clear()  # the scratch (GBs at depth 9) goes now; the outputs are views that keep their own buffers
+    alloc.tensor = None
+    return out
+
+
+def gaussian_points(xyz, scaling, rotation, mesh_center, mesh_scale):
+    """The oriented points extract_mesh(method="poisson") reconstructs from: the centres normalised by
+    (xyz - mesh_center) * mesh_scale (fp32), and each Gaussian's shortest axis (the rotation's column of the smallest
+    scaling; rotation [P, 4] as w, x, y, z, not normalised) turned to point away from the normalised origin."""
+    p = (f32(xyz) - mesh_center) * mesh_scale
+    q = torch.nn.functional.normalize(f32(rotation).double(), dim=1)
+    w, x, y, z = q.unbind(1)
+    cols = torch.stack([torch.stack([1 - 2 * (y * y + z * z), 2 * (x * y + w * z), 2 * (x * z - w * y)], 1),
+                        torch.stack([2 * (x * y - w * z), 1 - 2 * (x * x + z * z), 2 * (y * z + w * x)], 1),
+                        torch.stack([2 * (x * z + w * y), 2 * (y * z - w * x), 1 - 2 * (x * x + y * y)], 1)], 1)
+    n = cols[torch.arange(len(p), device=p.device), f32(scaling).argmin(1)]
+    n = torch.where(((n * p.double()).sum(1) < 0)[:, None], -n, n)
+    return p.contiguous(), n.float().contiguous()
+
+
 def clean_remesh_then_decimate(vertices, faces, decimate_target):
     """The reference's whole extract_mesh post-processing (gs_core.py:862-863): `clean` with its defaults, `remesh` to
     edges of 0.015 in 3 iterations, then `decimate` to decimate_target faces when more are left.  The signature of
@@ -411,6 +553,10 @@ def parser():
                          "non-manifold parts), as the reference's clean_mesh without remeshing")
     ap.add_argument("--remesh", type=float, nargs="?", const=0.015, default=None, metavar="LEN",
                     help="remesh isotropically to edges of about LEN (default 0.015), after --clean when both are given")
+    ap.add_argument("--poisson", type=int, nargs="?", const=9, default=None, metavar="DEPTH",
+                    help="reconstruct by screened Poisson from the Gaussians' centres and shortest axes at DEPTH "
+                         "(default 9) instead of marching the opacity field (--resolution and --density-thresh are then "
+                         "unused)")
     ap.add_argument("--colors", action="store_true",
                     help="colour the final vertices from the Gaussians (at the SH degree of the file's f_rest_* "
                          "properties) and write the colours and vertex normals")
@@ -446,8 +592,9 @@ def main(argv=None):
     from .renderer import GaussianModel
     gm = GaussianModel(ply_sh_degree(args.ply) if args.colors else 0)
     gm.load_ply(args.ply)
+    method = dict(method="field") if args.poisson is None else dict(method="poisson", depth=args.poisson)
     mesh = gm.to("cuda").extract_mesh(density_thresh=args.density_thresh, resolution=args.resolution,
-                                      vertex_colors=args.colors, **_postprocess(args))
+                                      vertex_colors=args.colors, **method, **_postprocess(args))
     mesh.export(args.out)
     print(f"{args.out}: {len(mesh.vertices)} vertices, {len(mesh.faces)} faces")
 

@@ -273,7 +273,7 @@ class GaussianModel:
         return occ
 
     def extract_mesh(self, density_thresh=0.005, resolution=256, decimate_target=1e5, postprocess=None,
-                     vertex_colors=False):
+                     vertex_colors=False, method="field", depth=9):
         """gs_core.py:855-869: extract_fields(resolution, num_blocks=64), marching cubes at density_thresh on the GPU,
         vertices mapped by v / (resolution - 1) * 2 - 1 (in the normalised frame: not mapped back by mesh_center /
         mesh_scale, as in the reference) -> dgs_b200.mesh.Mesh (vertices float32 [V, 3], faces int64 [F, 3]).
@@ -284,10 +284,26 @@ class GaussianModel:
         `dgs_b200.mesh.clean_then_decimate` the chain without its remeshing, `dgs_b200.mesh.decimate` decimates only.
         With `vertex_colors`, the final vertices (after `postprocess`) also get `Mesh.vertex_colors` and
         `Mesh.vertex_normals` from the model's Gaussians and SH features on the field's grid
-        (`dgs_b200.mesh.vertex_colors`); the geometry is the same as without."""
+        (`dgs_b200.mesh.vertex_colors`); the geometry is the same as without.
+        method="poisson" replaces the field and marching cubes by the reference's poisson_mesh_reconstruction
+        (`dgs_b200.mesh.poisson_reconstruction` with its defaults, at `depth`) of the centres normalised by mesh_center /
+        mesh_scale, as extract_fields sets them, with each Gaussian's shortest axis turned away from the origin as its
+        normal (`dgs_b200.mesh.gaussian_points`): a watertight surface in the same frame, less the vertices of its 10 %
+        lowest sample density, and density_thresh is unused.  `postprocess` and `vertex_colors` (still over the field's grid at `resolution`)
+        apply to it unchanged."""
         from . import mesh as _mesh
-        occ = self.extract_fields(resolution, num_blocks=64)
-        mesh = _mesh.extract_mesh(occ, density_thresh, resolution, postprocess, decimate_target)
+        if method == "field":
+            occ = self.extract_fields(resolution, num_blocks=64)
+            mesh = _mesh.extract_mesh(occ, density_thresh, resolution, postprocess, decimate_target)
+        elif method == "poisson":
+            self.mesh_center, self.mesh_scale = _mesh.mesh_frame(self._xyz.detach().float())
+            p, n = _mesh.gaussian_points(self._xyz, self._scaling, self._rotation, self.mesh_center, self.mesh_scale)
+            vertices, faces = (t.cpu().numpy() for t in _mesh.poisson_reconstruction(p, n, depth=depth))
+            if postprocess is not None:
+                vertices, faces = postprocess(vertices, faces, decimate_target)
+            mesh = _mesh.Mesh(vertices, faces)
+        else:
+            raise ValueError(f"extract_mesh: method must be 'field' or 'poisson' (got {method!r})")
         if vertex_colors:
             mesh.vertex_colors, mesh.vertex_normals = _mesh.vertex_colors(
                 self._xyz, self.get_features, self._scaling, self._rotation, self._opacity, mesh.vertices, mesh.faces,
