@@ -873,6 +873,32 @@ int dgs_mesh_render(const float* vertices, long long num_vertices, const int* fa
                     float near, const float* normal_bg, const float* color_bg, size_t max_arena_bytes,
                     int* out_face_id, float* out_depth, float* out_alpha, float* out_normal, float* out_rgb,
                     dgs_alloc_fn alloc, void* alloc_user, void* stream);
+/* TSDF fusion (csrc/tsdf.cu; the exact fp32 contract is its header, restated by oracle/tsdf.py).  The volume is four
+ * caller-owned device arrays over resolution^3 points (resolution R in [2, 512]) at lin (device fp32 [R], the grid
+ * linspace(-1, 1, R)), indexed [x][y][z]: tsdf_sum fp32 [R^3], weight int32 [R^3], rgb_sum fp32 [R^3, 3] and
+ * rgb_weight int32 [R^3], zeroed by the caller before the first view (24 B per point).
+ * dgs_tsdf_integrate fuses n_views >= 0 views, in order: c2w device fp32 [n, 4, 4] (OpenCV, row-major), fxfycxcy device
+ * fp32 [n, 4], and the rasterizer's maps of each view at H x W: image fp32 [n, 3, H, W] (on a white background),
+ * accumulated depth fp32 [n, H, W] and alpha fp32 [n, H, W].  trunc > 0 is the truncation distance and alpha_thresh in
+ * (0, 1] the alpha below which a pixel is background (carved).  alloc is called once, for 64 B per view.  One thread
+ * per point and no atomics: the same bits whatever the views' chunking. */
+int dgs_tsdf_integrate(int n_views, const float* c2w, const float* fxfycxcy, int H, int W, const float* image,
+                       const float* depth, const float* alpha, const float* lin, int resolution, float trunc,
+                       float alpha_thresh, float* tsdf_sum, int* weight, float* rgb_sum, int* rgb_weight,
+                       dgs_alloc_fn alloc, void* alloc_user, void* stream);
+/* Marching cubes of -(tsdf_sum / weight) at 0 over the observed points (weight > 0) only: a voxel emits triangles when
+ * its 8 corners are observed, an edge a vertex when both its ends are and a voxel containing it is.  Every vertex is
+ * referenced, no face touches an unobserved point, and faces are oriented outwards.  *out_vertices (fp32 [V, 3], index
+ * coordinates) and *out_faces (int32 [F, 3]) are allocated by alloc after the scratch (4 B per point, then
+ * dgs_marching_cubes's own), vertices first, each only when not empty.  The stream is synchronised once. */
+int dgs_tsdf_extract(const float* tsdf_sum, const int* weight, int resolution, dgs_alloc_fn alloc, void* alloc_user,
+                     float** out_vertices, int** out_faces, long long* out_num_vertices, long long* out_num_faces,
+                     void* stream);
+/* Vertex colours from the volume: vertices device fp32 [V, 3] in the grid's [-1, 1] frame -> out_rgb device fp32
+ * [V, 3] in [0, 1], the trilinear blend over the containing cell's corners that have rgb_weight > 0 (weights
+ * renormalised over them) of each corner's rgb_sum / rgb_weight; white where no corner is coloured. */
+int dgs_tsdf_colors(const float* rgb_sum, const int* rgb_weight, int resolution, const float* vertices,
+                    long long num_vertices, float* out_rgb, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * B3. The elementwise callers either side of the path.

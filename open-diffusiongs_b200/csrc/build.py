@@ -13,12 +13,13 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.abspath(os.path.join(HERE, "..", ".."))
 OUT_DIR = os.path.join(HERE, "..", "dgs_b200", "lib")
 OUT = os.path.abspath(os.path.join(OUT_DIR, "libdgs_b200.so"))
-SOURCES = ["core.cu", "raster.cu", "dit_glue.cu", "gemm_sm90.cu", "attention_sm90.cu", "attention_bwd_sm90.cu", "dit_api.cu", "diffusion_steps.cu", "lpips.cu", "ssim.cu", "geometry_loss.cu", "mesh.cu", "mesh_decimate.cu", "mesh_clean.cu", "mesh_remesh.cu", "mesh_color.cu", "mesh_render.cu", "knn.cu", "poisson.cu"]
+SOURCES = ["core.cu", "raster.cu", "dit_glue.cu", "gemm_sm90.cu", "attention_sm90.cu", "attention_bwd_sm90.cu", "dit_api.cu", "diffusion_steps.cu", "lpips.cu", "ssim.cu", "geometry_loss.cu", "mesh.cu", "mesh_decimate.cu", "mesh_clean.cu", "mesh_remesh.cu", "mesh_color.cu", "mesh_render.cu", "knn.cu", "poisson.cu", "tsdf.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-O3"]
 FILE_FLAGS = {  # their fp64 decisions round every product and sum, as their oracles do
     "mesh_clean.cu": ["-fmad=false"], "mesh_remesh.cu": ["-fmad=false"], "mesh_color.cu": ["-fmad=false"],
-    "mesh_render.cu": ["-fmad=false"], "knn.cu": ["-fmad=false"], "poisson.cu": ["-fmad=false"]}
+    "mesh_render.cu": ["-fmad=false"], "knn.cu": ["-fmad=false"], "poisson.cu": ["-fmad=false"],
+    "tsdf.cu": ["-fmad=false"]}
 
 
 def _stale(obj, deps):

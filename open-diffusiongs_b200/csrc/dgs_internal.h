@@ -80,6 +80,12 @@ struct Carver {
 
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
+// dgs_marching_cubes (mesh.cu) with its messages prefixed by `name`; with a weight array [nx, ny, nz] (else nullptr)
+// only the points of weight > 0 are observed, and the mesh keeps to the voxels whose 8 corners are (mesh.cu's header).
+int marching_cubes(const char* name, const float* field, const int* weight, int nx, int ny, int nz, float iso,
+                   dgs_alloc_fn alloc, void* alloc_user, float** vertices, int** triangles, long long* num_vertices,
+                   long long* num_triangles, cudaStream_t st);
+
 // Launch with programmatic dependent launch allowed (DGS_PDL=0 disables it).  ONLY for kernels that execute
 // griddepcontrol.wait before their first access to global memory written by earlier kernels.
 bool pdl_enabled();

@@ -7,6 +7,9 @@
 // Marching cubes: a classify pass over grid points (sign-changing edges owned by the point, case of the voxel it is
 // the origin of), in-place scans of the vertex and triangle counts, one read-back of the two totals, and an emit pass.
 // Vertex order is by owning edge (grid point, then axis), triangle order by voxel, then case-table order.
+// The masked instantiation (the TSDF extraction of tsdf.cu) keeps only what observed points support: a voxel emits
+// triangles only when its 8 corners are observed, and an edge a vertex only when both its ends are observed and a voxel
+// containing it is, so every vertex is referenced and no face touches an unobserved point.
 #include <cub/cub.cuh>
 
 #include "dgs_internal.h"
@@ -83,9 +86,21 @@ __global__ void __launch_bounds__(32 * kEvalWarps) field_eval_kernel(Grid grid, 
 }
 
 // ---------------------------------------------------------------------------------------------------- marching cubes
+// Bit (dx + 1) + 3 (dy + 1) + 9 (dz + 1) of the 27-bit neighbourhood mask; whether all 8 corners of the voxel whose
+// origin is offset (ox, oy, oz) in {-1, 0}^3 from the centre are set.
+__device__ __forceinline__ int nb_bit(int dx, int dy, int dz) { return (dx + 1) + 3 * (dy + 1) + 9 * (dz + 1); }
+__device__ __forceinline__ bool voxel_full(uint32_t nb, int ox, int oy, int oz) {
+#pragma unroll
+  for (int c = 0; c < 8; c++)
+    if (!((nb >> nb_bit(ox + (c & 1), oy + ((c >> 1) & 1), oz + (c >> 2))) & 1)) return false;
+  return true;
+}
+
+// kMasked: only points with weight > 0 are observed (the rules in the header); weight is unused otherwise.
+template <bool kMasked>
 __global__ void mc_classify_kernel(const float* __restrict__ f, int nx, int ny, int nz, float iso,
                                    uint8_t* __restrict__ ecode, uint8_t* __restrict__ cases, uint32_t* __restrict__ vscan,
-                                   uint32_t* __restrict__ tscan) {
+                                   uint32_t* __restrict__ tscan, const int* __restrict__ weight) {
   const long long N = (long long)nx * ny * nz;
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
@@ -102,6 +117,28 @@ __global__ void mc_classify_kernel(const float* __restrict__ f, int nx, int ny, 
     for (int c = 0; c < 8; c++)
       if (f[i + (c & 1) * sx + ((c >> 1) & 1) * sy + (c >> 2)] > iso) cs |= 1u << c;
     nt = kMcNumTris[cs];
+  }
+  if constexpr (kMasked) {
+    uint32_t nb = 0;  // observed points of the 3 x 3 x 3 neighbourhood; points outside the grid are not observed
+    for (int dz = -1; dz <= 1; dz++)
+      for (int dy = -1; dy <= 1; dy++)
+        for (int dx = -1; dx <= 1; dx++) {
+          const int qx = x + dx, qy = y + dy, qz = z + dz;
+          if (qx >= 0 && qx < nx && qy >= 0 && qy < ny && qz >= 0 && qz < nz && weight[i + dx * sx + dy * sy + dz] > 0)
+            nb |= 1u << nb_bit(dx, dy, dz);
+        }
+    // an edge along axis a lies in the 4 voxels with origin offset 0 along a and -1 or 0 along the other two axes
+    const bool fx = voxel_full(nb, 0, -1, -1) || voxel_full(nb, 0, 0, -1) || voxel_full(nb, 0, -1, 0) ||
+                    voxel_full(nb, 0, 0, 0);
+    const bool fy = voxel_full(nb, -1, 0, -1) || voxel_full(nb, 0, 0, -1) || voxel_full(nb, -1, 0, 0) ||
+                    voxel_full(nb, 0, 0, 0);
+    const bool fz = voxel_full(nb, -1, -1, 0) || voxel_full(nb, 0, -1, 0) || voxel_full(nb, -1, 0, 0) ||
+                    voxel_full(nb, 0, 0, 0);
+    const bool here = (nb >> nb_bit(0, 0, 0)) & 1;
+    if (!(here && ((nb >> nb_bit(1, 0, 0)) & 1) && fx)) e &= ~1u;
+    if (!(here && ((nb >> nb_bit(0, 1, 0)) & 1) && fy)) e &= ~2u;
+    if (!(here && ((nb >> nb_bit(0, 0, 1)) & 1) && fz)) e &= ~4u;
+    if (!voxel_full(nb, 0, 0, 0)) cs = nt = 0;
   }
   ecode[i] = (uint8_t)e;
   cases[i] = (uint8_t)cs;
@@ -193,17 +230,27 @@ int dgs_mesh_field(int P, const float* xyz, const float* scaling, const float* r
 int dgs_marching_cubes(const float* field, int nx, int ny, int nz, float iso, dgs_alloc_fn alloc, void* alloc_user,
                        float** vertices, int** triangles, long long* num_vertices, long long* num_triangles,
                        void* stream) {
+  return marching_cubes("marching cubes", field, nullptr, nx, ny, nz, iso, alloc, alloc_user, vertices, triangles,
+                        num_vertices, num_triangles, reinterpret_cast<cudaStream_t>(stream));
+}
+
+}  // extern "C"
+
+namespace dgs {
+
+int marching_cubes(const char* name, const float* field, const int* weight, int nx, int ny, int nz, float iso,
+                   dgs_alloc_fn alloc, void* alloc_user, float** vertices, int** triangles, long long* num_vertices,
+                   long long* num_triangles, cudaStream_t st) {
   DGS_REQUIRE(field && alloc && vertices && triangles && num_vertices && num_triangles,
-              "marching cubes: field, alloc and the four outputs must not be NULL");
-  DGS_REQUIRE(nx >= 2 && ny >= 2 && nz >= 2, "marching cubes: the field must be at least 2 x 2 x 2 (got %d x %d x %d)",
+              "%s: field, alloc and the four outputs must not be NULL", name);
+  DGS_REQUIRE(nx >= 2 && ny >= 2 && nz >= 2, "%s: the field must be at least 2 x 2 x 2 (got %d x %d x %d)", name,
               nx, ny, nz);
   const long long N = (long long)nx * ny * nz;
-  DGS_REQUIRE(N * DGS_MC_MAX_TRIS <= 0x7fffffffLL, "marching cubes: %d x %d x %d grid points is too many (at most %lld)",
+  DGS_REQUIRE(N * DGS_MC_MAX_TRIS <= 0x7fffffffLL, "%s: %d x %d x %d grid points is too many (at most %lld)", name,
               nx, ny, nz, 0x7fffffffLL / DGS_MC_MAX_TRIS);
   *vertices = nullptr;
   *triangles = nullptr;
   *num_vertices = *num_triangles = 0;
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   size_t temp_bytes = 0;
   uint32_t* nul = nullptr;
   DGS_CUDA_OK(cub::DeviceScan::InclusiveSum(nullptr, temp_bytes, nul, nul, (int)N));
@@ -220,10 +267,13 @@ int dgs_marching_cubes(const float* field, int nx, int ny, int nz, float iso, dg
   uint32_t *vscan, *tscan;
   void* temp;
   void* buf = alloc(carve(nullptr, &ecode, &cases, &vscan, &tscan, &temp), alloc_user);
-  if (!buf) { set_error("marching cubes: scratch allocation failed"); return DGS_ERR_ALLOC; }
+  if (!buf) { set_error("%s: scratch allocation failed", name); return DGS_ERR_ALLOC; }
   carve(buf, &ecode, &cases, &vscan, &tscan, &temp);
   const unsigned grid = (unsigned)((N + 255) / 256);
-  mc_classify_kernel<<<grid, 256, 0, st>>>(field, nx, ny, nz, iso, ecode, cases, vscan, tscan);
+  if (weight)
+    mc_classify_kernel<true><<<grid, 256, 0, st>>>(field, nx, ny, nz, iso, ecode, cases, vscan, tscan, weight);
+  else
+    mc_classify_kernel<false><<<grid, 256, 0, st>>>(field, nx, ny, nz, iso, ecode, cases, vscan, tscan, nullptr);
   DGS_POST_LAUNCH();
   DGS_CUDA_OK(cub::DeviceScan::InclusiveSum(temp, temp_bytes, vscan, vscan, (int)N, st));
   DGS_CUDA_OK(cub::DeviceScan::InclusiveSum(temp, temp_bytes, tscan, tscan, (int)N, st));
@@ -234,7 +284,7 @@ int dgs_marching_cubes(const float* field, int nx, int ny, int nz, float iso, dg
   if (tot[0] == 0) return DGS_OK;          // no sign change: no vertex and no triangle
   float* v = reinterpret_cast<float*>(alloc((size_t)tot[0] * 3 * sizeof(float), alloc_user));
   int* t = tot[1] ? reinterpret_cast<int*>(alloc((size_t)tot[1] * 3 * sizeof(int), alloc_user)) : nullptr;
-  if (!v || (tot[1] && !t)) { set_error("marching cubes: output allocation failed"); return DGS_ERR_ALLOC; }
+  if (!v || (tot[1] && !t)) { set_error("%s: output allocation failed", name); return DGS_ERR_ALLOC; }
   mc_emit_kernel<<<grid, 256, 0, st>>>(field, nx, ny, nz, iso, ecode, cases, vscan, tscan, v, t);
   DGS_POST_LAUNCH();
   *vertices = v;
@@ -244,4 +294,4 @@ int dgs_marching_cubes(const float* field, int nx, int ny, int nz, float iso, dg
   return DGS_OK;
 }
 
-}  // extern "C"
+}  // namespace dgs

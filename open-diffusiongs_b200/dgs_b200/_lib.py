@@ -251,6 +251,11 @@ def lib():
                                               C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_longlong),
                                               C.POINTER(C.c_longlong), C.POINTER(PoissonStats),
                                               C.POINTER(PoissonTrace), vp]
+        L.dgs_tsdf_integrate.argtypes = [C.c_int, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int, C.c_float,
+                                         C.c_float, vp, vp, vp, vp, ALLOC_FN, vp, vp]
+        L.dgs_tsdf_extract.argtypes = [vp, vp, C.c_int, ALLOC_FN, vp, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                       C.POINTER(C.c_longlong), C.POINTER(C.c_longlong), vp]
+        L.dgs_tsdf_colors.argtypes = [vp, vp, C.c_int, vp, C.c_longlong, vp, vp]
         _lib = L
     return _lib
 
@@ -342,4 +347,5 @@ EXPORTED = [  # every symbol include/dgs_b200.h declares (checked by tests/test_
     "dgs_dit_workspace_bytes_fp8_ex", "dgs_dit_forward_fp8_ex", "dgs_attention_quantize_e4m3", "dgs_attention_fwd_fp8",
     "dgs_mesh_decimate", "dgs_render_frames", "dgs_mesh_clean", "dgs_mesh_remesh",
     "dgs_mesh_closest_points", "dgs_mesh_vertex_colors", "dgs_mesh_render", "dgs_knn", "dgs_poisson_reconstruct",
+    "dgs_tsdf_integrate", "dgs_tsdf_extract", "dgs_tsdf_colors",
 ]

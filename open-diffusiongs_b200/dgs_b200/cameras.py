@@ -37,6 +37,30 @@ def get_turntable_cameras(hfov=50, num_views=8, w=384, h=384, radius=2.7, elevat
     return w, h, num_views, fxfycxcy, c2ws
 
 
+def sphere_cameras(num_views=100, image_size=512):
+    """-> (fxfycxcy fp64 [n, 4], c2ws fp64 [n, 4, 4]): OpenCV-convention cameras (as get_turntable_cameras) on the
+    sphere of radius 4, each looking at the origin.  View k looks from the Fibonacci-sphere direction with
+    z = 1 - (2k + 1) / n at azimuth k * pi * (3 - sqrt(5)), with +z up (+y where the direction is within 0.99 of +-z).
+    The images are square, image_size pixels wide, with the half-angle asin(sqrt(3) / 4): the sphere around the cube
+    [-1, 1]^3 just fits in every view."""
+    n, s = int(num_views), float(image_size)
+    fx = s / (2 * math.tan(math.asin(math.sqrt(3.0) / 4)))
+    fxfycxcy = np.array([fx, fx, s / 2.0, s / 2.0]).reshape(1, 4).repeat(n, axis=0)
+    c2ws = np.zeros((n, 4, 4))
+    for k in range(n):
+        z = 1 - (2 * k + 1) / n
+        ring, az = math.sqrt(max(0.0, 1 - z * z)), k * math.pi * (3 - math.sqrt(5))
+        d = np.array([ring * math.cos(az), ring * math.sin(az), z])
+        fwd = -d
+        right = np.cross(fwd, (0.0, 1.0, 0.0) if abs(z) > 0.99 else (0.0, 0.0, 1.0))
+        right = right / np.linalg.norm(right)
+        up = np.cross(right, fwd)
+        up = up / np.linalg.norm(up)
+        c2ws[k] = np.eye(4)
+        c2ws[k, :3, 0], c2ws[k, :3, 1], c2ws[k, :3, 2], c2ws[k, :3, 3] = right, -up, fwd, 4 * d
+    return fxfycxcy, c2ws
+
+
 def _unit(q):
     q = np.array(q, dtype=np.float64)
     return q / math.sqrt(np.dot(q, q))

@@ -290,7 +290,13 @@ class GaussianModel:
         mesh_scale, as extract_fields sets them, with each Gaussian's shortest axis turned away from the origin as its
         normal (`dgs_b200.mesh.gaussian_points`): a watertight surface in the same frame, less the vertices of its 10 %
         lowest sample density, and density_thresh is unused.  `postprocess` and `vertex_colors` (still over the field's grid at `resolution`)
-        apply to it unchanged."""
+        apply to it unchanged.
+        method="tsdf" fuses the model's own depth, alpha and colour renders from 100 `sphere_cameras` views at 512 x 512
+        into a truncated signed distance volume at `resolution` points per axis (`dgs_b200.mesh.tsdf_fusion`, in the
+        frame of mesh_center / mesh_scale, which it sets) and marches its zero crossing where it was observed
+        (`dgs_b200.mesh.tsdf_mesh`); density_thresh is unused and `postprocess` applies unchanged.  With
+        `vertex_colors` the final vertices are coloured from the fused renders (`dgs_b200.mesh.tsdf_colors`) and get
+        the fp64 normals of `dgs_b200.mesh_render.unit_vertex_normals`."""
         from . import mesh as _mesh
         if method == "field":
             occ = self.extract_fields(resolution, num_blocks=64)
@@ -302,8 +308,21 @@ class GaussianModel:
             if postprocess is not None:
                 vertices, faces = postprocess(vertices, faces, decimate_target)
             mesh = _mesh.Mesh(vertices, faces)
+        elif method == "tsdf":
+            volume = _mesh.tsdf_fusion(self._xyz, self.get_features, self._scaling, self._rotation, self._opacity,
+                                       self.scaling_modifier, resolution=resolution)
+            self.mesh_center, self.mesh_scale = volume["mesh_center"], volume["mesh_scale"]
+            vertices, faces = (t.cpu().numpy() for t in _mesh.tsdf_mesh(volume))
+            if postprocess is not None:
+                vertices, faces = postprocess(vertices, faces, decimate_target)
+            mesh = _mesh.Mesh(vertices, faces)
+            if vertex_colors:
+                from .mesh_render import unit_vertex_normals
+                mesh.vertex_colors = _mesh.tsdf_colors(volume, mesh.vertices)
+                mesh.vertex_normals = unit_vertex_normals(mesh.vertices, mesh.faces).cpu().numpy()
+            return mesh
         else:
-            raise ValueError(f"extract_mesh: method must be 'field' or 'poisson' (got {method!r})")
+            raise ValueError(f"extract_mesh: method must be 'field', 'poisson' or 'tsdf' (got {method!r})")
         if vertex_colors:
             mesh.vertex_colors, mesh.vertex_normals = _mesh.vertex_colors(
                 self._xyz, self.get_features, self._scaling, self._rotation, self._opacity, mesh.vertices, mesh.faces,
